@@ -1,11 +1,12 @@
-"""bench.py — tokens/s of the Llama-3-8B bf16 pre-training step (BASELINE.json configs[1] / configs[2]).
+"""bench.py — tokens/s of a Llama-3 bf16 pre-training step on H100 80 GB (Llama-3.2-3B shapes; BASELINE.json configs[1] / configs[2]
+used Llama-3-8B, whose full-parameter AdamW state alone is 128 GB).
 
     python bench.py [--gpus N --steps K --warmup W]                 # N = 1 (default) runs in-process
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W                      # one rank per GPU, NCCL
     python bench.py --impl reference ...                            # the reference's math on the host CPU (oracle port)
 
-One "step" = one optimizer step over per-GPU batch 8 x seq 4096 synthetic tokens (4 micro-batches of 2 sequences with
+One "step" = one optimizer step over per-GPU batch 8 x seq 4096 synthetic tokens (8 micro-batches of 1 sequence with
 gradient accumulation into the flat gradient buffer — the Trainer's gradient_accumulation_steps semantics,
 trainer.py:1045-1091), including the data-parallel gradient all-reduce and the AdamW update; nothing is skipped.
 Every step sees a FRESH random batch (drawn on the CPU from one seeded generator before the timed region).
@@ -14,7 +15,7 @@ Trainer-facing API (model(input_ids, labels) -> loss.backward() -> optimizer.ste
 copies and a D2H read of the loss inside the timed region.
 
 The same line also carries BASELINE.json configs[3] and configs[4] under `other_configs` (skip with --only-pretrain):
-  sft     Qwen2-7B full-parameter SFT, seq 2048, through Trainer.train() (pure data parallel over the launched ranks)
+  sft     Qwen2-1.5B full-parameter SFT, seq 2048, through Trainer.train() (pure data parallel over the launched ranks)
   decode  Llama-3-8B generation, batch 64, prompt 128 -> +1920, FusedMultiTransformer KV-cache path (rank 0, N=1 only:
           the decode path does not shard — replicas only)
 and `breakdown`: the in-step device time of every kernel family (CUDA events around each C-ABI call during one extra
@@ -37,34 +38,7 @@ sys.path.insert(0, ROOT)
 
 SEQ = 4096
 PER_GPU_BATCH = 8
-METRIC = "tokens/sec Llama-3-8B seq4096 bf16 pretrain step (global, all GPUs)"
-
-
-def gemm_traffic_from_profile(per_shape=None):
-    """DRAM bytes per GEMM launch (dram__bytes_read.sum + dram__bytes_write.sum) from the committed ncu capture of every GEMM
-    shape of the step (profiles/r02_gemm_traffic.json, written by tools/gemm_shapes.py --summarise: cold L2, one launch per
-    shape).  Returns (mean bytes per launch weighted by this run's launch counts, mean algorithmic bytes, per-shape table) or
-    (None, None, None) if the profile is absent."""
-    path = os.path.join(ROOT, "profiles", "r02_gemm_traffic.json")
-    try:
-        shapes = json.load(open(path))["shapes"]
-    except Exception:
-        return None, None, None
-    table = {(s["M"], s["N"], s["K"]): s for s in shapes}
-    if not per_shape:
-        n = len(shapes)
-        return sum(s["dram_bytes"] for s in shapes) / n, sum(s["algorithmic_bytes"] for s in shapes) / n, None
-    tot = alg = cnt = 0.0
-    rows = {}
-    for shp, v in per_shape.items():
-        s = table.get(tuple(shp))
-        if s is None:
-            continue
-        tot += s["dram_bytes"] * v[0]; alg += s["algorithmic_bytes"] * v[0]; cnt += v[0]
-        rows[f"{shp[0]}x{shp[1]}x{shp[2]}"] = {"dram_bytes": s["dram_bytes"], "algorithmic_bytes": s["algorithmic_bytes"], "ratio": s["ratio"]}
-    if not cnt:
-        return None, None, None
-    return tot / cnt, alg / cnt, rows
+METRIC = "tokens/sec Llama-3.2-3B seq4096 bf16 pretrain step (global, all GPUs)"
 
 
 def load_peaks():
@@ -74,7 +48,7 @@ def load_peaks():
         return dict(bf16_burst=p["bf16_tflops"], bf16_sustained=p["bf16_tflops_sustained"], hbm=p["hbm_gbs"],
                     source="measured (MEASURED_PEAKS.json)")
     except Exception:
-        return dict(bf16_burst=1590.0, bf16_sustained=1400.0, hbm=6650.0, source="fallback (B200_PROFILING.md)")
+        return dict(bf16_burst=989.0, bf16_sustained=989.0, hbm=3350.0, source="H100 SXM data sheet (dense BF16, 700 W)")
 
 
 class ClockSampler:
@@ -125,13 +99,13 @@ class ClockSampler:
 # ----------------------------------------------------------------------------------------------------------------
 # CPU baseline (oracle port): one decoder layer fwd+bwd + lm_head/criterion fwd+bwd on a bounded token sample
 # ----------------------------------------------------------------------------------------------------------------
-def cpu_reference_sample(layer_tokens: int = 512, head_tokens: int = 128, attn_heads: int = 8, threads: int | None = None):
+def cpu_reference_sample(layer_tokens: int = 512, head_tokens: int = 128, attn_heads: int = 6, threads: int | None = None):
     """Times the oracle (oracle/llama_ref.py, bf16-rounding mode) on the host cores and extrapolates tokens/s of the
-    full Llama-3-8B step:  tokens/s = 1 / (32 * (t_layer/token + t_attn4096/token) + t_head/token)  where
+    full benchmark step (Llama-3.2-3B shapes):  tokens/s = 1 / (L * (t_layer/token + t_attn4096/token) + t_head/token)  where
       t_layer     = fwd+bwd of ONE full-width decoder layer on `layer_tokens` tokens (its own attention runs at that short
                     length: ~1 % of the layer's work),
-      t_attn4096  = fwd+bwd of the causal GQA attention at the REAL sequence length 4096 on `attn_heads` of the 32 q heads
-                    (attn_heads/4 kv heads), scaled to 32 heads,
+      t_attn4096  = fwd+bwd of the causal GQA attention at the REAL sequence length 4096 on `attn_heads` of the q heads
+                    (attn_heads/3 kv heads), scaled to all heads,
       t_head      = final norm + lm_head + criterion fwd+bwd on `head_tokens` tokens."""
     import torch
 
@@ -147,7 +121,7 @@ def cpu_reference_sample(layer_tokens: int = 512, head_tokens: int = 128, attn_h
             threads = os.cpu_count() or 1
     torch.set_num_threads(threads)
     cores = torch.get_num_threads()
-    cfg = R.llama3_8b()
+    cfg = R.llama3_2_3b()
     g = torch.Generator().manual_seed(0)
     h, I, d = cfg.hidden_size, cfg.intermediate_size, cfg.head_dim
     kvd = cfg.num_key_value_heads * d
@@ -191,7 +165,7 @@ def cpu_reference_sample(layer_tokens: int = 512, head_tokens: int = 128, attn_h
                 sample=(f"oracle/llama_ref.py (torch CPU, bf16-rounding mode) fwd+bwd of ONE full-width decoder layer on "
                         f"{layer_tokens} tokens ({t_layer:.2f} s) + causal GQA attention fwd+bwd at seq {SEQ} on {akv * rep} of "
                         f"{cfg.num_attention_heads} q heads (scaled to all heads: {t_attn:.2f} s) + final-norm/lm_head/criterion "
-                        f"on {head_tokens} tokens ({t_head:.2f} s); extrapolated x32 layers; optimizer step not included"),
+                        f"on {head_tokens} tokens ({t_head:.2f} s); extrapolated x{cfg.num_hidden_layers} layers; optimizer step not included"),
                 seconds=t_layer + t_attn * (akv * rep) / cfg.num_attention_heads + t_head)
 
 
@@ -211,7 +185,7 @@ def run_reference(args):
     out = {"impl": "reference", "metric": METRIC, "value": v, "unit": "tokens/s", "n_gpus": args.gpus, "steps": args.steps,
            "warmup": args.warmup, "ms_per_step": secs * 1e3, "higher_is_better": True, "scaling": "weak",
            "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
-           "config": {"workload": "Llama-3-8B bf16 pretrain step, per-GPU batch 8 x seq 4096 (BASELINE.json configs[1])",
+           "config": {"workload": "Llama-3.2-3B bf16 pretrain step, per-GPU batch 8 x seq 4096",
                       "note": "reference arm = the reference's math on host CPU cores (PaddlePaddle is not installable "
                               "here); each step is a bounded sample, value extrapolated to the full model"},
            "cpu_baseline": base,
@@ -224,10 +198,10 @@ def run_reference(args):
 # ----------------------------------------------------------------------------------------------------------------
 # kernel family of every C-ABI entry point the training step calls (for `breakdown`)
 FAMILY = {
-    "b200_gemm_bf16_ex": "gemm (tcgen05)", "b200_gemm_bf16": "gemm (tcgen05)",
-    "b200_gemm_swiglu_bf16": "gemm + swiglu epilogue (tcgen05)", "b200_gemm_swiglu_bwd_bf16": "gemm + swiglu-bwd epilogue (tcgen05)",
-    "b200_fa_fwd_flashmask": "attention fwd (tcgen05)", "b200_fa_fwd": "attention fwd (tcgen05)",
-    "b200_fa_bwd_flashmask": "attention bwd (tcgen05)", "b200_fa_bwd": "attention bwd (tcgen05)",
+    "b200_gemm_bf16_ex": "gemm (wgmma)", "b200_gemm_bf16": "gemm (wgmma)",
+    "b200_gemm_swiglu_bf16": "gemm + swiglu epilogue (wgmma)", "b200_gemm_swiglu_bwd_bf16": "gemm + swiglu-bwd epilogue (wgmma)",
+    "b200_fa_fwd_flashmask": "attention fwd (mma.sync)", "b200_fa_fwd": "attention fwd (mma.sync)",
+    "b200_fa_bwd_flashmask": "attention bwd (mma.sync)", "b200_fa_bwd": "attention bwd (mma.sync)",
     "b200_rmsnorm_fwd": "rmsnorm", "b200_rmsnorm_bwd": "rmsnorm", "b200_rope_inplace": "rope",
     "b200_swiglu_fwd": "swiglu", "b200_swiglu_bwd": "swiglu", "b200_embedding_fwd": "embedding",
     "b200_embedding_bwd": "embedding", "b200_ce_fwd": "cross-entropy", "b200_ce_bwd": "cross-entropy",
@@ -270,7 +244,7 @@ def run_native(args):
     dev = torch.device("cuda", local)
     _lib.call("b200_device_check")
 
-    cfg = T.LlamaConfig.llama3_8b(num_hidden_layers=args.layers) if args.layers else T.LlamaConfig.llama3_8b()
+    cfg = T.LlamaConfig.llama3_2_3b(num_hidden_layers=args.layers) if args.layers else T.LlamaConfig.llama3_2_3b()
     model = T.LlamaForCausalLM(cfg)
     eng = model.engine
     dp = dist_env.DataParallel(model) if world > 1 else None
@@ -302,7 +276,7 @@ def run_native(args):
     host_ids = tok_e2e[:, :, :-1].contiguous().pin_memory()
     host_lab = tok_e2e[:, :, 1:].contiguous().pin_memory()
     del tok_res, tok_e2e
-    l2_flush = torch.empty(192 * 1024 * 1024, dtype=torch.uint8, device=dev)   # > 126 MB L2
+    l2_flush = torch.empty(192 * 1024 * 1024, dtype=torch.uint8, device=dev)   # > 50 MB L2
     step_losses = []        # device scalars of the first micro-batch of every resident step (read after the timed region)
 
     def step_resident(i):
@@ -385,6 +359,8 @@ def run_native(args):
     _lib.call_hook = hook if rank == 0 else None
     ms = timed(step_resident, args.steps, first=args.warmup)
     _lib.call_hook = None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, step_losses[args.warmup + args.steps - 1], model)
     launches = _lib.launch_count - launches0
     clocks = sampler.stop() if rank == 0 else None
     gemm_ms = sum(e0.elapsed_time(e1) for e0, e1, _, _ in gemm_events)
@@ -439,18 +415,16 @@ def run_native(args):
     hbm_peak_gb = torch.cuda.max_memory_allocated() / 2 ** 30
     out = None
     if rank == 0:
-        traffic, traffic_alg, traffic_rows = gemm_traffic_from_profile(per_shape)
         out = {
             "metric": METRIC, "value": value, "unit": "tokens/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "bf16",
             "data": "synthetic",
-            "config": {"workload": "Llama-3-8B bf16 pretrain step, per-GPU batch 8 x seq 4096 (BASELINE.json configs[1]; "
-                                   "configs[2] at 8 GPUs)",
-                       "model": "Llama-3-8B" if not args.layers else f"Llama-3-8B width, {args.layers} layers (DEBUG, not the metric)",
+            "config": {"workload": "Llama-3.2-3B bf16 pretrain step, per-GPU batch 8 x seq 4096",
+                       "model": "Llama-3.2-3B" if not args.layers else f"Llama-3.2-3B width, {args.layers} layers (DEBUG, not the metric)",
                        "global_batch": PER_GPU_BATCH * world, "seq_len": SEQ, "micro_batch": mb, "grad_accum": accum,
                        "parallelism": f"dp{world}", "optimizer": "AdamW fp32 master + global-norm clip, in the timed step",
                        "batches": "a fresh uniform-random batch every step (seed 1234, drawn on the CPU before the timed region)",
-                       "l2": "inputs (weights 16 GB, activations) exceed the 126 MB L2; a 192 MB flush precedes the timed region"},
+                       "l2": "inputs (weights 7 GB, activations) exceed the 50 MB L2; a 192 MB flush precedes the timed region"},
             "clocks": clocks,
             "gpu_launches": launches,
             "hbm_peak_allocated_gb": hbm_peak_gb,
@@ -461,19 +435,14 @@ def run_native(args):
             "model_tflops_per_gpu": tf_per_gpu,
             "clock_normalised": {"sm_mhz_over_max": (clocks["sm_mhz"] / clocks["sm_max_mhz"]) if clocks and clocks.get("sm_mhz") else None,
                                  "model_tflops_per_gpu_per_ghz": (tf_per_gpu / (clocks["sm_mhz"] / 1e3)) if clocks and clocks.get("sm_mhz") else None,
-                                 "note": "the step runs under sw_power_cap: compare rounds/boxes by TFLOP/s per GHz of median SM clock"},
-            "mfu": {"algorithmic_gflop_per_token": flops_per_token / 1e9, "vs_nominal_2250": tf_per_gpu / 2250.0,
+                                 "note": "compare runs on different boxes by TFLOP/s per GHz of median SM clock"},
+            "mfu": {"algorithmic_gflop_per_token": flops_per_token / 1e9, "vs_nominal_989": tf_per_gpu / 989.0,
                     "vs_measured_burst": tf_per_gpu / peaks["bf16_burst"], "vs_measured_sustained": tf_per_gpu / peaks["bf16_sustained"]},
-            "roofline": {"bound": "tensor", "kernel": "gemm_bf16_kernel (tcgen05, all projection/lm_head GEMMs fwd+bwd)",
+            "roofline": {"bound": "tensor", "kernel": "gemm_bf16_kernel (wgmma, all projection/lm_head GEMMs fwd+bwd)",
                          "achieved": gemm_tf, "peak": peaks["bf16_sustained"], "unit": "TFLOP/s",
                          "frac": (gemm_tf / peaks["bf16_sustained"]) if gemm_tf else None, "peak_source": peaks["source"] + ", sustained",
                          "launches_timed": n_gemm, "avg_launch_ms": gemm_ms / max(1, n_gemm), "share_of_step": gemm_ms / ms,
                          "algorithmic_flops_per_launch": gemm_flops / max(1, n_gemm),
-                         "traffic": traffic, "traffic_algorithmic": traffic_alg,
-                         "traffic_ratio": (traffic / traffic_alg) if traffic and traffic_alg else None,
-                         "traffic_unit": "DRAM bytes/launch, mean over this run's launches; per shape from the committed ncu capture "
-                                         "profiles/r02_gemm_traffic.json (cold L2)",
-                         "traffic_per_shape": traffic_rows,
                          "per_shape_MNK": {f"{k[0]}x{k[1]}x{k[2]}": {"launches": v[0], "ms_per_launch": round(v[1] / v[0], 4),
                                                                        "tflops": round(v[2] / (v[1] / 1e3) / 1e12, 1)}
                                            for k, v in sorted(per_shape.items(), key=lambda kv: -kv[1][1])}},
@@ -525,16 +494,36 @@ def run_native(args):
     print(json.dumps(out), flush=True)
 
 
+def dump_outputs(out_dir, loss, model, per_tensor=16384):
+    """What the timed path leaves to its caller after its last step: that step's loss (first micro-batch) and the updated
+    parameters, as a fixed seeded sample of `per_tensor` entries per tensor (float32, ~16 MB in all)."""
+    import numpy as np
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), loss.detach().float().reshape(-1).cpu().numpy())
+    g = torch.Generator().manual_seed(4321)
+    samples = []
+    for name, t in sorted(model.state_dict().items()):
+        flat = t.detach().reshape(-1)
+        idx = torch.randint(0, flat.numel(), (min(per_tensor, flat.numel()),), generator=g)
+        samples.append(flat[idx.to(flat.device)].float().cpu())
+    np.save(os.path.join(out_dir, "param_sample.npy"), torch.cat(samples).numpy())
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=4)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="native", choices=["native", "reference"])
-    ap.add_argument("--micro-batch", type=int, default=2, choices=[1, 2, 4, 8])
+    ap.add_argument("--micro-batch", type=int, default=1, choices=[1, 2, 4, 8])
     ap.add_argument("--layers", type=int, default=0, help="debug only: fewer layers (invalidates the metric)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
-    ap.add_argument("--only-pretrain", action="store_true", help="skip the Qwen2-7B SFT and Llama-3-8B decode sub-benchmarks")
+    ap.add_argument("--only-pretrain", action="store_true", help="skip the Qwen2-1.5B SFT and Llama-3-8B decode sub-benchmarks")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last timed step's loss and a fixed, seeded sample of the updated "
+                         "parameters as DIR/<name>.npy (float32), to compare two builds output for output")
     ap.add_argument("--sft-steps", type=int, default=4)
     args = ap.parse_args()
     if args.impl == "reference":

@@ -1,5 +1,5 @@
 /*
- * b200nlp.h — C-ABI of libb200nlp.so: hand-written sm_100a kernels for the PaddleNLP LLM decoder hot path.
+ * b200nlp.h — C-ABI of libb200nlp.so: hand-written sm_90a (H100) kernels for the PaddleNLP LLM decoder hot path.
  *
  * This is the drop-in boundary (SURVEY.md §8b).  Each entry point replaces one native op the reference reaches
  * through Paddle's custom-op C++ API (PD_BUILD_OP) or through a Paddle-core kernel; the reference call site is
@@ -33,34 +33,22 @@ typedef struct CUstream_st* cudaStream_t;
 /* ---- plumbing ------------------------------------------------------------------------------------------ */
 const char* b200_last_error(void);
 int b200_abi_version(void);
-/* 0 if the current device is compute capability 10.x (B200); error otherwise. */
+/* 0 if the current device is compute capability 9.0 (H100); error otherwise. */
 int b200_device_check(void);
 /* Programmatic dependent launch for the GEMM kernels (returns the previous setting; NOT an error code): when enabled, a GEMM
- * may start while the previous kernel of the stream is still draining — it prefetches its weight tiles and sets up TMEM /
- * barriers, and only waits (griddepcontrol.wait) before touching activations or outputs.  Used for the decode-step chain. */
+ * may become resident while the previous kernel of the stream is still draining; it waits (griddepcontrol.wait) before
+ * touching operands or outputs.  Used for the decode-step chain. */
 int b200_set_pdl(int enable);
-/* Which kernel serves the plain-causal b200_fa_fwd (returns the previous setting; NOT an error code): 2 (default) = two
- * 128-row q tiles per CTA with P kept in tensor memory (csrc/fa_fwd2.cu), 1 = one q tile per CTA (csrc/fa_fwd.cu, which
- * also serves every FlashMask call).  Same rounding points; kept switchable for A/B measurements.  The initial value can
- * be set with the environment variable B200_FA_FWD_IMPL. */
+/* q-tile height of b200_fa_fwd / b200_fa_fwd_flashmask (returns the previous setting; NOT an error code): 2 (default) = 128
+ * rows (8 warps) per CTA, 1 = 64 rows (4 warps).  Same rounding points; kept switchable for A/B measurements.  The initial
+ * value can be set with the environment variable B200_FA_FWD_IMPL. */
 int b200_set_fa_fwd_impl(int impl);
-/* Same for the plain-causal b200_fa_bwd: 2 (default) = transposed score tiles (kv on the UMMA M dimension), 64-row q steps,
- * S^T double-buffered, P^T kept in tensor memory (csrc/fa_bwd2.cu); 1 = csrc/fa_bwd.cu (also every FlashMask call).
+/* Same for b200_fa_bwd / b200_fa_bwd_flashmask: 2 (default) = 128-row q steps per 64-row kv tile, 1 = 64-row q steps.
  * Environment override: B200_FA_BWD_IMPL. */
 int b200_set_fa_bwd_impl(int impl);
-/* Share of the forward softmax exponentials (generation-2 kernel) evaluated by a degree-3 polynomial on the FMA pipe instead of
- * MUFU.EX2 (the MUFU's 16 ex2/clk/SM equals the tensor time of a kv step): 0 = none, 1 (default) = a quarter, 2 = half.
- * Relative error of the polynomial 7.5e-5, below the bf16 rounding P receives.  Environment override: B200_FA_EXP_POLY.
- * Returns the previous setting. */
-int b200_set_fa_exp_poly(int mode);
-/* Which kernel serves b200_gemm_bf16_splitk for M <= 128 with a row-major A (returns the previous setting; NOT an error
- * code): 1 (default) = the swapped-operand, two-CTA-per-SM weight-streaming kernel (csrc/gemm_skinny.cu), 2 = its stream-K
- * variant (M <= 64), 0 = the persistent 128x256 kernel in split-K mode.  Same results up to fp32 summation order; kept switchable
- * for A/B measurements. */
-int b200_set_skinny_gemm(int impl);
 
 /* ---- GEMM: replaces paddle.matmul / nn.Linear (cuBLASLt) --------------------------------------------------
- * C[M,N] (+)= op(A)[M,K] * op(B)[K,N] (+ bias[N]);  bf16 operands, fp32 accumulation in TMEM, ONE rounding to bf16.
+ * C[M,N] (+)= op(A)[M,K] * op(B)[K,N] (+ bias[N]);  bf16 operands, fp32 accumulation in registers (wgmma), ONE rounding to bf16.
  *   a_mn_major = 0 : A is stored [M,K] row-major (lda = row stride in elements)          — activations
  *   a_mn_major = 1 : A is stored [K,M] row-major (i.e. the caller passes A^T)            — dW = X^T * dY
  *   b_mn_major = 1 : B is stored [K,N] row-major — Paddle's nn.Linear weight layout [in,out]
@@ -78,7 +66,7 @@ int b200_gemm_bf16(const void* A, const void* B, void* C, const float* bias, int
  *   residual (bf16 [M,N], leading dimension ldr; exclusive with accumulate):
  *       C = bf16( bf16(acc + bias) + residual )  — the Linear-output rounding followed by the decoder layer's residual
  *       add (llama/modeling.py:1212, 1218), i.e. the reference's two rounding points in one kernel.
- *   cta_group 1 (one CTA per 128x256 tile) or 2 (CTA pair per 256x256 tile);
+ *   cta_group 1 or 2: accepted for compatibility; H100 has no CTA-pair MMA, both run one CTA per 128x256 tile;
  *   max_ctas > 0 limits the persistent grid (used to leave SMs to a concurrent kernel). */
 int b200_gemm_bf16_ex(const void* A, const void* B, void* C, const float* bias, const void* residual, int64_t M,
                       int64_t N, int64_t K, int64_t lda, int64_t ldb, int64_t ldc, int64_t ldr, int a_mn_major,
@@ -98,7 +86,7 @@ int b200_gemm_bf16_splitk(const void* A, const void* B, void* C, const float* bi
 /* gate|up projection + SwiGLU in ONE kernel — LlamaMLP.forward with fuse_attention_ffn (llama/modeling.py:632-652, swiglu :38-45):
  *   GU[M, 2I] = bf16(X[M,K] * W[K,2I])  (gate columns [0,I), up columns [I,2I); kept for the backward),
  *   Mout[M, I] = bf16(silu(gate) * up)  with gate/up rounded to bf16 first (the unfused rounding points).
- * A 256-column tcgen05 tile is formed from 128 gate columns and the 128 up columns of the same channels, so no interleaved
+ * A 256-column wgmma tile is formed from 128 gate columns and the 128 up columns of the same channels, so no interleaved
  * weight layout is needed; requires I % 128 == 0.  Bit-identical to b200_gemm_bf16 followed by b200_swiglu_fwd. */
 int b200_gemm_swiglu_bf16(const void* X, const void* W, void* GU, void* Mout, int64_t M, int64_t inter, int64_t K, int64_t ldx,
                           int64_t ldw, int64_t ldgu, int64_t ldm, int cta_group, cudaStream_t stream);
@@ -142,35 +130,13 @@ int b200_swiglu_fwd(const void* gate_up, void* out, int64_t rows, int64_t inter,
  * re-zeroed): the decode step's ffn1 -> fused_bias_act("swiglu") pair (fused_transformer_layers.py:100-168). */
 int b200_swiglu_fwd_f32(float* gate_up_f32_ws, void* out, int64_t rows, int64_t inter, cudaStream_t stream);
 /* Decode-step ffn1 + SwiGLU in one kernel (M <= 64 token rows): act[M, inter] = bf16(silu(g) * u) with g|u = bf16(X W).
- * W [K, 2*inter] is the reference-layout fused ffn1 weight (gate | up): one 128-feature tile of the swapped-operand
- * weight-streaming kernel is fed by two 64-column TMA boxes, gate channels [64j, 64j+64) and the up columns of the same channels
+ * W [K, 2*inter] is the reference-layout fused ffn1 weight (gate | up): the wgmma GEMM with 64-row tiles streams 128 gate
+ * columns and the up columns of the same channels per tile and applies the SwiGLU in its epilogue; gate|up are not stored
  * (fused_transformer_layers.py:100-168 fused_bias_act("swiglu") after ffn1).  inter % 64 == 0; ldact = row stride of act. */
 int b200_gemm_swiglu_skinny(const void* X, const void* W_gate_up, void* act, int64_t M, int64_t inter, int64_t K,
                             int64_t ldx, int64_t ldw, int64_t ldact, cudaStream_t stream);
 int b200_swiglu_bwd(const void* gate_up, const void* dout, void* dgate_up, int64_t rows, int64_t inter,
                     cudaStream_t stream);
-/* The GEMM chain of one decode-step layer (M <= 64 token rows) as ONE persistent kernel of two CTAs per SM whose six steps are
- * separated by grid-wide barriers instead of kernel boundaries, the weight stream running ahead across them
- * (fused_transformer_layers.py:895-896 out-linear, :937-949 ffn layernorm, :100-168 ffn1 + swiglu, ffn2, :976-999 residual +
- * next layernorm, :843-856 the NEXT layer's qkv projection):
- *   acc_h += attn @ W_o ; residual += bf16(acc_h), ln = rmsnorm(residual) * w_ffn_ln ; act = swiglu(bf16(ln @ W_ffn1)) ;
- *   acc_h += act @ W_ffn2 ; residual += bf16(acc_h), ln = rmsnorm(residual) * w_next_ln ; acc_qkv += ln @ W_next_qkv^T
- * attn bf16 [M, attn_width]; W_o [attn_width, h], W_ffn1 [h, 2*inter] (gate | up), W_ffn2 [inter, h], W_next_qkv [qkv_n, h] (the
- * reference layouts); residual bf16 [M, h] in/out; ln_buf [M, h] and act_buf [M, inter] bf16 scratch; acc_h fp32 [M, h] and
- * acc_qkv fp32 [M, qkv_n]: zero on entry, acc_h zero again on exit, acc_qkv holds the projection sums (same contract as
- * b200_gemm_bf16_splitk's workspace: the RoPE-append consumer rounds and re-zeroes).  w_next_ln / w_next_qkv NULL (last layer):
- * the chain ends with the residual update.  sync_ws: b200_decode_layer_chain_workspace_bytes() bytes, zero before the first call
- * (handed back zeroed).  Same rounding points and summation structure as the unfused kernels. */
-int64_t b200_decode_layer_chain_workspace_bytes(void);
-/* Debugging aid (tools/decode_probe.py chain): stamps = device buffer of 2 * 6 * 8 bytes per CTA (2 x SM count CTAs) that the next
- * launches fill with %globaltimer values — [cta][phase][0] = the producer saw the phase's inputs, [1] = the CTA published the
- * phase; NULL switches it off. */
-int b200_decode_layer_chain_debug(void* stamps);
-int b200_decode_layer_chain(const void* attn, const void* w_o, const void* w_ffn_ln, const void* w_ffn1, const void* w_ffn2,
-                            const void* w_next_ln, const void* w_next_qkv, void* residual, void* ln_buf, void* act_buf, float* acc_h,
-                            float* acc_qkv, void* sync_ws, int64_t M, int64_t h, int64_t attn_width, int64_t inter, int64_t qkv_n,
-                            float eps, cudaStream_t stream);
-
 /* ---- Embedding gather / scatter-add (nn.Embedding, llama/modeling.py:1465-1468, 1634). ids are int64. */
 int b200_embedding_fwd(const int64_t* ids, const void* table, void* out, int64_t tokens, int64_t h, int64_t vocab,
                        cudaStream_t stream);
@@ -266,8 +232,9 @@ int64_t b200_decode_attention_workspace_bytes(int64_t B, int64_t num_heads, int6
 int b200_decode_attention(const void* qkv, const void* cache, const int32_t* seq_lens, void* out, void* workspace, int64_t B,
                           int64_t num_heads, int64_t num_kv_heads, int64_t head_dim, int64_t max_len, int64_t ld,
                           float softmax_scale, int64_t num_splits, cudaStream_t stream);
-/* Same contract on the tensor cores: a persistent tcgen05 kernel streams the cache with TMA through a 192 KB ring per SM
- * (S^T = K_tile Q^T and O^T += V_tile^T P^T, the G query heads of a group padded to N=16); GQA group size 1, 2, 4, 7 or 8.
+/* Same contract, Hopper streaming kernel: a producer warp moves 32-row K/V chunks with cp.async.bulk into a 4-stage shared-memory
+ * ring on mbarriers, four consumer warps compute (a half-warp per cache row, the G heads of a group sharing each row); GQA group
+ * size 1, 2, 4, 7 or 8.
  * Cache rows past the sequence length must hold finite values (zero-filled allocation, as the reference's paddle.zeros). */
 int b200_decode_attention_tc(const void* qkv, const void* cache, const int32_t* seq_lens, void* out, void* workspace, int64_t B,
                              int64_t num_heads, int64_t num_kv_heads, int64_t head_dim, int64_t max_len, int64_t ld,
@@ -277,7 +244,7 @@ int b200_decode_attention_tc(const void* qkv, const void* cache, const int32_t* 
  * csrc/gpu/append_attention.cu:428-851): key_cache / value_cache [num_blocks, kvh, block_size, head_dim] bf16,
  * block_tables [B, max_blocks_per_seq] int32 (logical block -> physical block).  Same math as the dense entry points above:
  * prefill cache fill, decode RoPE + append (acc_f32_ws / bias optional as in b200_decode_rope_append_f32), decode attention
- * (tcgen05 kernel; each 128-row tile is gathered page by page with TMA; block_size 32, 64 or 128). */
+ * (the streaming kernel reads each cache row through the block table; block_size 32, 64 or 128). */
 int b200_write_cache_kv_paged(const void* qkv, void* key_cache, void* value_cache, const int32_t* block_tables,
                               const int32_t* seq_lens, int64_t B, int64_t S, int64_t num_heads, int64_t num_kv_heads,
                               int64_t head_dim, int64_t block_size, int64_t max_blocks_per_seq, int64_t ld, cudaStream_t stream);
@@ -361,7 +328,7 @@ int b200_save_output_stream(const int64_t* next_tokens, const int32_t* stop_coun
  * qkv [token_num, ldq] (rows cu_seqlens_q[b] ..), at absolute positions seq_lens_decoder[b] + i.  RoPE (rotate-half, tables
  * [rope_positions, 64] fp32) is applied to q and k in place, k and v are appended to the pages, and every row attends to cache
  * positions [0, its own]: prompts and prompt CHUNKS on top of a cached prefix (seq_lens_encoder[b] > 0 or more than one row)
- * through the tcgen05 flash kernel with page-gathered K/V, single decode rows through the decode kernel.  out [token_num, ldo].
+ * through the flash kernel with page-gathered K/V, single decode rows through the decode kernel.  out [token_num, ldo].
  * max_q_len >= max(seq_lens_this_time) (host bound for the grid; the reference passes max_enc_len_this_time the same way).
  * cu_seqlens_q replaces padding_offsets / cum_offsets (same information; get_padding_offset produces it).
  * No host synchronisation.  Workspace: b200_append_attention_workspace_bytes(). */

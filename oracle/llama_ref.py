@@ -64,6 +64,11 @@ def llama3_8b() -> RefConfig:
     return RefConfig()
 
 
+def llama3_2_3b() -> RefConfig:
+    """Llama-3.2-3B shapes with untied embeddings (the pre-training benchmark's model)."""
+    return RefConfig(hidden_size=3072, intermediate_size=8192, num_hidden_layers=28, num_attention_heads=24, num_key_value_heads=8)
+
+
 def qwen2_7b() -> RefConfig:
     return RefConfig(vocab_size=152064, hidden_size=3584, intermediate_size=18944, num_hidden_layers=28,
                      num_attention_heads=28, num_key_value_heads=4, rms_norm_eps=1e-6, rope_theta=1e6,

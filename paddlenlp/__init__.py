@@ -1,6 +1,6 @@
 """`paddlenlp` import-path shim: `import paddlenlp.X` resolves to `paddlenlp_b200.X` (the same module object).
 
-The B200-native implementation lives in `paddlenlp_b200/` (so that it can be installed next to the reference without
+The H100-native implementation lives in `paddlenlp_b200/` (so that it can be installed next to the reference without
 shadowing it); putting THIS directory on sys.path makes the reference's own import lines work unchanged for the hot path —
     from paddlenlp.trainer import PdArgumentParser, Trainer, TrainingArguments, get_last_checkpoint, set_seed, speed_metrics
     from paddlenlp.transformers import AutoConfig, AutoModelForCausalLM, LlamaConfig, LlamaForCausalLM, ...

@@ -1,4 +1,4 @@
-"""paddlenlp_b200 — B200-native (sm_100a) implementation of PaddleNLP's LLM decoder hot path.
+"""paddlenlp_b200 — H100-native (sm_90a) implementation of PaddleNLP's LLM decoder hot path.
 
 Sub-packages mirror the reference's import paths for the classes on that path:
     paddlenlp_b200.transformers  ~ paddlenlp.transformers  (LlamaConfig, LlamaForCausalLM, Qwen2ForCausalLM, Auto*)

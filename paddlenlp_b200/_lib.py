@@ -24,10 +24,8 @@ _SIGNATURES = {
     "b200_abi_version": [],
     "b200_device_check": [],
     "b200_set_pdl": [I],
-    "b200_set_skinny_gemm": [I],
     "b200_set_fa_fwd_impl": [I],
     "b200_set_fa_bwd_impl": [I],
-    "b200_set_fa_exp_poly": [I],
     "b200_gemm_bf16": [P, P, P, P, I64, I64, I64, I64, I64, I64, I, I, I, P],
     "b200_gemm_bf16_ex": [P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I, I, I, I, I, P],
     "b200_gemm_swiglu_bf16": [P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I, P],
@@ -44,9 +42,6 @@ _SIGNATURES = {
     "b200_swiglu_fwd_f32": [P, P, I64, I64, P],
     "b200_gemm_swiglu_skinny": [P, P, P, I64, I64, I64, I64, I64, I64, P],
     "b200_swiglu_bwd": [P, P, P, I64, I64, P],
-    "b200_decode_layer_chain_workspace_bytes": [],
-    "b200_decode_layer_chain_debug": [P],
-    "b200_decode_layer_chain": [P, P, P, P, P, P, P, P, P, P, P, P, P, I64, I64, I64, I64, I64, F, P],
     "b200_embedding_fwd": [P, P, P, I64, I64, I64, P],
     "b200_embedding_bwd": [P, P, P, I64, I64, I64, P],
     "b200_fa_fwd": [P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I64, I64, F, P],
@@ -99,7 +94,6 @@ _RESTYPE = {
     "b200_fa_bwd_workspace_bytes": c_int64,
     "b200_append_attention_workspace_bytes": c_int64,
     "b200_grad_sqnorm_workspace_bytes": c_int64,
-    "b200_decode_layer_chain_workspace_bytes": c_int64,
 }
 
 

@@ -36,28 +36,16 @@ int check_launch(const char* what) {
 
 static int g_pdl = 0;
 bool pdl_enabled() { return g_pdl != 0; }
-static int g_skinny_impl = 1;
-int skinny_gemm_impl() { return g_skinny_impl; }
-// attention kernel generations: forward 2 = two q tiles per CTA (fa_fwd2.cu), 1 = one q tile per CTA (fa_fwd.cu);
-// the initial value can be overridden with B200_FA_FWD_IMPL / B200_FA_BWD_IMPL for A/B runs of unmodified scripts
+// attention kernel tile sizes (fa_fwd.cu, fa_bwd.cu); the initial value can be overridden with B200_FA_FWD_IMPL /
+// B200_FA_BWD_IMPL for A/B runs of unmodified scripts
 static int env_int(const char* name, int dflt) {
   const char* v = getenv(name);
   return (v && *v) ? atoi(v) : dflt;
 }
 static int g_fa_fwd_impl = env_int("B200_FA_FWD_IMPL", 2);
 int fa_fwd_impl() { return g_fa_fwd_impl; }
-// backward 2 = transposed tiles, software-pipelined (fa_bwd2.cu), 1 = fa_bwd.cu
 static int g_fa_bwd_impl = env_int("B200_FA_BWD_IMPL", 2);
 int fa_bwd_impl() { return g_fa_bwd_impl; }
-// share of the forward softmax exponentials evaluated by a polynomial on the FMA pipe (fa_fwd2.cu exp2_poly2): 0, 1 (1/4), 2 (1/2)
-// Weight bytes a decode-step GEMM requests into L2 (beyond its shared-memory ring) before griddepcontrol.wait.  Round 1 used 64 MB;
-// with every kernel of the step launched programmatically the flood delays the small row-wise kernels that run meanwhile more than
-// it shortens the GEMM: generation 12.8 / 13.2 / 13.5 k tokens/s at 128 / 64 / 16 MB and 13.96 / 14.05 / 14.03 k at 16 / 8 / 0 MB
-// (profiles/r02_gen_bench_l2_prefetch_sweep.log).
-static int g_l2_prefetch_mb = env_int("B200_L2_PREFETCH_MB", 8);
-int l2_prefetch_mb() { return g_l2_prefetch_mb < 0 ? 0 : g_l2_prefetch_mb; }
-static int g_fa_exp_poly = env_int("B200_FA_EXP_POLY", 1);
-int fa_exp_poly() { return g_fa_exp_poly; }
 
 int sm_count() {
   static int cached[64];
@@ -67,7 +55,7 @@ int sm_count() {
   if (cached[dev] == 0) {
     int n = 0;
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    cached[dev] = n > 0 ? n : 148;
+    cached[dev] = n > 0 ? n : 132;
   }
   return cached[dev];
 }
@@ -151,21 +139,9 @@ int b200_set_fa_fwd_impl(int impl) {
   return old;
 }
 
-int b200_set_fa_exp_poly(int mode) {
-  int old = b200::g_fa_exp_poly;
-  b200::g_fa_exp_poly = mode < 0 ? 0 : (mode > 2 ? 2 : mode);
-  return old;
-}
-
 int b200_set_fa_bwd_impl(int impl) {
   int old = b200::g_fa_bwd_impl;
   b200::g_fa_bwd_impl = impl == 1 ? 1 : 2;
-  return old;
-}
-
-int b200_set_skinny_gemm(int impl) {
-  int old = b200::g_skinny_impl;
-  b200::g_skinny_impl = impl < 0 ? 0 : (impl > 2 ? 2 : impl);
   return old;
 }
 
@@ -179,7 +155,7 @@ int b200_device_check(void) {
   int major = 0, minor = 0;
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
   cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
-  if (major != 10) return b200::fail_arg("device %d is sm_%d%d; this library is built for sm_100a only", dev, major, minor);
+  if (major != 9 || minor != 0) return b200::fail_arg("device %d is sm_%d%d; this library is built for sm_90a only", dev, major, minor);
   return 0;
 }
 

@@ -1,8 +1,8 @@
-// Device-side primitives for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (UMMA + TMEM),
+// Device-side primitives for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma, mma.sync / ldmatrix, cp.async,
 // plus small vector / bf16 helpers shared by every kernel in this directory.
 //
-// Everything here is inline PTX; there is no CUTLASS/CuTe dependency.  Descriptor bit layouts follow the
-// PTX ISA "tcgen05 matrix descriptor" / "instruction descriptor" tables.
+// Everything here is inline PTX; there is no CUTLASS/CuTe dependency.  The wgmma descriptor layout follows the
+// PTX ISA "matrix descriptor" table for sm_90.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -48,11 +48,6 @@ __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
-// Mask that clears the "peer CTA" bit of a shared::cluster address, so that the address refers to the
-// even (leader) CTA of a CTA pair.
-static constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-
-
 // ------------------------------------------------------------------------------------------------
 // mbarrier
 // ------------------------------------------------------------------------------------------------
@@ -71,11 +66,6 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
 }
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// Arrive on the barrier at the same smem offset in the leader CTA of the pair (works from either CTA).
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & kPeerBitMask)
-               : "memory");
 }
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
@@ -126,14 +116,12 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* tm, uint64_t* bar
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-// Same, issued by either CTA of a pair; the transaction bytes are credited to the LEADER CTA's barrier.
-__device__ __forceinline__ void tma_load_2d_pair(const CUtensorMap* tm, uint64_t* bar, void* smem_dst, int c0,
-                                                 int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, "
-      "%4}], [%2];" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
+// Contiguous global -> shared copy by the bulk-copy (TMA) engine, completion on an mbarrier in this CTA; 16-byte aligned,
+// `bytes` a multiple of 16.
+__device__ __forceinline__ void bulk_load(void* smem_dst, const void* src, uint32_t bytes, uint64_t* bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(smem_dst)),
+               "l"(src), "r"(bytes), "r"(smem_u32(bar))
+               : "memory");
 }
 __device__ __forceinline__ void tma_load_3d(const CUtensorMap* tm, uint64_t* bar, void* smem_dst, int c0, int c1,
                                             int c2) {
@@ -195,133 +183,69 @@ __device__ __forceinline__ void tma_store_wait() {
 }
 
 // ------------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, MMA, commit, ld/st
+// Hopper warpgroup MMA (wgmma.mma_async): operands in shared memory, fp32 accumulators in registers
 // ------------------------------------------------------------------------------------------------
-template <int CG>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  if constexpr (CG == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-                 "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  } else {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-                 "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-}
-template <int CG>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  if constexpr (CG == 1)
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-  else
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// 64-bit shared-memory matrix descriptor (sm_100 "version 1"), 128-byte swizzle.
+// 64-bit shared-memory matrix descriptor (sm_90), 128-byte swizzle.
 //   start address  bits [0,14)   (>>4)
-//   LBO            bits [16,30)  (>>4)
-//   SBO            bits [32,46)  (>>4)
-//   version        bits [46,48)  = 1
-//   layout type    bits [61,64)  = 2 (SWIZZLE_128B)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+//   LBO            bits [16,30)  (>>4)   MN-major: byte distance between 64-element swizzle atoms along M/N
+//   SBO            bits [32,46)  (>>4)   byte distance between groups of 8 rows (K-major) / 8 k (MN-major)
+//   layout type    bits [62,64)  = 1 (SWIZZLE_128B)
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
-// 32-bit instruction descriptor for kind::f16 with bf16 inputs and fp32 accumulation.
-//   c_format [4,6)=1 (f32); a_format [7,10)=1 (bf16); b_format [10,13)=1 (bf16);
-//   a_major bit 15, b_major bit 16 (0 = K-major, 1 = MN-major); n>>3 at [17,23); m>>4 at [24,29).
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N, bool a_mn, bool b_mn) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(a_mn) << 15) |
-         (static_cast<uint32_t>(b_mn) << 16) | (static_cast<uint32_t>(N >> 3) << 17) |
-         (static_cast<uint32_t>(M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Register budget of a warpgroup (warp-specialised kernels: the TMA producer gives registers to the MMA warpgroups).
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+
+// d[64 x 256] (+)= A[64 x 16] * B[16 x 256], bf16 in, fp32 accumulate.  TA / TB: operand is MN-major (transposed).
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, %131, %132;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate), "n"(TA), "n"(TB));
 }
 
-// D[tmem] (+)= A[smem] * B[smem].  One thread issues on behalf of the CTA (pair).
-template <int CG>
-__device__ __forceinline__ void umma_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                        uint32_t accumulate) {
-  if constexpr (CG == 1) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-  }
-}
-// D[tmem] (+)= A[tmem] * B[smem]  (A operand read from tensor memory; K-major only).
-__device__ __forceinline__ void umma_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                        uint32_t accumulate) {
+// ------------------------------------------------------------------------------------------------
+// warp-level MMA (mma.sync m16n8k16, bf16 in, fp32 accumulate) and ldmatrix, for the attention kernels
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void mma_bf16_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+      "{%0, %1, %2, %3};"
+      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
-// Make an mbarrier track completion of all previously issued MMAs (implies fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+__device__ __forceinline__ void ldsm_x4(uint32_t saddr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(saddr));
 }
-// CTA-pair version: arrives on the barrier at this smem offset in both CTAs of the pair.
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(static_cast<uint16_t>(3))
-      : "memory");
+__device__ __forceinline__ void ldsm_x4_t(uint32_t saddr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(saddr));
 }
-
-// TMEM -> registers: this thread's lane (= 32*(warp%4) + lane), 32 consecutive fp32 columns.
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
+// 16-byte global -> shared copy (cp.async, L2 only); src_bytes = 0 fills the destination with zeros.
+__device__ __forceinline__ void cp_async_16(uint32_t saddr, const void* gptr, uint32_t src_bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(saddr), "l"(gptr), "r"(src_bytes) : "memory");
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// registers -> TMEM (same lane/column mapping as tmem_ld32).
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-      "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-      "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
 // ------------------------------------------------------------------------------------------------
 // bf16 / vector helpers
@@ -376,34 +300,20 @@ __device__ __forceinline__ float fast_rcp(float x) {
   return y;
 }
 
-// Packed fp32x2 arithmetic (FMUL2 / FADD2 / FFMA2: one issue slot for two IEEE round-to-nearest results, bit-identical to the
-// scalar .rn instructions and never re-associated or contracted by the compiler).
+// Pairs of fp32 operations with explicit round-to-nearest intrinsics: never re-associated or contracted by the compiler, so
+// every kernel that uses them (and the fused GEMM epilogues) produces the same bits.
 struct f32x2 { float x, y; };
-__device__ __forceinline__ f32x2 f2_mul(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("{\n\t.reg .b64 ra, rb, rd;\n\tmov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\tmul.rn.f32x2 rd, ra, rb;\n\t"
-      "mov.b64 {%0, %1}, rd;\n\t}" : "=f"(r.x), "=f"(r.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-  return r;
-}
-__device__ __forceinline__ f32x2 f2_add(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("{\n\t.reg .b64 ra, rb, rd;\n\tmov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\tadd.rn.f32x2 rd, ra, rb;\n\t"
-      "mov.b64 {%0, %1}, rd;\n\t}" : "=f"(r.x), "=f"(r.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-  return r;
-}
+__device__ __forceinline__ f32x2 f2_mul(f32x2 a, f32x2 b) { return f32x2{__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)}; }
+__device__ __forceinline__ f32x2 f2_add(f32x2 a, f32x2 b) { return f32x2{__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)}; }
 __device__ __forceinline__ f32x2 f2_fma(f32x2 a, f32x2 b, f32x2 c) {
-  f32x2 r;
-  asm("{\n\t.reg .b64 ra, rb, rc, rd;\n\tmov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\tmov.b64 rc, {%6, %7};\n\t"
-      "fma.rn.f32x2 rd, ra, rb, rc;\n\tmov.b64 {%0, %1}, rd;\n\t}"
-      : "=f"(r.x), "=f"(r.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y), "f"(c.x), "f"(c.y));
-  return r;
+  return f32x2{__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)};
 }
 
 // SwiGLU forward for two adjacent channels (llama/modeling.py:38-45, 648-650): m = bf16(silu(g) * u) from the bf16-rounded gate and
 // up projections.  sigmoid = rcp.approx(1 + ex2.approx(-g log2 e)) like the backward below (two SFU operations; an IEEE division
 // plus expf costs ~35 instructions per element, which made the fused ffn1 epilogue of the decode step 6 us long).  The ONE
-// definition used by b200_swiglu_fwd / _f32 and by the GEMM epilogues that fuse it (gemm_tcgen05.cu mode 4, gemm_skinny.cu
-// SWIGLU): the operation order is pinned by the packed instructions, so all of them produce the same bits.
+// definition used by b200_swiglu_fwd / _f32 and by the GEMM epilogue that fuses it (gemm_wgmma.cu mode 4): the operation order
+// is pinned by the round-to-nearest intrinsics, so all of them produce the same bits.
 __device__ __forceinline__ uint32_t swiglu_fwd_pair(uint32_t g2, uint32_t u2) {
   const float2 gf = unpack_bf16x2(g2), uf = unpack_bf16x2(u2);
   const f32x2 g{gf.x, gf.y}, u{uf.x, uf.y}, one{1.f, 1.f};
@@ -418,7 +328,7 @@ __device__ __forceinline__ uint32_t swiglu_fwd_pair(uint32_t g2, uint32_t u2) {
 //   sg = sigmoid(g) ; d(gate) = d * u * sg * (1 + g (1 - sg)) ; d(up) = d * g * sg          (fp32, results rounded once to bf16)
 // sigmoid = rcp.approx(1 + ex2.approx(-g log2 e)): two SFU operations (a few fp32 ulp, far inside the bf16 rounding of the
 // outputs) instead of an IEEE division.  The ONE definition used by b200_swiglu_bwd and by the GEMM epilogue that fuses it
-// (gemm_tcgen05.cu mode 5): the operation order is pinned by the packed instructions, so both produce the same bits.
+// (gemm_wgmma.cu mode 5): the operation order is pinned by the round-to-nearest intrinsics, so both produce the same bits.
 __device__ __forceinline__ void swiglu_bwd_pair(uint32_t g2, uint32_t u2, float d0, float d1, uint32_t& dg2, uint32_t& du2) {
   const float2 gf = unpack_bf16x2(g2), uf = unpack_bf16x2(u2);
   const f32x2 g{gf.x, gf.y}, u{uf.x, uf.y}, d{d0, d1}, one{1.f, 1.f};

@@ -1,4 +1,4 @@
-// Decode attention on tcgen05: one query token per sequence over the KV cache, GQA, head_dim 128.
+// Decode attention over the dense and the paged KV cache on Hopper: one query token per sequence, GQA, head_dim 128.
 //
 //   out[b, h, :] = softmax(q[b, h, :] K[b, kv(h), 0:len_b, :]^T / sqrt(d)) V[b, kv(h), 0:len_b, :]
 //
@@ -6,491 +6,267 @@
 // (paddlenlp/experimental/transformers/fused_transformer_layers.py:884-893;
 //  csrc/gpu/append_attn/append_attention_c16_impl.cuh:377-744, split-KV :826-1000).
 //
-// The op is a pure stream of the cache through the SM (2*len*d*2 bytes per (b, kv head), ~4 flop/byte), so the design
-// goal is bytes in flight, not math:
-//   * persistent kernel, two CTAs per SM; work items (split, b, kv head) are walked round-robin, and the TMA producer runs
-//     ahead ACROSS items, so the 3 x 32 KB K/V ring per CTA (192 KB in flight per SM) never drains between items;
-//   * "swapped" orientation so the cache tile is the 128-row M operand and the G query heads of the group are the
-//     (padded to 16) N operand:  S^T[kv, h] = K_tile Q^T  (UMMA 128x16x16 x8),  O^T[d, h] += V_tile^T P^T  (V consumed
-//     MN-major straight from the row-major cache tile); no CUDA-core instruction ever touches a K/V byte;
-//   * 4 softmax warps, one thread per cache row: G scores per thread and tile, tile max / final sum reduced with
-//     shuffles + 4-way smem exchange, lazy rescale of the TMEM-resident O^T accumulator (threshold 8 in log2 units);
-//   * split-KV partials use the layout of decode_attention_merge_kernel (generation.cu).
-//   * the last (partial) tile of a sequence is fetched in 32-row boxes, only as many as hold valid rows (at a context of ~1000
-//     tokens a full 128-row tail tile is 5-10 % of an item's bytes).
-// Masked rows contribute P = 0 (the shared-memory ring starts zero-filled, so the rows a partial tile does not fetch hold finite
-// values: zeros or an earlier tile).
-// Measured and NOT adopted (profiles/r02_decode_probe_attn_balanced_negative.log): cutting the launch's tiles into equal contiguous
-// runs per CTA (stream-K, pieces merged in-kernel through flags) instead of whole (b, kv head) items dealt round-robin — 512 items
-// on 296 CTAs look unbalanced (216 CTAs with two items), but the kernel is bound by the HBM stream, not by the longest CTA: the
-// balanced version was 4 % slower (51.8 vs 49.8 us at context 1048), the work it adds per segment is not paid back.
+// The op is a pure stream of the cache through the SM (2*len*d*2 bytes per (b, kv head), ~4 flop/byte, far below the
+// tensor-core ridge point), so the design goal is bytes in flight:
+//   * one producer warp moves 32-row K and V chunks (8 KB each, contiguous in both cache layouts: a page holds 32, 64 or 128
+//     rows) with the bulk-copy engine (cp.async.bulk) into a 4-stage shared-memory ring, completion on mbarriers; with two
+//     CTAs per SM (GQA groups up to 4) that is 128 KB of cache in flight per SM, independent of the math;
+//   * four consumer warps: a half-warp per cache row (16 lanes x 8 dims), the GQA group's G heads share every K/V row,
+//     online softmax in fp32 (exp2), the 8 half-warp partials merged through shared memory at the end;
+//   * split-KV partials ([B*nh, nsplit, 132] fp32: unnormalised o, running max, sum) are merged by
+//     decode_attention_merge_kernel (generation.cu).
+// b200_decode_attention (generation.cu, plain global loads) computes the same function and is the cross-check.
 #include "../../include/b200nlp.h"
 #include "common.cuh"
 #include "host_util.h"
 
 namespace b200 {
-namespace dtc {
+// generation.cu
+int launch_decode_attention_merge(const float* partial, void* out, int rows, int nsplit, cudaStream_t stream);
+
+namespace dab {
 
 constexpr int D = 128;
-constexpr int BKV = 128;                       // cache rows per tile
-constexpr int NPAD = 16;                       // query heads padded to the minimum UMMA N for M=128
-constexpr int TILE_BYTES = BKV * D * 2;        // 32 KB, two 64-column halves of 16 KB
-constexpr int HALF_BYTES = TILE_BYTES / 2;
-constexpr int QP_BYTES = NPAD * D * 2;         // 4 KB: [16 rows x 128] in two 2 KB halves (Q tile and P^T tile)
-constexpr int QP_HALF = QP_BYTES / 2;
-constexpr int NSLOT = 3;                       // x 2 CTAs per SM = 192 KB of cache tiles in flight per SM
-constexpr int NUM_THREADS = 192;               // TMA warp, MMA warp, 4 softmax warps
-constexpr int OFF_Q = NSLOT * TILE_BYTES;
-constexpr int OFF_P = OFF_Q + 2 * QP_BYTES;
-constexpr int OFF_BAR = OFF_P + QP_BYTES;
-constexpr int OFF_RED = OFF_BAR + 256;
-constexpr int SMEM_BYTES = OFF_RED + 512 + 1024;
-constexpr float RESCALE_THRESHOLD = 8.f;
+constexpr int ROWS = 32;                       // cache rows per chunk
+constexpr int NST = 4;                         // ring stages
+constexpr int CHUNK_BYTES = ROWS * D * 2;      // 8 KB of K (and as much of V) per stage
+constexpr int SMEM_BYTES = NST * 2 * CHUNK_BYTES;
+constexpr int NUM_THREADS = 160;               // 4 consumer warps + 1 producer warp
 
 struct Params {
+  const bf16* qkv;
+  const bf16* kc;
+  const bf16* vc;
   const int* seq_lens;
   bf16* out;          // [B, nh*128]
   float* partial;     // [B*nh, nsplit, 132] or null
-  int B, nh, kvh, max_len, nsplit, items;
+  int B, nh, kvh, max_len;
+  int64_t ld;
   float scale_log2;
-  // paged cache (block_tables != nullptr): key/value caches are [num_blocks, kvh, block_size, 128] and sequence b's logical
-  // block i lives in physical block block_tables[b * max_blocks + i]  (FusedBlockMultiTransformer / append_attention)
+  // paged cache (block_tables != nullptr): [num_blocks, kvh, block_size, 128], sequence b's logical block i in physical block
+  // block_tables[b * max_blocks + i]; dense: [B, kvh, max_len, 128]
   const int* block_tables;
   int max_blocks, block_size;
 };
 
-struct Item {
-  int b, kh, split, t_begin, t_end, ntiles;
-};
-
-__device__ __forceinline__ Item get_item(int idx, const Params& p) {
-  Item it;
-  const int bk = p.B * p.kvh;
-  it.split = idx / bk;                         // split-major: the (possibly empty) high splits are the tail of the walk
-  const int r = idx - it.split * bk;
-  it.b = r / p.kvh;
-  it.kh = r - it.b * p.kvh;
-  const int total = min(__ldg(p.seq_lens + it.b) + 1, p.max_len);   // the new token was appended at index seq_lens[b]
-  const int chunk = (((total + p.nsplit - 1) / p.nsplit) + BKV - 1) & ~(BKV - 1);
-  it.t_begin = it.split * chunk;
-  it.t_end = min(total, it.t_begin + chunk);
-  it.ntiles = it.t_end > it.t_begin ? (it.t_end - it.t_begin + BKV - 1) / BKV : 0;
-  return it;
-}
-
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t (&r)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t (&r)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(r[0]),
-               "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-
 template <int G, bool PAGED>
-__global__ void __launch_bounds__(NUM_THREADS, 2)
-decode_attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                           const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmK32,
-                           const __grid_constant__ CUtensorMap tmV32, const Params p) {
-  static_assert(G >= 1 && G <= 8, "group size");
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQ = smem + OFF_Q;               // 2 buffers
-  uint8_t* sP = smem + OFF_P;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
-  uint64_t* full = bars;                    // [NSLOT <= 6]
-  uint64_t* empty = bars + 6;               // [NSLOT <= 6]
-  uint64_t* q_full = bars + 12;             // [2]
-  uint64_t* q_empty = bars + 14;            // [2]
-  uint64_t* s_full = bars + 16;             // [2]
-  uint64_t* s_empty = bars + 18;            // [2]
-  uint64_t* p_full = bars + 20;             // [1]
-  uint64_t* pv_done = bars + 21;            // [1]
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 22);
-  float* s_red = reinterpret_cast<float*>(smem + OFF_RED);        // [2][4][8] tile maxima
-  float* s_lsum = s_red + 64;                                     // [4][8] row-sum partials
-
+__global__ void __launch_bounds__(NUM_THREADS, (G <= 4 ? 2 : 1)) decode_attention_bulk_kernel(const Params p) {
+  extern __shared__ __align__(128) uint8_t ring[];
+  __shared__ uint64_t full_bar[NST], empty_bar[NST];
+  __shared__ float s_m[8][G], s_l[8][G];
+  __shared__ float s_o[8][G][D];
+  const int b = blockIdx.x / p.kvh, kh = blockIdx.x % p.kvh;
+  const int total_len = min(p.seq_lens[b] + 1, p.max_len);   // the new token was appended at index seq_lens[b]
+  const int nsplit = gridDim.y, split = blockIdx.y;
+  const int chunk = (((max(total_len, 0) + nsplit - 1) / nsplit) + ROWS - 1) / ROWS * ROWS;
+  const int t_begin = split * chunk;
+  const int len = min(total_len, t_begin + chunk);
+  const int nchunks = len > t_begin ? (len - t_begin + ROWS - 1) / ROWS : 0;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  pdl_launch_dependents();
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV);
-    for (int i = 0; i < NSLOT; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&q_full[i], 1); mbar_init(&q_empty[i], 1);
-      mbar_init(&s_full[i], 1); mbar_init(&s_empty[i], 4);
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < NST; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 4);
     }
-    mbar_init(p_full, 128);
-    mbar_init(pv_done, 1);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc<1>(tmem_ptr_smem, 64);
-  if (warp >= 2) {   // P^T rows G..15 stay zero for the whole kernel
-    const int t = threadIdx.x - 64;
-    *reinterpret_cast<uint4*>(sP + t * 32) = make_uint4(0, 0, 0, 0);
-    *reinterpret_cast<uint4*>(sP + t * 32 + 16) = make_uint4(0, 0, 0, 0);
-    // pages / 32-row boxes past the end of a sequence are not fetched: their smem rows must still be finite (P = 0 there, but
-    // 0 * NaN = NaN in the PV accumulation)
-    for (int i = t; i < NSLOT * TILE_BYTES / 16; i += 128) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
-    fence_proxy_async_smem();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  pdl_wait();                                // q / cache / seq_lens belong to the predecessor kernels until now
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  const uint32_t tS0 = tmem_base, tO = tmem_base + 32;
+  pdl_launch_dependents();
+  pdl_wait();
 
-  if (warp == 0) {
-    // ------------------------------- TMA producer -------------------------------
+  if (warp == 4) {
+    // ------------------------------- producer -------------------------------
     if (lane == 0) {
-      uint32_t c = 0;      // ring counter (K and V tiles alternate)
-      int qi = 0;          // non-empty items so far
-      for (int idx = blockIdx.x; idx < p.items; idx += gridDim.x) {
-        const Item it = get_item(idx, p);
-        if (it.ntiles == 0) continue;
-        const int qb = qi & 1;
-        mbar_wait(&q_empty[qb], ((qi >> 1) & 1) ^ 1u);
-        mbar_arrive_expect_tx(&q_full[qb], QP_BYTES);
-        tma_load_3d(&tmQ, &q_full[qb], sQ + qb * QP_BYTES, 0, it.kh * G, it.b);
-        tma_load_3d(&tmQ, &q_full[qb], sQ + qb * QP_BYTES + QP_HALF, 64, it.kh * G, it.b);
-        ++qi;
-        const int plane = it.b * p.kvh + it.kh;
-        for (int j = 0; j < it.ntiles; ++j) {
-          const int t0 = it.t_begin + j * BKV;
-          if constexpr (PAGED) {
-            // a 128-row tile = 128 / block_size pages looked up in the block table; pages at or past t_end are skipped
-            const int ppt = BKV / p.block_size;
-            int phys[4];
-            int npages = 0;
-            for (int pg = 0; pg < ppt; ++pg) {
-              const int tpos = t0 + pg * p.block_size;
-              if (tpos < it.t_end) phys[npages++] = __ldg(p.block_tables + static_cast<size_t>(it.b) * p.max_blocks + tpos / p.block_size);
-            }
-            const uint32_t page_bytes = static_cast<uint32_t>(p.block_size) * D * 2;
-#pragma unroll
-            for (int kv = 0; kv < 2; ++kv, ++c) {
-              const uint32_t slot = c % NSLOT;
-              mbar_wait(&empty[slot], ((c / NSLOT) & 1u) ^ 1u);
-              mbar_arrive_expect_tx(&full[slot], page_bytes * npages);
-              const CUtensorMap* tm = kv ? &tmV : &tmK;
-              for (int pg = 0; pg < npages; ++pg) {
-                uint8_t* dst = smem + slot * TILE_BYTES + pg * (page_bytes / 2);
-                tma_load_4d(tm, &full[slot], dst, 0, 0, it.kh, phys[pg]);
-                tma_load_4d(tm, &full[slot], dst + HALF_BYTES, 64, 0, it.kh, phys[pg]);
-              }
-            }
-          } else {
-            const int rows = it.t_end - t0;                  // valid cache rows of this tile (< 128 only in a sequence's last tile)
-            const int nbox = (rows + 31) >> 5;               // 32-row boxes that hold them
-#pragma unroll
-            for (int kv = 0; kv < 2; ++kv, ++c) {
-              const uint32_t slot = c % NSLOT;
-              mbar_wait(&empty[slot], ((c / NSLOT) & 1u) ^ 1u);
-              uint8_t* dst = smem + slot * TILE_BYTES;
-              if (rows >= BKV) {
-                mbar_arrive_expect_tx(&full[slot], TILE_BYTES);
-                const CUtensorMap* tm = kv ? &tmV : &tmK;
-                tma_load_3d(tm, &full[slot], dst, 0, t0, plane);
-                tma_load_3d(tm, &full[slot], dst + HALF_BYTES, 64, t0, plane);
-              } else {
-                // a 32-row box = 4 KB per 64-column half = four 8-row swizzle atoms: same layout as the rows of the full box
-                mbar_arrive_expect_tx(&full[slot], static_cast<uint32_t>(nbox) * 8192u);
-                const CUtensorMap* tm = kv ? &tmV32 : &tmK32;
-                for (int bx = 0; bx < nbox; ++bx) {
-                  tma_load_3d(tm, &full[slot], dst + bx * 4096, 0, t0 + bx * 32, plane);
-                  tma_load_3d(tm, &full[slot], dst + HALF_BYTES + bx * 4096, 64, t0 + bx * 32, plane);
-                }
-              }
-            }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------- MMA issuer -------------------------------
-    if (lane == 0) {
-      constexpr uint32_t idesc_qk = umma_idesc_bf16(128, NPAD, false, false);   // A = K tile (K-major), B = Q (K-major)
-      constexpr uint32_t idesc_pv = umma_idesc_bf16(128, NPAD, true, false);    // A = V tile (MN-major), B = P^T (K-major)
-      struct Cursor { int idx; Item it; int j; int qi; bool valid; };
-      auto seek = [&](Cursor& cur) {          // cur.idx -> first non-empty item at or after it
-        cur.valid = false;
-        for (; cur.idx < p.items; cur.idx += gridDim.x) {
-          cur.it = get_item(cur.idx, p);
-          if (cur.it.ntiles > 0) { cur.valid = true; cur.j = 0; return; }
-        }
-      };
-      auto next = [&](Cursor& cur) {
-        if (cur.j + 1 < cur.it.ntiles) { ++cur.j; return; }
-        cur.idx += gridDim.x; ++cur.qi;
-        seek(cur);
-      };
-      const uint32_t sP_a = smem_u32(sP);
-      auto issue_qk = [&](const Cursor& cur, uint32_t n) {
-        const uint32_t sb = n & 1u;
-        mbar_wait(&s_empty[sb], ((n >> 1) & 1u) ^ 1u);
-        const int qb = cur.qi & 1;
-        if (cur.j == 0) mbar_wait(&q_full[qb], (cur.qi >> 1) & 1);
-        const uint32_t c = 2 * n, slot = c % NSLOT;
-        mbar_wait(&full[slot], (c / NSLOT) & 1u);
-        tc_fence_after();
-        const uint32_t sK_a = smem_u32(smem + slot * TILE_BYTES), sQ_a = smem_u32(sQ + qb * QP_BYTES);
-#pragma unroll
-        for (int kk = 0; kk < D / 16; ++kk) {
-          const uint32_t a_off = (kk >> 2) * HALF_BYTES + (kk & 3) * 32;
-          const uint32_t b_off = (kk >> 2) * QP_HALF + (kk & 3) * 32;
-          umma_ss<1>(tS0 + sb * NPAD, umma_desc_sw128(sK_a + a_off, 16, 1024), umma_desc_sw128(sQ_a + b_off, 16, 1024),
-                     idesc_qk, kk > 0 ? 1u : 0u);
-        }
-        umma_commit(&empty[slot]);
-        umma_commit(&s_full[sb]);
-        if (cur.j == cur.it.ntiles - 1) umma_commit(&q_empty[qb]);
-      };
-      Cursor a;
-      a.idx = blockIdx.x; a.qi = 0; a.j = 0;
-      seek(a);
-      if (a.valid) {
-        Cursor c = a;
-        issue_qk(a, 0);
-        next(a);
-        uint32_t n = 0;
-        while (c.valid) {
-          if (a.valid) { issue_qk(a, n + 1); next(a); }
-          const uint32_t cc = 2 * n + 1, slot = cc % NSLOT;
-          mbar_wait(&full[slot], (cc / NSLOT) & 1u);
-          mbar_wait(p_full, n & 1u);
-          tc_fence_after();
-          const uint32_t sV_a = smem_u32(smem + slot * TILE_BYTES);
-#pragma unroll
-          for (int kk = 0; kk < BKV / 16; ++kk) {
-            const uint32_t a_off = kk * 16 * 128;                             // 16 cache rows = 2 KB (MN-major A)
-            const uint32_t b_off = (kk >> 2) * QP_HALF + (kk & 3) * 32;       // P^T: kv along K
-            umma_ss<1>(tO, umma_desc_sw128(sV_a + a_off, HALF_BYTES, 1024), umma_desc_sw128(sP_a + b_off, 16, 1024),
-                       idesc_pv, (c.j > 0 || kk > 0) ? 1u : 0u);
-          }
-          umma_commit(&empty[slot]);
-          umma_commit(pv_done);
-          next(c);
-          ++n;
-        }
-      }
-    }
-  } else {
-    // ------------------------------- softmax / epilogue -------------------------------
-    const int quad = warp & 3;
-    const int r = quad * 32 + lane;            // cache row within the tile (S^T lane) and output dim d (O^T lane)
-    const uint32_t lane_off = static_cast<uint32_t>(quad * 32) << 16;
-    const uint32_t sP_a = smem_u32(sP);
-    const uint32_t p_addr = sP_a + (r >> 6) * QP_HALF + (r & 7) * 2;   // + h*128 + (((r&63)>>3) ^ (h&7))*16
-    const int rc = (r & 63) >> 3;
-    uint32_t n = 0;
-    for (int idx = blockIdx.x; idx < p.items; idx += gridDim.x) {
-      const Item it = get_item(idx, p);
-      if (it.ntiles == 0) {
-        if (p.partial != nullptr) {            // an empty split still owns its partial slot
-#pragma unroll
-          for (int h = 0; h < G; ++h) {
-            float* dst = p.partial + ((static_cast<size_t>(it.b) * p.nh + it.kh * G + h) * p.nsplit + it.split) * (D + 4);
-            dst[r] = 0.f;
-            if (r == 0) { dst[D] = -INFINITY; dst[D + 1] = 0.f; }
-          }
-        }
-        continue;
-      }
-      float m_used[G], l[G];
-#pragma unroll
-      for (int h = 0; h < G; ++h) { m_used[h] = -INFINITY; l[h] = 0.f; }
-      for (int j = 0; j < it.ntiles; ++j, ++n) {
-        const uint32_t sb = n & 1u;
-        mbar_wait(&s_full[sb], (n >> 1) & 1u);
-        tc_fence_after();
-        uint32_t sv[8];
-        tmem_ld8(tS0 + lane_off + sb * NPAD, sv);
-        tmem_ld_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&s_empty[sb]);
-        const bool valid = it.t_begin + j * BKV + r < it.t_end;
-        float x[G];
-#pragma unroll
-        for (int h = 0; h < G; ++h) {
-          x[h] = valid ? __uint_as_float(sv[h]) * p.scale_log2 : -INFINITY;
-          const float wm = warp_max(x[h]);
-          if (lane == 0) s_red[(sb * 4 + quad) * 8 + h] = wm;
-        }
-        named_bar_sync(2, 128);
-        bool rescale = false;
-        float factor[G];
-#pragma unroll
-        for (int h = 0; h < G; ++h) {
-          const float* sr = s_red + sb * 32 + h;
-          const float mt = fmaxf(fmaxf(sr[0], sr[8]), fmaxf(sr[16], sr[24]));   // finite: every tile has a valid row
-          factor[h] = 1.f;
-          if (j == 0) {
-            m_used[h] = mt;
-          } else if (mt > m_used[h] + RESCALE_THRESHOLD) {                      // uniform over the CTA
-            factor[h] = fast_exp2(m_used[h] - mt);
-            l[h] *= factor[h];
-            m_used[h] = mt;
-            rescale = true;
-          }
-        }
-        float pr[G];
-#pragma unroll
-        for (int h = 0; h < G; ++h) {
-          pr[h] = fast_exp2(x[h] - m_used[h]);       // exp2(-inf) = 0 for masked rows
-          l[h] += pr[h];
-        }
-        if (n > 0) {
-          mbar_wait(pv_done, (n - 1) & 1u);          // P^T buffer free, O^T accumulator quiescent
-          tc_fence_after();
-        }
-        if (rescale) {
-          uint32_t o[8];
-          tmem_ld8(tO + lane_off, o);
-          tmem_ld_wait();
-#pragma unroll
-          for (int h = 0; h < G; ++h) o[h] = __float_as_uint(__uint_as_float(o[h]) * factor[h]);
-          tmem_st8(tO + lane_off, o);
-          tmem_st_wait();
-        }
-#pragma unroll
-        for (int h = 0; h < G; ++h) {
-          const uint32_t addr = p_addr + h * 128 + ((rc ^ (h & 7)) << 4);
-          const unsigned short bits = __bfloat16_as_ushort(__float2bfloat16_rn(pr[h]));
-          asm volatile("st.shared.b16 [%0], %1;" ::"r"(addr), "h"(bits) : "memory");
-        }
-        fence_proxy_async_smem();
-        tc_fence_before();
-        mbar_arrive(p_full);
-      }
-      // ---- item epilogue: O^T / l (or the split partial) ----
-#pragma unroll
-      for (int h = 0; h < G; ++h) {
-        const float ws = warp_sum(l[h]);
-        if (lane == 0) s_lsum[quad * 8 + h] = ws;
-      }
-      mbar_wait(pv_done, (n - 1) & 1u);
-      tc_fence_after();
-      uint32_t o[8];
-      tmem_ld8(tO + lane_off, o);
-      tmem_ld_wait();
-      tc_fence_before();
-      named_bar_sync(2, 128);
-#pragma unroll
-      for (int h = 0; h < G; ++h) {
-        const float lt = s_lsum[h] + s_lsum[8 + h] + s_lsum[16 + h] + s_lsum[24 + h];
-        const int head = it.kh * G + h;
-        if (p.partial == nullptr) {
-          p.out[(static_cast<size_t>(it.b) * p.nh + head) * D + r] = __float2bfloat16_rn(__uint_as_float(o[h]) / lt);
+      for (int c = 0; c < nchunks; ++c) {
+        const int st = c % NST;
+        mbar_wait(&empty_bar[st], ((c / NST) & 1) ^ 1);
+        const int t0 = t_begin + c * ROWS;
+        const uint32_t bytes = static_cast<uint32_t>(min(ROWS, len - t0)) * D * 2;
+        size_t off;
+        if constexpr (PAGED) {
+          const int page = __ldg(p.block_tables + static_cast<size_t>(b) * p.max_blocks + t0 / p.block_size);
+          off = ((static_cast<size_t>(page) * p.kvh + kh) * p.block_size + t0 % p.block_size) * D;
         } else {
-          float* dst = p.partial + ((static_cast<size_t>(it.b) * p.nh + head) * p.nsplit + it.split) * (D + 4);
-          dst[r] = __uint_as_float(o[h]);
-          if (r == 0) { dst[D] = m_used[h]; dst[D + 1] = lt; }
+          off = ((static_cast<size_t>(b) * p.kvh + kh) * p.max_len + t0) * D;
+        }
+        mbar_arrive_expect_tx(&full_bar[st], 2 * bytes);
+        bulk_load(ring + st * 2 * CHUNK_BYTES, p.kc + off, bytes, &full_bar[st]);
+        bulk_load(ring + st * 2 * CHUNK_BYTES + CHUNK_BYTES, p.vc + off, bytes, &full_bar[st]);
+      }
+    }
+    return;
+  }
+
+  // ------------------------------- consumers -------------------------------
+  const int hw = warp * 2 + (lane >> 4);               // half-warp id 0..7
+  const int sub = lane & 15;                           // which 8 dims of the row
+  const unsigned hmask = (lane < 16) ? 0x0000ffffu : 0xffff0000u;
+  float q[G][8], o[G][8], m[G], l[G];
+#pragma unroll
+  for (int g = 0; g < G; ++g) {
+    const uint4 qv = *reinterpret_cast<const uint4*>(p.qkv + static_cast<size_t>(b) * p.ld + (kh * G + g) * D + sub * 8);
+    const uint32_t* qi = reinterpret_cast<const uint32_t*>(&qv);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float2 f = unpack_bf16x2(qi[j]);
+      q[g][2 * j] = f.x * p.scale_log2; q[g][2 * j + 1] = f.y * p.scale_log2;
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) o[g][j] = 0.f;
+    m[g] = -INFINITY; l[g] = 0.f;
+  }
+  constexpr int U = ROWS / 8;                          // rows per half-warp and chunk
+  const uint32_t ring_s = smem_u32(ring);
+  for (int c = 0; c < nchunks; ++c) {
+    const int st = c % NST;
+    const int rows = min(ROWS, len - (t_begin + c * ROWS));
+    mbar_wait(&full_bar[st], (c / NST) & 1);
+    const uint32_t kb = ring_s + st * 2 * CHUNK_BYTES, vb = kb + CHUNK_BYTES;
+    uint4 kv[U], vv[U];
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const int r = hw + 8 * u;
+      if (r < rows) {
+        kv[u] = ld_shared_v4(kb + r * (D * 2) + sub * 16);
+        vv[u] = ld_shared_v4(vb + r * (D * 2) + sub * 16);
+      }
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty_bar[st]);        // this warp's reads of the stage are in registers
+    float sc[U][G];
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const uint32_t* ki = reinterpret_cast<const uint32_t*>(&kv[u]);
+      float kf[8];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) { const float2 a = unpack_bf16x2(ki[j]); kf[2 * j] = a.x; kf[2 * j + 1] = a.y; }
+#pragma unroll
+      for (int g = 0; g < G; ++g) {
+        float sdot = 0.f;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) sdot += q[g][j] * kf[j];
+        sc[u][g] = sdot;
+      }
+    }
+#pragma unroll
+    for (int off = 8; off > 0; off >>= 1)
+#pragma unroll
+      for (int u = 0; u < U; ++u)
+#pragma unroll
+        for (int g = 0; g < G; ++g) sc[u][g] += __shfl_xor_sync(hmask, sc[u][g], off);
+#pragma unroll
+    for (int g = 0; g < G; ++g) {
+      float mn = m[g];
+#pragma unroll
+      for (int u = 0; u < U; ++u)
+        if (hw + 8 * u < rows) mn = fmaxf(mn, sc[u][g]);
+      // m = -inf before this half-warp's first valid row -> corr = 0 (o and l are still 0); a chunk may hold no row of this
+      // half-warp at all (mn = -inf): exp2(-inf - -inf) must not be evaluated
+      const float corr = (mn == -INFINITY) ? 1.f : fast_exp2(m[g] - mn);
+      m[g] = mn;
+      l[g] *= corr;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) o[g][j] *= corr;
+    }
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      if (hw + 8 * u < rows) {                         // uniform within the half-warp
+        const uint32_t* vi = reinterpret_cast<const uint32_t*>(&vv[u]);
+        float vf[8];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) { const float2 cc = unpack_bf16x2(vi[j]); vf[2 * j] = cc.x; vf[2 * j + 1] = cc.y; }
+#pragma unroll
+        for (int g = 0; g < G; ++g) {
+          const float pr = fast_exp2(sc[u][g] - m[g]);
+          l[g] += pr;
+#pragma unroll
+          for (int j = 0; j < 8; ++j) o[g][j] += pr * vf[j];
         }
       }
-      named_bar_sync(2, 128);                        // s_lsum is rewritten by the next item
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<1>(tmem_base, 64);
+  // merge the 8 half-warp partials (consumer warps only: the producer warp has left)
+#pragma unroll
+  for (int g = 0; g < G; ++g) {
+    if (sub == 0) { s_m[hw][g] = m[g]; s_l[hw][g] = l[g]; }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) s_o[hw][g][sub * 8 + j] = o[g][j];
+  }
+  named_bar_sync(1, 128);
+  for (int idx = threadIdx.x; idx < G * D; idx += 128) {
+    const int g = idx / D, dd = idx % D;
+    float mm = -INFINITY;
+#pragma unroll
+    for (int w = 0; w < 8; ++w) mm = fmaxf(mm, s_m[w][g]);
+    float acc = 0.f, lt = 0.f;
+#pragma unroll
+    for (int w = 0; w < 8; ++w) {
+      const float f = (s_m[w][g] == -INFINITY) ? 0.f : exp2f(s_m[w][g] - mm);
+      acc += s_o[w][g][dd] * f;
+      lt += s_l[w][g] * f;
+    }
+    if (nsplit == 1) {
+      p.out[static_cast<size_t>(b) * p.nh * D + (kh * G + g) * D + dd] = __float2bfloat16_rn(lt > 0.f ? acc / lt : 0.f);
+    } else {
+      float* dst = p.partial + ((static_cast<size_t>(b) * p.nh + kh * G + g) * nsplit + split) * (D + 4);
+      dst[dd] = acc;
+      if (dd == 0) { dst[D] = mm; dst[D + 1] = lt; }
+    }
   }
 }
 
-}  // namespace dtc
-
-// defined in generation.cu
-int launch_decode_attention_merge(const float* partial, void* out, int rows, int nsplit, cudaStream_t stream);
-
-}  // namespace b200
-
-namespace b200 {
-namespace dtc {
-
 template <bool PAGED>
-static int launch(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const CUtensorMap& tmK32,
-                  const CUtensorMap& tmV32, const Params& p, int G, void* out, int64_t B, int64_t num_heads, int64_t num_splits,
-                  cudaStream_t stream) {
-  const int max_ctas = 2 * sm_count();      // two co-resident CTAs per SM: item prologues/epilogues of one overlap the other's stream
-  const unsigned grid = static_cast<unsigned>(p.items < max_ctas ? p.items : max_ctas);
-#define B200_DTC(GG)                                                                                                 \
+static int launch(const Params& p, int G, int64_t num_splits, cudaStream_t stream) {
+  const dim3 grid(static_cast<unsigned>(p.B * p.kvh), static_cast<unsigned>(num_splits));
+#define B200_DAB(GG)                                                                                                 \
   case GG: {                                                                                                         \
     static bool attr_set = false;                                                                                    \
     if (!attr_set) {                                                                                                 \
-      cudaError_t e = cudaFuncSetAttribute(decode_attention_tc_kernel<GG, PAGED>,                                    \
+      cudaError_t e = cudaFuncSetAttribute(decode_attention_bulk_kernel<GG, PAGED>,                                  \
                                            cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);                \
       if (e != cudaSuccess) {                                                                                        \
-        set_last_error("decode_attention_tc smem attr: %s", cudaGetErrorString(e));                                  \
+        set_last_error("decode_attention smem attr: %s", cudaGetErrorString(e));                                     \
         return static_cast<int>(e);                                                                                  \
       }                                                                                                              \
       attr_set = true;                                                                                               \
     }                                                                                                                \
-    launch_pdl(decode_attention_tc_kernel<GG, PAGED>, dim3(grid), dim3(NUM_THREADS), SMEM_BYTES, stream, tmQ, tmK, tmV, tmK32, \
-               tmV32, p);                                                                                            \
+    launch_pdl(decode_attention_bulk_kernel<GG, PAGED>, grid, dim3(NUM_THREADS), SMEM_BYTES, stream, p);             \
   } break;
   switch (G) {
-    B200_DTC(1) B200_DTC(2) B200_DTC(4) B200_DTC(7) B200_DTC(8)
+    B200_DAB(1) B200_DAB(2) B200_DAB(4) B200_DAB(7) B200_DAB(8)
     default:
       return fail_arg("decode_attention_tc: GQA group size %d not instantiated (1, 2, 4, 7, 8)", G);
   }
-#undef B200_DTC
+#undef B200_DAB
   int rc = check_launch("decode_attention_tc");
   if (rc || num_splits == 1) return rc;
-  return launch_decode_attention_merge(p.partial, out, static_cast<int>(B * num_heads), static_cast<int>(num_splits), stream);
+  return launch_decode_attention_merge(p.partial, p.out, p.B * p.nh, static_cast<int>(num_splits), stream);
 }
 
-static int make_q_map(CUtensorMap* tm, const void* qkv, int64_t B, int64_t num_heads, int64_t ld) {
-  uint64_t dims[3] = {128, static_cast<uint64_t>(num_heads), static_cast<uint64_t>(B)};
-  uint64_t strides[2] = {128 * 2, static_cast<uint64_t>(ld) * 2};
-  uint32_t box[3] = {64, NPAD, 1};
-  return encode_tmap_bf16(tm, qkv, 3, dims, strides, box);
-}
-
-}  // namespace dtc
+}  // namespace dab
 }  // namespace b200
 
 extern "C" int b200_decode_attention_tc(const void* qkv, const void* cache, const int32_t* seq_lens, void* out, void* workspace,
                                         int64_t B, int64_t num_heads, int64_t num_kv_heads, int64_t head_dim, int64_t max_len,
                                         int64_t ld, float softmax_scale, int64_t num_splits, cudaStream_t stream) {
-  using namespace b200;
-  using namespace b200::dtc;
   B200_CHECK_ARG(qkv && cache && seq_lens && out, "decode_attention_tc: null pointer");
   B200_CHECK_ARG(num_splits >= 1 && num_splits <= 64 && (num_splits == 1 || workspace),
                  "decode_attention_tc: bad num_splits / workspace");
   B200_CHECK_ARG(head_dim == 128, "decode_attention_tc: head_dim must be 128 (got %lld)", (long long)head_dim);
   B200_CHECK_ARG(B > 0 && num_kv_heads > 0 && num_heads % num_kv_heads == 0 && max_len > 0 && ld % 8 == 0,
                  "decode_attention_tc: bad shape");
-  CUtensorMap tmQ, tmK, tmV, tmK32, tmV32;
-  int rc;
-  if ((rc = make_q_map(&tmQ, qkv, B, num_heads, ld)) != 0) return rc;
-  {
-    uint64_t dims[3] = {128, static_cast<uint64_t>(max_len), static_cast<uint64_t>(B * num_kv_heads)};
-    uint64_t strides[2] = {128 * 2, static_cast<uint64_t>(max_len) * 128 * 2};
-    uint32_t box[3] = {64, BKV, 1};
-    uint32_t box32[3] = {64, 32, 1};           // a sequence's last, partial tile
-    const bf16* kbase = static_cast<const bf16*>(cache);
-    const bf16* vbase = kbase + static_cast<size_t>(B) * num_kv_heads * max_len * 128;
-    if ((rc = encode_tmap_bf16(&tmK, kbase, 3, dims, strides, box)) != 0) return rc;
-    if ((rc = encode_tmap_bf16(&tmV, vbase, 3, dims, strides, box)) != 0) return rc;
-    if ((rc = encode_tmap_bf16(&tmK32, kbase, 3, dims, strides, box32)) != 0) return rc;
-    if ((rc = encode_tmap_bf16(&tmV32, vbase, 3, dims, strides, box32)) != 0) return rc;
-  }
-  Params p = {};
+  using namespace b200;
+  dab::Params p = {};
+  p.qkv = static_cast<const bf16*>(qkv);
+  p.kc = static_cast<const bf16*>(cache);
+  p.vc = p.kc + static_cast<size_t>(B) * num_kv_heads * max_len * 128;
   p.seq_lens = seq_lens;
   p.out = static_cast<bf16*>(out);
-  p.partial = num_splits > 1 ? static_cast<float*>(workspace) : nullptr;
+  p.partial = static_cast<float*>(workspace);
   p.B = static_cast<int>(B); p.nh = static_cast<int>(num_heads); p.kvh = static_cast<int>(num_kv_heads);
-  p.max_len = static_cast<int>(max_len); p.nsplit = static_cast<int>(num_splits);
-  p.items = static_cast<int>(B * num_kv_heads * num_splits);
+  p.max_len = static_cast<int>(max_len); p.ld = ld;
   p.scale_log2 = softmax_scale * 1.4426950408889634f;
-  return launch<false>(tmQ, tmK, tmV, tmK32, tmV32, p, static_cast<int>(num_heads / num_kv_heads), out, B, num_heads, num_splits,
-                       stream);
+  return dab::launch<false>(p, static_cast<int>(num_heads / num_kv_heads), num_splits, stream);
 }
 
 extern "C" int b200_decode_attention_paged(const void* qkv, const void* key_cache, const void* value_cache,
@@ -498,8 +274,6 @@ extern "C" int b200_decode_attention_paged(const void* qkv, const void* key_cach
                                            int64_t B, int64_t num_heads, int64_t num_kv_heads, int64_t head_dim,
                                            int64_t num_blocks, int64_t block_size, int64_t max_blocks_per_seq, int64_t ld,
                                            float softmax_scale, int64_t num_splits, cudaStream_t stream) {
-  using namespace b200;
-  using namespace b200::dtc;
   B200_CHECK_ARG(qkv && key_cache && value_cache && block_tables && seq_lens && out, "decode_attention_paged: null pointer");
   B200_CHECK_ARG(num_splits >= 1 && num_splits <= 64 && (num_splits == 1 || workspace),
                  "decode_attention_paged: bad num_splits / workspace");
@@ -509,28 +283,18 @@ extern "C" int b200_decode_attention_paged(const void* qkv, const void* key_cach
   B200_CHECK_ARG(B > 0 && num_kv_heads > 0 && num_heads % num_kv_heads == 0 && num_blocks > 0 && max_blocks_per_seq > 0 &&
                      ld % 8 == 0,
                  "decode_attention_paged: bad shape");
-  CUtensorMap tmQ, tmK, tmV;
-  int rc;
-  if ((rc = make_q_map(&tmQ, qkv, B, num_heads, ld)) != 0) return rc;
-  {
-    uint64_t dims[4] = {128, static_cast<uint64_t>(block_size), static_cast<uint64_t>(num_kv_heads),
-                        static_cast<uint64_t>(num_blocks)};
-    uint64_t strides[3] = {128 * 2, static_cast<uint64_t>(block_size) * 128 * 2,
-                           static_cast<uint64_t>(num_kv_heads) * block_size * 128 * 2};
-    uint32_t box[4] = {64, static_cast<uint32_t>(block_size), 1, 1};
-    if ((rc = encode_tmap_bf16(&tmK, key_cache, 4, dims, strides, box)) != 0) return rc;
-    if ((rc = encode_tmap_bf16(&tmV, value_cache, 4, dims, strides, box)) != 0) return rc;
-  }
-  Params p = {};
+  using namespace b200;
+  dab::Params p = {};
+  p.qkv = static_cast<const bf16*>(qkv);
+  p.kc = static_cast<const bf16*>(key_cache);
+  p.vc = static_cast<const bf16*>(value_cache);
   p.seq_lens = seq_lens;
   p.out = static_cast<bf16*>(out);
-  p.partial = num_splits > 1 ? static_cast<float*>(workspace) : nullptr;
+  p.partial = static_cast<float*>(workspace);
   p.B = static_cast<int>(B); p.nh = static_cast<int>(num_heads); p.kvh = static_cast<int>(num_kv_heads);
-  p.max_len = static_cast<int>(max_blocks_per_seq * block_size); p.nsplit = static_cast<int>(num_splits);
-  p.items = static_cast<int>(B * num_kv_heads * num_splits);
+  p.max_len = static_cast<int>(max_blocks_per_seq * block_size); p.ld = ld;
   p.scale_log2 = softmax_scale * 1.4426950408889634f;
   p.block_tables = block_tables;
-  p.max_blocks = static_cast<int>(max_blocks_per_seq);
-  p.block_size = static_cast<int>(block_size);
-  return launch<true>(tmQ, tmK, tmV, tmK, tmV, p, static_cast<int>(num_heads / num_kv_heads), out, B, num_heads, num_splits, stream);
+  p.max_blocks = static_cast<int>(max_blocks_per_seq); p.block_size = static_cast<int>(block_size);
+  return dab::launch<true>(p, static_cast<int>(num_heads / num_kv_heads), num_splits, stream);
 }

@@ -1,23 +1,18 @@
-// Causal GQA flash-attention backward on tcgen05 (head_dim 128).
+// Causal GQA flash-attention backward on Hopper tensor cores (mma.sync m16n8k16, head_dim 128).
 //
-//   inputs : q, k, v, o, do, lse            outputs: dq (fp32 accumulation buffer), dk, dv (bf16)
+//   inputs : q, k, v, o, do, lse            outputs: dq, dk, dv (bf16; fp32 accumulation buffers in the workspace)
 //   P = exp(S*scale - lse) ; dP = dO V^T ; dS = P o (dP - D) * scale, D = rowsum(dO o O)
 //   dV = P^T dO ; dK = dS^T Q ; dQ = dS K
 //
 // Replaces Paddle-core flash_attn_grad (reference: fusion_ops.py:240-246 backward of scaled_dot_product_attention;
 // wrapper shape in csrc/gpu/flash_attn_bwd.cc:22-92).
 //
-// One CTA = one (batch, q-head, 128-row kv tile); it loops over the q tiles i >= j, accumulating this head's dK/dV in
-// TMEM.  Work units are per q-head (not per kv-head) so that the 4096 units of a Llama-3 micro-batch balance over
-// 148 SMs (heaviest first); the GQA group's dK/dV partials and the dQ tiles are reduced into fp32 buffers by the TMA
-// unit (cp.reduce.async.bulk.tensor .add — no LSU atomics), then converted to bf16 by a finishing kernel.
-//   warp 0       TMA producer (K_j, V_j once; Q_i, dO_i per iteration)
-//   warp 1       MMA issuer   (5 UMMA GEMMs per iteration, operands K-major or MN-major straight from the same
-//                              swizzled tiles: Q and dO are consumed both ways)
-//   warps 2..9   two threads per q row (64 columns each; the backward needs no row reduction): P and dS from TMEM
-//                S / dP, written as bf16 to swizzled smem; dQ / dK / dV read-out
-//   TMEM: S [0,128)  dP|dQ [128,256)  dV [256,384)  dK [384,512).  dQ reuses the dP columns, so S_{i+1} = Q_{i+1} K^T is
-//   issued while the dQ_i tile is still being read out, and the Q/dO stage is released before the dQ GEMM is issued.
+// One CTA (8 warps) = one (batch, q-head, 64-row kv tile); it loops over the q tiles of BQ rows that can see the kv tile
+// (b200_set_fa_bwd_impl: 2 = 128-row q tiles, 1 = 64-row q tiles), keeping this head's dK / dV tile in registers.  Per q tile:
+//   phase 1   S and dP (BQ x 64) per warp in registers -> P, dS rounded to bf16 into shared memory
+//   phase 2   dV += P^T dO, dK += dS^T Q (operands transposed by ldmatrix.trans), dQ = dS K added to the fp32 dQ buffer
+// Work units are per q-head (not per kv-head) so that the GQA group's heads spread over the SMs; their dK/dV partials and the
+// dQ tiles are reduced into fp32 buffers with atomic adds, then converted to bf16 by a finishing kernel.
 #include "../../include/b200nlp.h"
 #include "common.cuh"
 #include "host_util.h"
@@ -25,256 +20,194 @@
 namespace b200 {
 namespace fab {
 
-constexpr int TILE_BYTES = 128 * 128 * 2;
-constexpr int HALF_BYTES = TILE_BYTES / 2;
-constexpr int NUM_THREADS = 320;   // TMA warp, MMA warp, 8 compute warps
-constexpr int STAGE_BYTES = 8 * 4096;                     // per-warp 32x32 fp32 staging for TMA reduce
-constexpr int SMEM_BYTES = 6 * TILE_BYTES + STAGE_BYTES + 256 + 1024;   // K, V, Q, dO, P, dS, staging
+constexpr int D = 128;
+constexpr int BKV = 64;
+constexpr int NUM_THREADS = 256;
 
 struct Params {
+  const bf16 *q, *k, *v, *dout;
+  int64_t ldq, ldk, ldv, lddo;
   int S, B, nh, kvh;
   float scale, scale_log2;
   const float* lse;     // [B, nh, S]  natural log
   const float* delta;   // [B, nh, S]  rowsum(dO o O)
   const int* mask_start;   // FlashMask causal-LT start rows [B, S] (see fa_fwd.cu) or nullptr
+  float* dq_acc;        // [B, S, nh, 128]
+  float* dk_acc;        // [B, S, kvh, 128]
+  float* dv_acc;
 };
 
-// TMEM accumulator (this warp's 32 lanes, fp32 columns [32*ch0, 32*(ch0+nch))) -> fp32 staging -> TMA reduce-add of
-// 32x32 boxes.  One 4 KB staging buffer per warp: the previous reduce must have finished reading it.
-__device__ __forceinline__ void reduce_out_tile(uint32_t tsrc, uint8_t* buf, const CUtensorMap* tm, int lane, int head,
-                                                int row0, int batch, int ch0) {
-  // both 32-column chunks are fetched from TMEM before the single wait (one tcgen05.ld round trip instead of two)
-  uint32_t o[2][32];
-  tmem_ld32(tsrc + ch0 * 32, o[0]);
-  tmem_ld32(tsrc + (ch0 + 1) * 32, o[1]);
-  tmem_ld_wait();
+// [rows][128] bf16 tiles: 16-byte chunks XOR-swizzled by row & 7 (as fa_fwd.cu); [rows][64] tiles (P, dS): 128-byte rows
+__device__ __forceinline__ uint32_t swz(int row, int chunk) { return static_cast<uint32_t>(row * 256 + ((chunk ^ (row & 7)) << 4)); }
+__device__ __forceinline__ uint32_t swz64(int row, int chunk) { return static_cast<uint32_t>(row * 128 + ((chunk ^ (row & 7)) << 4)); }
+
+template <int BQ, bool MASK>
+__global__ void __launch_bounds__(NUM_THREADS, 1) fa_bwd_kernel(const Params p) {
+  constexpr int RG = BQ / 16;            // phase 1: row groups of 16 q rows
+  constexpr int CH = 8 / RG;             //          column slices of the 64 kv columns
+  constexpr int NT = 8 / CH;             //          8-column n-tiles per warp
+  constexpr int QG = BQ / 16;            // dQ: row groups
+  constexpr int DH = 8 / QG;             //     d slices
+  constexpr int DTQ = 16 / DH;           //     8-column d tiles per warp
+  extern __shared__ __align__(128) uint8_t smem[];
+  const uint32_t sK = smem_u32(smem), sV = sK + BKV * 256, sQ = sV + BKV * 256, sdO = sQ + BQ * 256;
+  const uint32_t sP = sdO + BQ * 256, sdS = sP + BQ * 128;
+  float* s_lse = reinterpret_cast<float*>(smem + 2 * BKV * 256 + 2 * BQ * 256 + 2 * BQ * 128);
+  float* s_delta = s_lse + BQ;
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, tq = lane & 3;
+  const int num_kv_tiles = (p.S + BKV - 1) / BKV;
+  const int jt = static_cast<int>(blockIdx.x);   // early kv tiles see the most q rows (causal): launched first
+  const int head = blockIdx.y, batch = blockIdx.z;
+  const int kv_head = head / (p.nh / p.kvh);
+  const int kv0 = jt * BKV;
+  const size_t tok0 = static_cast<size_t>(batch) * p.S;
+  int q_lo = kv0 / BQ, q_hi = (p.S + BQ - 1) / BQ;
+  if constexpr (MASK) {   // rows at or past the last column's document end see none of this tile
+    const int last = __ldg(p.mask_start + tok0 + min(kv0 + BKV - 1, p.S - 1));
+    q_hi = min(q_hi, (last + BQ - 1) / BQ);
+  }
+  for (int i = threadIdx.x; i < BKV * 16; i += NUM_THREADS) {
+    const int r = i >> 4, ch = i & 15;
+    const bool ok = kv0 + r < p.S;
+    cp_async_16(sK + swz(r, ch), ok ? p.k + (tok0 + kv0 + r) * p.ldk + kv_head * D + ch * 8 : p.k, ok ? 16u : 0u);
+    cp_async_16(sV + swz(r, ch), ok ? p.v + (tok0 + kv0 + r) * p.ldv + kv_head * D + ch * 8 : p.v, ok ? 16u : 0u);
+  }
+  // dK / dV accumulators: warp = 16 kv rows (kg) x 64 d columns (dh)
+  const int kg = warp >> 1, dh = warp & 1;
+  float dk[8][4], dv[8][4];
 #pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    if (lane == 0) tma_store_wait_read<0>();
-    __syncwarp();
-    const uint32_t row_s = smem_u32(buf) + lane * 128;
-#pragma unroll
-    for (int c = 0; c < 8; ++c)
-      st_shared_v4(row_s + ((c ^ (lane & 7)) << 4), make_uint4(o[i][4 * c], o[i][4 * c + 1], o[i][4 * c + 2], o[i][4 * c + 3]));
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0) {
-      tma_reduce_add_4d(tm, buf, (ch0 + i) * 32, head, row0, batch);
-      tma_store_commit();
+  for (int i = 0; i < 8; ++i) dk[i][0] = dk[i][1] = dk[i][2] = dk[i][3] = dv[i][0] = dv[i][1] = dv[i][2] = dv[i][3] = 0.f;
+
+  for (int qt = q_lo; qt < q_hi; ++qt) {
+    const int q0 = qt * BQ;
+    for (int i = threadIdx.x; i < BQ * 16; i += NUM_THREADS) {
+      const int r = i >> 4, ch = i & 15;
+      const bool ok = q0 + r < p.S;
+      cp_async_16(sQ + swz(r, ch), ok ? p.q + (tok0 + q0 + r) * p.ldq + head * D + ch * 8 : p.q, ok ? 16u : 0u);
+      cp_async_16(sdO + swz(r, ch), ok ? p.dout + (tok0 + q0 + r) * p.lddo + head * D + ch * 8 : p.dout, ok ? 16u : 0u);
     }
-  }
-}
-
-template <bool MASK>     // MASK: FlashMask start rows present (kept out of the plain causal instantiation entirely)
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-fa_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-              const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO,
-              const __grid_constant__ CUtensorMap tmdQ, const __grid_constant__ CUtensorMap tmdK,
-              const __grid_constant__ CUtensorMap tmdV, const Params p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sK = smem;
-  uint8_t* sV = smem + TILE_BYTES;
-  uint8_t* sQ = smem + 2 * TILE_BYTES;
-  uint8_t* sdO = smem + 3 * TILE_BYTES;
-  uint8_t* sP = smem + 4 * TILE_BYTES;
-  uint8_t* sdS = smem + 5 * TILE_BYTES;
-  uint8_t* sStage = smem + 6 * TILE_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sStage + STAGE_BYTES);
-  uint64_t* kv_full = bars;
-  uint64_t* qdo_full = bars + 1;
-  uint64_t* qdo_empty = bars + 2;
-  uint64_t* s_full = bars + 3;
-  uint64_t* pds_full = bars + 4;
-  uint64_t* dq_full = bars + 5;
-  uint64_t* dq_empty = bars + 6;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 8);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int num_tiles = (p.S + 127) / 128;
-  const int jt = static_cast<int>(blockIdx.x);     // kv tile; tile 0 has the most work and is scheduled first
-  const int hq = blockIdx.y, batch = blockIdx.z;
-  const int kv_head = hq / (p.nh / p.kvh);
-  const int kv0 = jt * 128;
-  // q tiles jt .. hi-1: with a document mask, q tiles that start at or after the end of the last document of this kv tile
-  // see none of its columns (mask_start is non-decreasing; the diagonal tile always remains)
-  int hi = num_tiles;
-  if constexpr (MASK)
-    hi = min(num_tiles, (__ldg(p.mask_start + static_cast<size_t>(batch) * p.S + min(kv0 + 127, p.S - 1)) + 127) / 128);
-  const int n_iter = hi - jt;
-  __shared__ int s_start[MASK ? 128 : 1];          // mask start row of each column of this kv tile
-  if constexpr (MASK) {
-    if (threadIdx.x < 128) {
-      const int c = kv0 + static_cast<int>(threadIdx.x);
-      s_start[threadIdx.x] = c < p.S ? p.mask_start[static_cast<size_t>(batch) * p.S + c] : 0x7fffffff;
+    cp_async_commit();
+    for (int i = threadIdx.x; i < BQ; i += NUM_THREADS) {
+      const bool ok = q0 + i < p.S;
+      const size_t idx = (static_cast<size_t>(batch) * p.nh + head) * p.S + q0 + i;
+      s_lse[i] = ok ? __ldg(p.lse + idx) * 1.4426950408889634f : INFINITY;   // rows past S: P = 0
+      s_delta[i] = ok ? __ldg(p.delta + idx) : 0.f;
     }
-  }
+    cp_async_wait<0>();
+    __syncthreads();
 
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV); tma_prefetch_desc(&tmdO);
-    mbar_init(kv_full, 1);
-    mbar_init(qdo_full, 1);
-    mbar_init(qdo_empty, 1);
-    mbar_init(s_full, 1);
-    mbar_init(pds_full, 256);
-    mbar_init(dq_full, 1);
-    mbar_init(dq_empty, 256);
-    fence_mbar_init();
-  }
-  if (warp == 1) tmem_alloc<1>(tmem_ptr_smem, 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  const uint32_t tS = tmem_base, tdP = tmem_base + 128, tdV = tmem_base + 256, tdK = tmem_base + 384;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      mbar_arrive_expect_tx(kv_full, 2 * TILE_BYTES);
-      tma_load_4d(&tmK, kv_full, sK, 0, kv_head, kv0, batch);
-      tma_load_4d(&tmK, kv_full, sK + HALF_BYTES, 64, kv_head, kv0, batch);
-      tma_load_4d(&tmV, kv_full, sV, 0, kv_head, kv0, batch);
-      tma_load_4d(&tmV, kv_full, sV + HALF_BYTES, 64, kv_head, kv0, batch);
-      for (int n = 0; n < n_iter; ++n) {
-        const int q0 = (jt + n) * 128;
-        mbar_wait(qdo_empty, (n & 1) ^ 1u);
-        mbar_arrive_expect_tx(qdo_full, 2 * TILE_BYTES);
-        tma_load_4d(&tmQ, qdo_full, sQ, 0, hq, q0, batch);
-        tma_load_4d(&tmQ, qdo_full, sQ + HALF_BYTES, 64, hq, q0, batch);
-        tma_load_4d(&tmdO, qdo_full, sdO, 0, hq, q0, batch);
-        tma_load_4d(&tmdO, qdo_full, sdO + HALF_BYTES, 64, hq, q0, batch);
-      }
-    }
-  } else if (warp == 1) {
-    // MMA issuer: convergent code, one elected lane issues, descriptors advanced by byte offsets >> 4 (see fa_bwd2.cu)
+    // ---------------- phase 1: S = Q K^T, dP = dO V^T  (16 q rows x 8 NT kv columns per warp) ----------------
     {
-      const bool leader = elect_one();
-      const uint32_t tb = __shfl_sync(0xffffffffu, tmem_base, 0);
-      const uint32_t uS = tb, udP = tb + 128, udV = tb + 256, udK = tb + 384;
-      constexpr uint32_t id_kk = umma_idesc_bf16(128, 128, false, false);
-      constexpr uint32_t id_mm = umma_idesc_bf16(128, 128, true, true);
-      constexpr uint32_t id_km = umma_idesc_bf16(128, 128, false, true);
-      const uint32_t aK = smem_u32(sK), aV = smem_u32(sV), aQ = smem_u32(sQ), adO = smem_u32(sdO), aP = smem_u32(sP),
-                     adS = smem_u32(sdS);
-      // K-major operand (k-step = 16 of the contiguous dim) / MN-major operand (k-step = 16 rows = 2 KB) base descriptors
-      const uint64_t kQ = umma_desc_sw128(aQ, 16, 1024), kK = umma_desc_sw128(aK, 16, 1024), kdO = umma_desc_sw128(adO, 16, 1024),
-                     kV = umma_desc_sw128(aV, 16, 1024), kdS = umma_desc_sw128(adS, 16, 1024);
-      const uint64_t mP = umma_desc_sw128(aP, HALF_BYTES, 1024), mdO = umma_desc_sw128(adO, HALF_BYTES, 1024),
-                     mdS = umma_desc_sw128(adS, HALF_BYTES, 1024), mQ = umma_desc_sw128(aQ, HALF_BYTES, 1024),
-                     mK = umma_desc_sw128(aK, HALF_BYTES, 1024);
-      auto koff = [](int kk) { return static_cast<uint64_t>(((kk >> 2) * HALF_BYTES + (kk & 3) * 32) >> 4); };
-      auto moff = [](int kk) { return static_cast<uint64_t>(kk * 128); };
-      mbar_wait(kv_full, 0);
-      for (int n = 0; n < n_iter; ++n) {
-        mbar_wait(qdo_full, n & 1);
-        tc_fence_after();
-        if (leader) {
+      const int rg = warp % RG, cs = warp / RG;
+      float s[NT][4], dp[NT][4];
 #pragma unroll
-          for (int kk = 0; kk < 8; ++kk) umma_ss<1>(uS, kQ + koff(kk), kK + koff(kk), id_kk, kk > 0);      // S = Q K^T
-        }
-        mbar_wait(dq_empty, (n & 1) ^ 1u);     // dP|dQ columns drained by the previous iteration's dQ read-out
-        tc_fence_after();
-        if (leader) {
+      for (int i = 0; i < NT; ++i) s[i][0] = s[i][1] = s[i][2] = s[i][3] = dp[i][0] = dp[i][1] = dp[i][2] = dp[i][3] = 0.f;
 #pragma unroll
-          for (int kk = 0; kk < 8; ++kk) umma_ss<1>(udP, kdO + koff(kk), kV + koff(kk), id_kk, kk > 0);    // dP = dO V^T
-          umma_commit(s_full);
-        }
-        mbar_wait(pds_full, n & 1);
-        tc_fence_after();
-        const uint32_t acc0 = n > 0 ? 1u : 0u;
-        if (leader) {
+      for (int kc = 0; kc < 8; ++kc) {
+        uint32_t a[4], ad[4];
+        ldsm_x4(sQ + swz(rg * 16 + (lane & 15), kc * 2 + (lane >> 4)), a);
+        ldsm_x4(sdO + swz(rg * 16 + (lane & 15), kc * 2 + (lane >> 4)), ad);
 #pragma unroll
-          for (int kk = 0; kk < 8; ++kk) umma_ss<1>(udV, mP + moff(kk), mdO + moff(kk), id_mm, kk > 0 ? 1u : acc0);   // dV += P^T dO
-#pragma unroll
-          for (int kk = 0; kk < 8; ++kk) umma_ss<1>(udK, mdS + moff(kk), mQ + moff(kk), id_mm, kk > 0 ? 1u : acc0);   // dK += dS^T Q
-          umma_commit(qdo_empty);                // Q / dO are not read by the dQ GEMM: the next tiles can be loaded now
-#pragma unroll
-          for (int kk = 0; kk < 8; ++kk) umma_ss<1>(udP, kdS + koff(kk), mK + moff(kk), id_km, kk > 0);    // dQ = dS K
-          umma_commit(dq_full);
+        for (int np = 0; np < NT / 2; ++np) {
+          const int kr = cs * NT * 8 + np * 16 + (lane & 7) + ((lane >> 4) << 3);
+          uint32_t b[4], bv[4];
+          ldsm_x4(sK + swz(kr, kc * 2 + ((lane >> 3) & 1)), b);
+          ldsm_x4(sV + swz(kr, kc * 2 + ((lane >> 3) & 1)), bv);
+          mma_bf16_16816(s[2 * np], a, b[0], b[1]);
+          mma_bf16_16816(s[2 * np + 1], a, b[2], b[3]);
+          mma_bf16_16816(dp[2 * np], ad, bv[0], bv[1]);
+          mma_bf16_16816(dp[2 * np + 1], ad, bv[2], bv[3]);
         }
       }
-      __syncwarp();
-    }
-  } else {
-    const int quad = warp & 3;                 // TMEM lane quadrant (warps w and w+4 share the rows of a quadrant)
-    const int chalf = (warp - 2) >> 2;         // which 64 of the 128 tile columns this thread handles
-    const int r = quad * 32 + lane;
-    const uint32_t lane_off = static_cast<uint32_t>(quad * 32) << 16;
-    const uint32_t aP = smem_u32(sP), adS = smem_u32(sdS);
-    uint8_t* my_stage = sStage + (warp - 2) * 4096;
-    // row statistics of the NEXT q tile are fetched one iteration ahead (their global-load latency used to sit at the top of
-    // every iteration, in front of the s_full wait)
-    const size_t stat_base = (static_cast<size_t>(batch) * p.nh + hq) * p.S;
-    auto load_stats = [&](int q0n, float& l, float& d) {
-      const bool ok = (q0n + r) < p.S;
-      l = ok ? __ldg(p.lse + stat_base + q0n + r) : 0.f;
-      d = ok ? __ldg(p.delta + stat_base + q0n + r) : 0.f;
-    };
-    float lse_next, drow_next;
-    load_stats(jt * 128, lse_next, drow_next);
-    for (int n = 0; n < n_iter; ++n) {
-      const int qt = jt + n;
-      const int q0 = qt * 128;
-      const bool row_ok = (q0 + r) < p.S;
-      const float lse2 = lse_next * 1.4426950408889634f;
-      const float drow = drow_next;
-      if (n + 1 < n_iter) load_stats(q0 + 128, lse_next, drow_next);
-      const bool diag = (qt == jt);
-      const bool mtile = MASK && (q0 + 127 >= s_start[0]);   // some column's document ends in / before this q tile
-      const int qrow = q0 + r;
-      mbar_wait(s_full, n & 1);
-      tc_fence_after();
 #pragma unroll
-      for (int ch = chalf * 2; ch < chalf * 2 + 2; ++ch) {
-        uint32_t sv[32], dv[32];
-        tmem_ld32(tS + lane_off + ch * 32, sv);
-        tmem_ld32(tdP + lane_off + ch * 32, dv);
-        tmem_ld_wait();
-        uint32_t pp[16], dd[16];
+      for (int h = 0; h < 2; ++h) {
+        const int rl = rg * 16 + g + 8 * h, r = q0 + rl;
+        const float lse2 = s_lse[rl], dl = s_delta[rl];
 #pragma unroll
-        for (int c = 0; c < 16; ++c) {
-          const int col = ch * 32 + 2 * c;
-          float p0 = fast_exp2(fmaf(__uint_as_float(sv[2 * c]), p.scale_log2, -lse2));
-          float p1 = fast_exp2(fmaf(__uint_as_float(sv[2 * c + 1]), p.scale_log2, -lse2));
-          if (!row_ok || (diag && col > r)) p0 = 0.f;
-          if (!row_ok || (diag && col + 1 > r)) p1 = 0.f;
-          if constexpr (MASK) {
-            if (mtile && qrow >= s_start[col]) p0 = 0.f;
-            if (mtile && qrow >= s_start[col + 1]) p1 = 0.f;
+        for (int nt = 0; nt < NT; ++nt) {
+          float pv[2], dsv[2];
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int c = kv0 + cs * NT * 8 + nt * 8 + 2 * tq + e;
+            bool dead = c > r;
+            if constexpr (MASK) {
+              if (!dead && c < p.S) dead = r >= __ldg(p.mask_start + tok0 + c);
+            }
+            pv[e] = dead ? 0.f : fast_exp2(fmaf(s[nt][2 * h + e], p.scale_log2, -lse2));
+            dsv[e] = pv[e] * (dp[nt][2 * h + e] - dl) * p.scale;
           }
-          const float d0 = p0 * (__uint_as_float(dv[2 * c]) - drow) * p.scale;
-          const float d1 = p1 * (__uint_as_float(dv[2 * c + 1]) - drow) * p.scale;
-          pp[c] = pack_bf16x2(p0, p1);
-          dd[c] = pack_bf16x2(d0, d1);
-        }
-#pragma unroll
-        for (int k4 = 0; k4 < 4; ++k4) {
-          const int c16 = ch * 4 + k4;
-          const uint32_t off = (c16 >> 3) * HALF_BYTES + r * 128 + (((c16 & 7) ^ (r & 7)) << 4);
-          st_shared_v4(aP + off, make_uint4(pp[4 * k4], pp[4 * k4 + 1], pp[4 * k4 + 2], pp[4 * k4 + 3]));
-          st_shared_v4(adS + off, make_uint4(dd[4 * k4], dd[4 * k4 + 1], dd[4 * k4 + 2], dd[4 * k4 + 3]));
+          const int cc = cs * NT + nt;     // 8-column chunk index within the 64 kv columns
+          asm volatile("st.shared.b32 [%0], %1;" ::"r"(sP + swz64(rl, cc) + tq * 4), "r"(pack_bf16x2(pv[0], pv[1])) : "memory");
+          asm volatile("st.shared.b32 [%0], %1;" ::"r"(sdS + swz64(rl, cc) + tq * 4), "r"(pack_bf16x2(dsv[0], dsv[1])) : "memory");
         }
       }
-      fence_proxy_async_smem();
-      tc_fence_before();
-      mbar_arrive(pds_full);
-      // dQ tile read-out: TMEM -> fp32 staging -> TMA reduce-add into the fp32 dQ buffer (rows >= S are clipped)
-      mbar_wait(dq_full, n & 1);
-      tc_fence_after();
-      reduce_out_tile(tdP + lane_off, my_stage, &tmdQ, lane, hq, q0 + quad * 32, batch, chalf * 2);
-      tc_fence_before();
-      mbar_arrive(dq_empty);
     }
-    // epilogue: this head's dK / dV partials -> fp32 reduce-add (the GQA group's heads sum in L2)
-    reduce_out_tile(tdK + lane_off, my_stage, &tmdK, lane, kv_head, kv0 + quad * 32, batch, chalf * 2);
-    reduce_out_tile(tdV + lane_off, my_stage, &tmdV, lane, kv_head, kv0 + quad * 32, batch, chalf * 2);
-    if (lane == 0) tma_store_wait<0>();
+    __syncthreads();
+
+    // ---------------- phase 2: dV += P^T dO, dK += dS^T Q, dQ += dS K ----------------
+#pragma unroll
+    for (int qc = 0; qc < BQ / 16; ++qc) {
+      uint32_t ap[4], as[4];
+      const int pr = qc * 16 + (lane & 7) + ((lane >> 4) << 3), pc = kg * 2 + ((lane >> 3) & 1);
+      ldsm_x4_t(sP + swz64(pr, pc), ap);
+      ldsm_x4_t(sdS + swz64(pr, pc), as);
+#pragma unroll
+      for (int dp2 = 0; dp2 < 4; ++dp2) {
+        const int br = qc * 16 + (lane & 7) + ((lane >> 3) & 1) * 8, bc = dh * 8 + dp2 * 2 + (lane >> 4);
+        uint32_t bo[4], bq[4];
+        ldsm_x4_t(sdO + swz(br, bc), bo);
+        ldsm_x4_t(sQ + swz(br, bc), bq);
+        mma_bf16_16816(dv[2 * dp2], ap, bo[0], bo[1]);
+        mma_bf16_16816(dv[2 * dp2 + 1], ap, bo[2], bo[3]);
+        mma_bf16_16816(dk[2 * dp2], as, bq[0], bq[1]);
+        mma_bf16_16816(dk[2 * dp2 + 1], as, bq[2], bq[3]);
+      }
+    }
+    {
+      const int qg = warp % QG, dsl = warp / QG;
+      float dq[DTQ][4];
+#pragma unroll
+      for (int i = 0; i < DTQ; ++i) dq[i][0] = dq[i][1] = dq[i][2] = dq[i][3] = 0.f;
+#pragma unroll
+      for (int kc = 0; kc < BKV / 16; ++kc) {
+        uint32_t a[4];
+        ldsm_x4(sdS + swz64(qg * 16 + (lane & 15), kc * 2 + (lane >> 4)), a);
+#pragma unroll
+        for (int dp2 = 0; dp2 < DTQ / 2; ++dp2) {
+          uint32_t b[4];
+          ldsm_x4_t(sK + swz(kc * 16 + (lane & 7) + ((lane >> 3) & 1) * 8, dsl * (DTQ) + dp2 * 2 + (lane >> 4)), b);
+          mma_bf16_16816(dq[2 * dp2], a, b[0], b[1]);
+          mma_bf16_16816(dq[2 * dp2 + 1], a, b[2], b[3]);
+        }
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r = q0 + qg * 16 + g + 8 * h;
+        if (r >= p.S) continue;
+        float* dst = p.dq_acc + ((tok0 + r) * p.nh + head) * D + dsl * DTQ * 8 + 2 * tq;
+#pragma unroll
+        for (int dt = 0; dt < DTQ; ++dt) {
+          atomicAdd(dst + dt * 8, dq[dt][2 * h]);
+          atomicAdd(dst + dt * 8 + 1, dq[dt][2 * h + 1]);
+        }
+      }
+    }
+    __syncthreads();   // Q, dO, P, dS are overwritten by the next q tile
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<1>(tmem_base, 512);
+  // this head's dK / dV partials -> the kv head's fp32 buffers (the GQA group's heads add up there)
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int r = kv0 + kg * 16 + g + 8 * h;
+    if (r >= p.S) continue;
+    const size_t off = ((tok0 + r) * p.kvh + kv_head) * D + dh * 64 + 2 * tq;
+#pragma unroll
+    for (int dt = 0; dt < 8; ++dt) {
+      atomicAdd(p.dk_acc + off + dt * 8, dk[dt][2 * h]);
+      atomicAdd(p.dk_acc + off + dt * 8 + 1, dk[dt][2 * h + 1]);
+      atomicAdd(p.dv_acc + off + dt * 8, dv[dt][2 * h]);
+      atomicAdd(p.dv_acc + off + dt * 8 + 1, dv[dt][2 * h + 1]);
+    }
   }
 }
 
@@ -323,26 +256,29 @@ __global__ void fa_bwd_dq_finish_kernel(const float* __restrict__ acc, bf16* __r
   }
 }
 
-static int make_map(CUtensorMap* tm, const void* base, int64_t B, int64_t S, int64_t heads, int64_t ld) {
-  uint64_t dims[4] = {128, static_cast<uint64_t>(heads), static_cast<uint64_t>(S), static_cast<uint64_t>(B)};
-  uint64_t strides[3] = {128 * 2, static_cast<uint64_t>(ld) * 2, static_cast<uint64_t>(S) * ld * 2};
-  uint32_t box[4] = {64, 1, 128, 1};
-  return encode_tmap_bf16(tm, base, 4, dims, strides, box);
-}
-// fp32 accumulation buffer [B, S, heads, 128] contiguous; 32x32 boxes for the per-warp TMA reduce-add.
-static int make_acc_map(CUtensorMap* tm, const void* base, int64_t B, int64_t S, int64_t heads) {
-  uint64_t dims[4] = {128, static_cast<uint64_t>(heads), static_cast<uint64_t>(S), static_cast<uint64_t>(B)};
-  uint64_t strides[3] = {128 * 4, static_cast<uint64_t>(heads) * 128 * 4, static_cast<uint64_t>(S) * heads * 128 * 4};
-  uint32_t box[4] = {32, 1, 32, 1};
-  return encode_tmap_f32(tm, base, 4, dims, strides, box);
+template <int BQ, bool MASK>
+static int launch(const Params& p, cudaStream_t stream) {
+  constexpr int SMEM = 2 * BKV * 256 + 2 * BQ * 256 + 2 * BQ * 128 + 2 * BQ * 4;
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(fa_bwd_kernel<BQ, MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
+    if (e != cudaSuccess) {
+      set_last_error("fa_bwd smem attr: %s", cudaGetErrorString(e));
+      return static_cast<int>(e);
+    }
+    attr_set = true;
+  }
+  dim3 grid(static_cast<unsigned>((p.S + BKV - 1) / BKV), static_cast<unsigned>(p.nh), static_cast<unsigned>(p.B));
+  fa_bwd_kernel<BQ, MASK><<<grid, NUM_THREADS, SMEM, stream>>>(p);
+  return check_launch("fa_bwd");
 }
 
 }  // namespace fab
 }  // namespace b200
 
 extern "C" int64_t b200_fa_bwd_workspace_bytes(int64_t B, int64_t S, int64_t num_heads, int64_t head_dim) {
-  // fp32 dQ accumulation buffer + fp32 dK/dV accumulation buffers (at most num_heads wide) + per-row statistics; sized for both
-  // kernel generations: fa_bwd2.cu pads the sequence to a multiple of 64 and keeps two floats of statistics per row
+  // fp32 dQ accumulation buffer + fp32 dK/dV accumulation buffers (at most num_heads wide) + per-row statistics (the sequence padded
+  // to a multiple of 64, two floats per row)
   const int64_t Spad = (S + 63) / 64 * 64;
   return 3 * B * Spad * num_heads * head_dim * 4 + B * num_heads * Spad * 8;
 }
@@ -369,9 +305,6 @@ extern "C" int b200_fa_bwd_flashmask(const void* q, const void* k, const void* v
   B200_CHECK_ARG(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0 && lddo % 8 == 0 && lddq % 8 == 0 &&
                      lddk % 8 == 0 && lddv % 8 == 0,
                  "fa_bwd: token strides must be multiples of 8");
-  if (fa_bwd_impl() == 2)    // transposed, software-pipelined kernel (fa_bwd2.cu); plain causal or FlashMask start rows
-    return launch_fa_bwd2(q, k, v, o, dout, lse, mask_start_rows, dq, dk, dv, workspace, B, S, num_heads, num_kv_heads, ldq, ldk, ldv, ldo, lddo,
-                          lddq, lddk, lddv, softmax_scale, stream);
   float* dq_acc = static_cast<float*>(workspace);
   float* dk_acc = dq_acc + B * S * num_heads * 128;
   float* dv_acc = dk_acc + B * S * num_kv_heads * 128;
@@ -389,37 +322,20 @@ extern "C" int b200_fa_bwd_flashmask(const void* q, const void* k, const void* v
     int rc = check_launch("fa_bwd(delta)");
     if (rc) return rc;
   }
-  CUtensorMap tmQ, tmK, tmV, tmdO, tmdQ, tmdK, tmdV;
-  int rc;
-  if ((rc = make_map(&tmQ, q, B, S, num_heads, ldq)) != 0) return rc;
-  if ((rc = make_map(&tmK, k, B, S, num_kv_heads, ldk)) != 0) return rc;
-  if ((rc = make_map(&tmV, v, B, S, num_kv_heads, ldv)) != 0) return rc;
-  if ((rc = make_map(&tmdO, dout, B, S, num_heads, lddo)) != 0) return rc;
-  if ((rc = make_acc_map(&tmdQ, dq_acc, B, S, num_heads)) != 0) return rc;
-  if ((rc = make_acc_map(&tmdK, dk_acc, B, S, num_kv_heads)) != 0) return rc;
-  if ((rc = make_acc_map(&tmdV, dv_acc, B, S, num_kv_heads)) != 0) return rc;
-  static bool attr_set = false;
-  if (!attr_set) {
-    e = cudaFuncSetAttribute(fa_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(fa_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-    if (e != cudaSuccess) {
-      set_last_error("fa_bwd smem attr: %s", cudaGetErrorString(e));
-      return static_cast<int>(e);
-    }
-    attr_set = true;
-  }
   Params p;
+  p.q = static_cast<const bf16*>(q); p.k = static_cast<const bf16*>(k); p.v = static_cast<const bf16*>(v);
+  p.dout = static_cast<const bf16*>(dout);
+  p.ldq = ldq; p.ldk = ldk; p.ldv = ldv; p.lddo = lddo;
   p.S = (int)S; p.B = (int)B; p.nh = (int)num_heads; p.kvh = (int)num_kv_heads;
   p.scale = softmax_scale;
   p.scale_log2 = softmax_scale * 1.4426950408889634f;
   p.lse = lse; p.delta = delta;
   p.mask_start = mask_start_rows;
-  dim3 grid(static_cast<unsigned>((S + 127) / 128), static_cast<unsigned>(num_heads), static_cast<unsigned>(B));
-  if (mask_start_rows != nullptr)
-    fa_bwd_kernel<true><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(tmQ, tmK, tmV, tmdO, tmdQ, tmdK, tmdV, p);
-  else
-    fa_bwd_kernel<false><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(tmQ, tmK, tmV, tmdO, tmdQ, tmdK, tmdV, p);
-  if ((rc = check_launch("fa_bwd")) != 0) return rc;
+  p.dq_acc = dq_acc; p.dk_acc = dk_acc; p.dv_acc = dv_acc;
+  int rc;
+  if (fa_bwd_impl() == 1) rc = mask_start_rows ? launch<64, true>(p, stream) : launch<64, false>(p, stream);
+  else rc = mask_start_rows ? launch<128, true>(p, stream) : launch<128, false>(p, stream);
+  if (rc) return rc;
   {
     const int64_t tokens = B * S;
     const int width = static_cast<int>(num_heads * 128);

@@ -1,4 +1,4 @@
-// Causal GQA flash-attention forward on tcgen05 (head_dim 128).
+// Causal GQA flash-attention forward on Hopper tensor cores (mma.sync m16n8k16, head_dim 128).
 //
 //   O = softmax(Q K^T / sqrt(d) + causal) V ,  LSE saved for the backward.
 //   q [b, s, nh, d], k/v [b, s, kvh, d] (arbitrary token stride: they are views into the packed QKV projection),
@@ -8,14 +8,10 @@
 // (paddlenlp/transformers/llama/fusion_ops.py:240-246; eager math llama/modeling.py:244-301).
 // Rounding points: S and softmax in fp32 (scale applied to S), P rounded to bf16 before P@V, O rounded to bf16.
 //
-// One CTA = one (batch, q-head, 128-row q tile); kv tiles 0..i (square 128x128 causal tiles).
-//   warp 0        TMA producer: Q once, K and V through 2-stage rings (128B swizzle)
-//   warp 1        MMA issuer:   S[j&1] = Q K_j^T (UMMA 128x128x16 x8) ; O += P_j V_j (V consumed MN-major)
-//   warps 2..9    softmax:      two threads per q row (TMEM lane), 64 score columns each (row max exchanged through
-//                               smem); S read with tcgen05.ld, online softmax with lazy rescaling of the TMEM-resident
-//                               O accumulator, P written to swizzled smem as bf16
-//   TMEM: S0 [0,128) S1 [128,256) O [256,384).  QK_{j+1} is issued before P_j V_j so the tensor pipe works on the
-//   next scores while the softmax warps exponentiate the current ones.
+// One CTA = one (batch, q-head, BQ-row q tile), NW warps of 16 q rows each (BQ = 16 NW; b200_set_fa_fwd_impl: 2 = 128 rows,
+// 1 = 64 rows).  K/V tiles of 64 rows are double-buffered in 128-byte-row-swizzled shared memory with cp.async; Q stays in
+// registers as mma A fragments; S, P and the O accumulator never leave the registers of the warp that owns the rows.
+// Three instantiations: plain causal, FlashMask start rows, and the paged-cache prefill of append_attention.
 #include "../../include/b200nlp.h"
 #include "common.cuh"
 #include "host_util.h"
@@ -24,307 +20,254 @@ namespace b200 {
 namespace fa {
 
 constexpr int D = 128;       // head dim
-constexpr int BQ = 128;      // q rows per CTA
-constexpr int BKV = 128;     // kv rows per tile
-constexpr int TILE_BYTES = 128 * 128 * 2;   // 32 KB (two 64-column halves of 16 KB)
-constexpr int HALF_BYTES = TILE_BYTES / 2;
-constexpr int NUM_THREADS = 320;   // TMA warp, MMA warp, 8 softmax warps
-constexpr int SMEM_BYTES = 6 * TILE_BYTES + 256 + 3 * 1024 + 1024;   // Q, K0, K1, V0, V1, P + barriers + row-stat exchange + align slack
-constexpr float RESCALE_THRESHOLD = 8.f;                  // log2 units
+constexpr int BKV = 64;      // kv rows per tile
+constexpr int KV_TILE_BYTES = BKV * D * 2;   // 16 KB
+
+enum Mode { DENSE = 0, MASK = 1, PAGED = 2 };
 
 struct Params {
+  const bf16* q;
+  const bf16* k;
+  const bf16* v;
+  bf16* o;
+  float* lse;         // [B, nh, S] (DENSE / MASK)
+  int64_t ldq, ldk, ldv, ldo;
   int S, B, nh, kvh;
   float scale_log2;   // (1/sqrt(d)) * log2(e)
-  float* lse;         // [B, nh, S]
   // FlashMask, causal lower-triangular form (fusion_ops.py:218-231 -> F.flashmask_attention(startend_row_indices, causal=True)):
   // mask_start[b, c] = first query row that may NOT see key column c (the end of c's packed document, llm/utils/data.py:
-  // 200-204 + zero_padding_dataset.py:84-86); non-decreasing in c.  nullptr = plain causal.
+  // 200-204 + zero_padding_dataset.py:84-86); non-decreasing in c and > c.  Row i sees column c iff c <= i < mask_start[b, c].
   const int* mask_start;
+  // PAGED (prefill half of append_attention, csrc/gpu/append_attention.cu:428-851): sequence b contributes seq_this[b] new query
+  // rows (token rows cu_q[b] .. of the packed projection) at absolute positions seq_dec[b] + i and attends to cache positions
+  // [0, seq_dec[b] + i] of its pages; key/value caches [num_blocks, kvh, block_size, 128]
+  const int* cu_q;
+  const int* seq_dec;
+  const int* seq_this;
+  const int* seq_enc;
+  const int* block_tables;
+  int max_blocks, block_size;
 };
 
-template <bool MASK>     // MASK: FlashMask start rows present (kept out of the plain causal instantiation entirely)
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-fa_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-              const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmO, const Params p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQ = smem;
-  uint8_t* sK = smem + TILE_BYTES;          // 2 stages
-  uint8_t* sV = smem + 3 * TILE_BYTES;      // 2 stages
-  uint8_t* sP = smem + 5 * TILE_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 6 * TILE_BYTES);
-  uint64_t* q_full = bars;          // [1]
-  uint64_t* k_full = bars + 1;      // [2]
-  uint64_t* k_empty = bars + 3;     // [2]
-  uint64_t* v_full = bars + 5;      // [2]
-  uint64_t* v_empty = bars + 7;     // [2]
-  uint64_t* s_full = bars + 9;      // [2]
-  uint64_t* s_empty = bars + 11;    // [2]
-  uint64_t* p_full = bars + 13;     // [1]
-  uint64_t* pv_done = bars + 14;    // [1]
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 15);
-  float* s_stat = reinterpret_cast<float*>(smem + 6 * TILE_BYTES + 256);   // [3][2][128]: two max buffers + row sums
+// byte offset of 16-byte chunk `chunk` of row `row` in a [rows][128] bf16 tile (chunks XOR-swizzled by row & 7: conflict-free
+// ldmatrix for both the plain and the transposed reads)
+__device__ __forceinline__ uint32_t swz(int row, int chunk) { return static_cast<uint32_t>(row * 256 + ((chunk ^ (row & 7)) << 4)); }
+
+template <int NW, int MODE>
+__global__ void __launch_bounds__(NW * 32, 1) fa_fwd_kernel(const Params p) {
+  constexpr int BQ = 16 * NW;
+  extern __shared__ __align__(128) uint8_t smem[];
+  const uint32_t sQ = smem_u32(smem);
+  const uint32_t sK = sQ + BQ * 256;              // [2] K tiles
+  const uint32_t sV = sK + 2 * KV_TILE_BYTES;     // [2] V tiles
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int num_q_tiles = (p.S + BQ - 1) / BQ;
-  const int qt = num_q_tiles - 1 - static_cast<int>(blockIdx.x);   // heavy tiles first
   const int head = blockIdx.y, batch = blockIdx.z;
   const int kv_head = head / (p.nh / p.kvh);
+  int n_rows = p.S, pos0 = 0, tok0 = batch * p.S;
+  if constexpr (MODE == PAGED) {
+    n_rows = p.seq_this[batch];
+    // decode rows (one new token on top of a cache, no prompt) belong to the decode kernel; idle slots to nobody
+    if (n_rows <= 0 || (n_rows == 1 && p.seq_enc[batch] <= 0)) return;
+    pos0 = p.seq_dec[batch];
+    tok0 = p.cu_q[batch];
+  }
+  const int qt = (n_rows + BQ - 1) / BQ - 1 - static_cast<int>(blockIdx.x);   // heavy tiles first
+  if (qt < 0) return;
   const int q0 = qt * BQ;
-  // kv tiles j_lo .. qt.  With a document mask the leading tiles whose every column belongs to a document that ended at or
-  // before this q tile are skipped (mask_start is non-decreasing, so they form a prefix; the diagonal tile is never empty).
+  const int kv_total = pos0 + n_rows;                             // kv positions that exist
+  const int kv_end = pos0 + min(q0 + BQ, n_rows);                 // kv positions the tile's last row can see
+  const int n_kv = (kv_end + BKV - 1) / BKV;
+  // With a document mask the leading kv tiles whose every column belongs to a document that ended at or before this q tile
+  // are skipped (mask_start is non-decreasing, so they form a prefix; the diagonal tile is never empty).
   int j_lo = 0;
-  if constexpr (MASK) {
+  if constexpr (MODE == MASK) {
     const int* ms = p.mask_start + static_cast<size_t>(batch) * p.S;
-    while (j_lo < qt && __ldg(ms + min(j_lo * BKV + BKV - 1, p.S - 1)) <= q0) ++j_lo;
+    while (j_lo < n_kv - 1 && __ldg(ms + min(j_lo * BKV + BKV - 1, p.S - 1)) <= q0) ++j_lo;
   }
-  const int n_kv = qt + 1 - j_lo;
 
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV); tma_prefetch_desc(&tmO);
-    mbar_init(q_full, 1);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&k_full[i], 1); mbar_init(&k_empty[i], 1);
-      mbar_init(&v_full[i], 1); mbar_init(&v_empty[i], 1);
-      mbar_init(&s_full[i], 1); mbar_init(&s_empty[i], 8);
+  auto kv_row = [&](const bf16* base, int64_t ld, int c) -> const bf16* {
+    if constexpr (MODE == PAGED) {
+      const int page = __ldg(p.block_tables + static_cast<size_t>(batch) * p.max_blocks + c / p.block_size);
+      return base + ((static_cast<size_t>(page) * p.kvh + kv_head) * p.block_size + c % p.block_size) * D;
+    } else {
+      return base + static_cast<size_t>(tok0 + c) * ld + kv_head * D;
     }
-    mbar_init(p_full, 256);
-    mbar_init(pv_done, 1);
-    fence_mbar_init();
+  };
+  auto load_kv = [&](int j, int buf) {
+    for (int i = threadIdx.x; i < BKV * 16; i += NW * 32) {
+      const int r = i >> 4, ch = i & 15, c = j * BKV + r;
+      const bool ok = c < kv_total;
+      cp_async_16(sK + buf * KV_TILE_BYTES + swz(r, ch), ok ? kv_row(p.k, p.ldk, c) + ch * 8 : p.k, ok ? 16u : 0u);
+      cp_async_16(sV + buf * KV_TILE_BYTES + swz(r, ch), ok ? kv_row(p.v, p.ldv, c) + ch * 8 : p.v, ok ? 16u : 0u);
+    }
+  };
+  for (int i = threadIdx.x; i < BQ * 16; i += NW * 32) {
+    const int r = i >> 4, ch = i & 15;
+    const bool ok = q0 + r < n_rows;
+    cp_async_16(sQ + swz(r, ch), ok ? p.q + static_cast<size_t>(tok0 + q0 + r) * p.ldq + head * D + ch * 8 : p.q, ok ? 16u : 0u);
   }
-  if (warp == 1) tmem_alloc<1>(tmem_ptr_smem, 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  const uint32_t tS0 = tmem_base, tO = tmem_base + 256;
+  load_kv(j_lo, 0);
+  cp_async_commit();
 
-  if (warp == 0) {
-    // ------------------------------- TMA producer -------------------------------
-    if (lane == 0) {
-      mbar_arrive_expect_tx(q_full, TILE_BYTES);
-      tma_load_4d(&tmQ, q_full, sQ, 0, head, q0, batch);
-      tma_load_4d(&tmQ, q_full, sQ + HALF_BYTES, 64, head, q0, batch);
-      for (int j = 0; j < n_kv; ++j) {
-        const int st = j & 1;
-        const uint32_t ph = (j >> 1) & 1;
-        mbar_wait(&k_empty[st], ph ^ 1u);
-        mbar_arrive_expect_tx(&k_full[st], TILE_BYTES);
-        tma_load_4d(&tmK, &k_full[st], sK + st * TILE_BYTES, 0, kv_head, (j_lo + j) * BKV, batch);
-        tma_load_4d(&tmK, &k_full[st], sK + st * TILE_BYTES + HALF_BYTES, 64, kv_head, (j_lo + j) * BKV, batch);
-        mbar_wait(&v_empty[st], ph ^ 1u);
-        mbar_arrive_expect_tx(&v_full[st], TILE_BYTES);
-        tma_load_4d(&tmV, &v_full[st], sV + st * TILE_BYTES, 0, kv_head, (j_lo + j) * BKV, batch);
-        tma_load_4d(&tmV, &v_full[st], sV + st * TILE_BYTES + HALF_BYTES, 64, kv_head, (j_lo + j) * BKV, batch);
+  const int g = lane >> 2, tq = lane & 3;
+  const int row_a = q0 + warp * 16 + g;                 // tile rows of this thread: row_a and row_a + 8
+  float o[16][4];
+#pragma unroll
+  for (int i = 0; i < 16; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  uint32_t qf[8][4];
+
+  for (int j = j_lo; j < n_kv; ++j) {
+    const int buf = (j - j_lo) & 1;
+    if (j + 1 < n_kv) {
+      load_kv(j + 1, buf ^ 1);
+      cp_async_commit();
+      cp_async_wait<1>();
+    } else {
+      cp_async_wait<0>();
+    }
+    __syncthreads();
+    if (j == j_lo) {
+#pragma unroll
+      for (int kc = 0; kc < 8; ++kc) ldsm_x4(sQ + swz(warp * 16 + (lane & 15), kc * 2 + (lane >> 4)), qf[kc]);
+    }
+    // S = Q K^T   (16 rows x 64 kv columns per warp)
+    float s[8][4];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f;
+    const uint32_t kb = sK + buf * KV_TILE_BYTES, vb = sV + buf * KV_TILE_BYTES;
+#pragma unroll
+    for (int kc = 0; kc < 8; ++kc) {
+#pragma unroll
+      for (int np = 0; np < 4; ++np) {
+        uint32_t b[4];
+        ldsm_x4(kb + swz(np * 16 + (lane & 7) + ((lane >> 4) << 3), kc * 2 + ((lane >> 3) & 1)), b);
+        mma_bf16_16816(s[2 * np], qf[kc], b[0], b[1]);
+        mma_bf16_16816(s[2 * np + 1], qf[kc], b[2], b[3]);
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------- MMA issuer -------------------------------
-    // convergent code, one elected lane issues, descriptors advanced by adding byte offsets >> 4 (see fa_fwd2.cu: inside
-    // `if (lane == 0)` every UTCHMMA costs ~19 SASS instructions of descriptor rebuilding and R2UR traffic)
-    {
-      const bool leader = elect_one();
-      const uint32_t tb = __shfl_sync(0xffffffffu, tmem_base, 0);
-      const uint32_t uS0 = tb, uO = tb + 256;
-      constexpr uint32_t idesc_qk = umma_idesc_bf16(128, 128, false, false);   // A=Q K-major, B=K K-major
-      constexpr uint32_t idesc_pv = umma_idesc_bf16(128, 128, false, true);    // A=P K-major, B=V MN-major
-      const uint32_t sK_a0 = smem_u32(sK), sV_a0 = smem_u32(sV);
-      const uint64_t dQ = umma_desc_sw128(smem_u32(sQ), 16, 1024), dP = umma_desc_sw128(smem_u32(sP), 16, 1024);
-      auto koff = [](int kk) { return static_cast<uint64_t>(((kk >> 2) * HALF_BYTES + (kk & 3) * 32) >> 4); };
-      auto issue_qk = [&](int j) {
-        const int st = j & 1;
-        const uint64_t dK = umma_desc_sw128(sK_a0 + st * TILE_BYTES, 16, 1024);
-        const uint32_t tS = uS0 + static_cast<uint32_t>((j & 1) * 128);
-        if (leader) {
+    // masks: causal (kv position > query position), FlashMask (query row >= mask_start of the column)
+    const int c_base = j * BKV + 2 * tq;
+    const bool need_causal = j * BKV + BKV - 1 > pos0 + q0 + warp * 16;
+    bool need_mask = false;
+    if constexpr (MODE == MASK) need_mask = __ldg(p.mask_start + static_cast<size_t>(batch) * p.S + j * BKV) <= q0 + BQ - 1;
+    if (need_causal || need_mask) {
 #pragma unroll
-          for (int kk = 0; kk < D / 16; ++kk) umma_ss<1>(tS, dQ + koff(kk), dK + koff(kk), idesc_qk, kk > 0 ? 1u : 0u);
-          umma_commit(&k_empty[st]);
-          umma_commit(&s_full[j & 1]);
-        }
-      };
-      mbar_wait(q_full, 0);
-      mbar_wait(&k_full[0], 0);
-      tc_fence_after();
-      issue_qk(0);
-      for (int j = 0; j < n_kv; ++j) {
-        if (j + 1 < n_kv) {
-          const int jn = j + 1;
-          const uint32_t n = jn >> 1;   // use index of S buffer (jn & 1)
-          mbar_wait(&s_empty[jn & 1], (n & 1u) ^ 1u);
-          mbar_wait(&k_full[jn & 1], n & 1u);
-          tc_fence_after();
-          issue_qk(jn);
-        }
-        const int st = j & 1;
-        mbar_wait(&v_full[st], (j >> 1) & 1);
-        mbar_wait(p_full, j & 1);
-        tc_fence_after();
-        const uint64_t dV = umma_desc_sw128(sV_a0 + st * TILE_BYTES, HALF_BYTES, 1024);
-        const uint32_t acc0 = j > 0 ? 1u : 0u;
-        if (leader) {
+      for (int nt = 0; nt < 8; ++nt)
 #pragma unroll
-          for (int kk = 0; kk < BKV / 16; ++kk)     // P: kv along K (K-major);  V: 16 kv rows = 2 KB per k-step (MN-major)
-            umma_ss<1>(uO, dP + koff(kk), dV + static_cast<uint64_t>(kk * 128), idesc_pv, kk > 0 ? 1u : acc0);
-          umma_commit(&v_empty[st]);
-          umma_commit(pv_done);
-        }
-      }
-      __syncwarp();
-    }
-  } else {
-    // ------------------------------- softmax / epilogue -------------------------------
-    const int quad = warp & 3;                            // TMEM lane quadrant (warps w and w+4 share its rows)
-    const int chalf = (warp - 2) >> 2;                    // score / output columns [64*chalf, 64*chalf + 64)
-    const int r = quad * 32 + lane;                       // q row within the tile == TMEM lane
-    const uint32_t lane_off = static_cast<uint32_t>(quad * 32) << 16;
-    float m_used = -INFINITY, l = 0.f;                    // l: partial row sum over this thread's columns
-    const uint32_t sP_a = smem_u32(sP);
-    for (int j = 0; j < n_kv; ++j) {
-      const int sb = j & 1;
-      mbar_wait(&s_full[sb], (j >> 1) & 1);
-      tc_fence_after();
-      uint32_t sv[64];
-      {
-        uint32_t(*c)[32] = reinterpret_cast<uint32_t(*)[32]>(sv);
-        const uint32_t ta = tS0 + lane_off + static_cast<uint32_t>(sb * 128 + chalf * 64);
-        tmem_ld32(ta, c[0]); tmem_ld32(ta + 32, c[1]);
-        tmem_ld_wait();
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&s_empty[sb]);
-      // causal mask on the diagonal tile, row max over this thread's 64 columns (raw scores; the positive softmax
-      // scale is folded into the exponent below as one FFMA per element)
-      float rowmax = -INFINITY;
-      const int jg = j_lo + j;                            // global kv tile index
-      const bool diag = (jg == qt);
-      if (diag) {
-#pragma unroll
-        for (int c = 0; c < 64; ++c)
-          if ((chalf * 64 + c) > r) sv[c] = 0xff800000u;   // -inf
-      }
-      if constexpr (MASK) {
-        const int* ms = p.mask_start + static_cast<size_t>(batch) * p.S + jg * BKV;
-        if (__ldg(ms) <= q0 + BQ - 1) {                   // some document in this kv tile ends inside / before the q tile
-          const int row = q0 + r;
-          const int cmax = p.S - jg * BKV - chalf * 64;   // columns of this half that exist
-#pragma unroll                                            // full unroll: sv[] must stay in registers
-          for (int c = 0; c < 64; ++c) {
-            const int start = __ldg(ms + chalf * 64 + min(c, cmax - 1));
-            if (c < cmax && row >= start) sv[c] = 0xff800000u;
+        for (int e = 0; e < 4; ++e) {
+          const int c = c_base + nt * 8 + (e & 1);
+          const int r = row_a + (e >> 1) * 8;
+          bool dead = c > pos0 + r;
+          if constexpr (MODE == MASK) {
+            if (!dead && c < p.S) dead = r >= __ldg(p.mask_start + static_cast<size_t>(batch) * p.S + c);
           }
+          if (dead) s[nt][e] = -INFINITY;
         }
-      }
+    }
+    // online softmax (two rows per thread; a row's 64 columns live in the 4 threads of a quad)
+    uint32_t pa[4][4];
 #pragma unroll
-      for (int c = 0; c < 64; ++c) rowmax = fmaxf(rowmax, __uint_as_float(sv[c]));
-      rowmax *= p.scale_log2;
-      // exchange with the thread that owns the other 64 columns of this row
-      s_stat[(sb * 2 + chalf) * 128 + r] = rowmax;
-      named_bar_sync(2, 256);
-      rowmax = fmaxf(rowmax, s_stat[(sb * 2 + (chalf ^ 1)) * 128 + r]);
-      bool rescale = false;
-      float factor = 1.f;
-      if (j == 0) {
-        m_used = rowmax;
-      } else {
-        const bool need = rowmax > m_used + RESCALE_THRESHOLD;
-        rescale = __any_sync(0xffffffffu, need);          // identical in both warps of the row pair
-        if (need) {
-          factor = fast_exp2(m_used - rowmax);
-          l *= factor;
-          m_used = rowmax;
-        }
-      }
-      uint32_t pk[32];
+    for (int h = 0; h < 2; ++h) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int nt = 0; nt < 8; ++nt) mx = fmaxf(mx, fmaxf(s[nt][2 * h], s[nt][2 * h + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m[h], mx * p.scale_log2);
+      const float corr = (m[h] == -INFINITY) ? 0.f : fast_exp2(m[h] - m_new);
+      m[h] = m_new;
+      // a row can be fully masked in its first tiles (documents): exp2(-inf - (-inf)) must not be evaluated
+      const float neg_m = (m_new == -INFINITY) ? 0.f : -m_new;
       float rs = 0.f;
-      // with documents a row can be fully masked in its first tiles: exp2(-inf - (-inf)) must not be evaluated
-      const float neg_m = (MASK && m_used == -INFINITY) ? 0.f : -m_used;
 #pragma unroll
-      for (int c = 0; c < 32; ++c) {
-        const float p0 = fast_exp2(fmaf(__uint_as_float(sv[2 * c]), p.scale_log2, neg_m));
-        const float p1 = fast_exp2(fmaf(__uint_as_float(sv[2 * c + 1]), p.scale_log2, neg_m));
+      for (int nt = 0; nt < 8; ++nt) {
+        const float p0 = fast_exp2(fmaf(s[nt][2 * h], p.scale_log2, neg_m));
+        const float p1 = fast_exp2(fmaf(s[nt][2 * h + 1], p.scale_log2, neg_m));
         rs += p0 + p1;
-        pk[c] = pack_bf16x2(p0, p1);
+        pa[nt >> 1][(nt & 1) * 2 + h] = pack_bf16x2(p0, p1);
       }
-      l += rs;
-      if (j > 0) {
-        mbar_wait(pv_done, (j - 1) & 1);   // P buffer free, O accumulator quiescent
-        tc_fence_after();
-        if (rescale) {                     // each thread rescales its 64 output columns
+      l[h] = l[h] * corr + rs;
 #pragma unroll
-          for (int ch = 0; ch < 2; ++ch) {
-            uint32_t o[32];
-            tmem_ld32(tO + lane_off + chalf * 64 + ch * 32, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int c = 0; c < 32; ++c) o[c] = __float_as_uint(__uint_as_float(o[c]) * factor);
-            tmem_st32(tO + lane_off + chalf * 64 + ch * 32, o);
-          }
-          tmem_st_wait();
-        }
-      }
-      // P -> swizzled smem (A operand, K-major along kv); this thread's 64 columns are exactly half `chalf`
-#pragma unroll
-      for (int k = 0; k < 8; ++k) {
-        const uint32_t addr = sP_a + chalf * HALF_BYTES + r * 128 + ((k ^ (r & 7)) << 4);
-        st_shared_v4(addr, make_uint4(pk[4 * k], pk[4 * k + 1], pk[4 * k + 2], pk[4 * k + 3]));
-      }
-      fence_proxy_async_smem();
-      tc_fence_before();
-      mbar_arrive(p_full);
+      for (int dt = 0; dt < 16; ++dt) { o[dt][2 * h] *= corr; o[dt][2 * h + 1] *= corr; }
     }
-    // epilogue: O / l -> bf16 -> smem (reuse Q tile) -> TMA store ; LSE
-    s_stat[(4 + chalf) * 128 + r] = l;
-    mbar_wait(pv_done, (n_kv - 1) & 1);
-    tc_fence_after();
-    named_bar_sync(2, 256);
-    l += s_stat[(4 + (chalf ^ 1)) * 128 + r];
-    const float inv_l = 1.f / l;
-    const uint32_t sO_a = smem_u32(sQ);
+    // O += P V
 #pragma unroll
-    for (int ch = 0; ch < 2; ++ch) {
-      uint32_t o[32];
-      tmem_ld32(tO + lane_off + chalf * 64 + ch * 32, o);
-      tmem_ld_wait();
+    for (int kc = 0; kc < 4; ++kc) {
 #pragma unroll
-      for (int c8 = 0; c8 < 4; ++c8) {
-        const int k = ch * 4 + c8;     // 16-byte chunk within this thread's 128-byte half row
-        uint4 v;
-        v.x = pack_bf16x2(__uint_as_float(o[c8 * 8 + 0]) * inv_l, __uint_as_float(o[c8 * 8 + 1]) * inv_l);
-        v.y = pack_bf16x2(__uint_as_float(o[c8 * 8 + 2]) * inv_l, __uint_as_float(o[c8 * 8 + 3]) * inv_l);
-        v.z = pack_bf16x2(__uint_as_float(o[c8 * 8 + 4]) * inv_l, __uint_as_float(o[c8 * 8 + 5]) * inv_l);
-        v.w = pack_bf16x2(__uint_as_float(o[c8 * 8 + 6]) * inv_l, __uint_as_float(o[c8 * 8 + 7]) * inv_l);
-        st_shared_v4(sO_a + chalf * HALF_BYTES + r * 128 + ((k ^ (r & 7)) << 4), v);
+      for (int dp = 0; dp < 8; ++dp) {
+        uint32_t b[4];
+        ldsm_x4_t(vb + swz(kc * 16 + (lane & 7) + ((lane >> 3) & 1) * 8, dp * 2 + (lane >> 4)), b);
+        mma_bf16_16816(o[2 * dp], pa[kc], b[0], b[1]);
+        mma_bf16_16816(o[2 * dp + 1], pa[kc], b[2], b[3]);
       }
     }
-    if (chalf == 0 && q0 + r < p.S)
-      p.lse[(static_cast<size_t>(batch) * p.nh + head) * p.S + q0 + r] = (m_used + log2f(l)) * 0.6931471805599453f;
-    fence_proxy_async_smem();
-    named_bar_sync(1, 256);
-    if (warp == 2 && lane == 0) {
-      tma_store_4d(&tmO, sQ, 0, head, q0, batch);
-      tma_store_4d(&tmO, sQ + HALF_BYTES, 64, head, q0, batch);
-      tma_store_commit();
-      tma_store_wait<0>();
-    }
+    __syncthreads();   // the buffer is refilled by the next iteration's prefetch
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<1>(tmem_base, 512);
+  // epilogue: O / l -> bf16 ; LSE
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float lt = l[h];
+    lt += __shfl_xor_sync(0xffffffffu, lt, 1);
+    lt += __shfl_xor_sync(0xffffffffu, lt, 2);
+    const int r = row_a + 8 * h;
+    if (r >= n_rows) continue;
+    const float inv = 1.f / lt;
+    bf16* orow = p.o + static_cast<size_t>(tok0 + r) * p.ldo + head * D;
+#pragma unroll
+    for (int dt = 0; dt < 16; ++dt)
+      *reinterpret_cast<uint32_t*>(orow + dt * 8 + 2 * tq) = pack_bf16x2(o[dt][2 * h] * inv, o[dt][2 * h + 1] * inv);
+    if constexpr (MODE != PAGED) {
+      if (tq == 0) p.lse[(static_cast<size_t>(batch) * p.nh + head) * p.S + r] = (m[h] + log2f(lt)) * 0.6931471805599453f;
+    }
   }
 }
 
-// 4-D map over a [B, S, heads, 128] bf16 view with token stride `ld` (elements): dims {128, heads, S, B}.
-static int make_map(CUtensorMap* tm, const void* base, int64_t B, int64_t S, int64_t heads, int64_t ld) {
-  uint64_t dims[4] = {128, static_cast<uint64_t>(heads), static_cast<uint64_t>(S), static_cast<uint64_t>(B)};
-  uint64_t strides[3] = {128 * 2, static_cast<uint64_t>(ld) * 2, static_cast<uint64_t>(S) * ld * 2};
-  uint32_t box[4] = {64, 1, 128, 1};
-  return encode_tmap_bf16(tm, base, 4, dims, strides, box);
+template <int NW, int MODE>
+static int launch(const Params& p, int q_rows, cudaStream_t stream) {
+  constexpr int SMEM = 16 * NW * 256 + 4 * KV_TILE_BYTES;
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(fa_fwd_kernel<NW, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
+    if (e != cudaSuccess) {
+      set_last_error("fa_fwd smem attr: %s", cudaGetErrorString(e));
+      return static_cast<int>(e);
+    }
+    attr_set = true;
+  }
+  dim3 grid(static_cast<unsigned>((q_rows + 16 * NW - 1) / (16 * NW)), static_cast<unsigned>(p.nh), static_cast<unsigned>(p.B));
+  fa_fwd_kernel<NW, MODE><<<grid, NW * 32, SMEM, stream>>>(p);
+  return check_launch("fa_fwd");
 }
 
 }  // namespace fa
+
+// Prefill half of append_attention: causal attention of the NEW token rows of every prompt / prompt-chunk sequence over its paged
+// cache (cached prefix + the rows themselves, already appended).  qkv: packed projection [token_num, ldq] (q heads first, rotated);
+// key / value caches [num_blocks, kvh, block_size, 128]; out [token_num, ldo].  max_q_len bounds seq_lens_this_time (grid size).
+int launch_fa_prefill_paged(const void* qkv, const void* key_cache, const void* value_cache, void* out, const int32_t* cu_seqlens_q,
+                            const int32_t* seq_lens_encoder, const int32_t* seq_lens_decoder, const int32_t* seq_lens_this_time,
+                            const int32_t* block_tables, int64_t B, int64_t token_num, int64_t max_q_len, int64_t num_heads,
+                            int64_t num_kv_heads, int64_t num_blocks, int64_t block_size, int64_t max_blocks_per_seq, int64_t ldq,
+                            int64_t ldo, float softmax_scale, cudaStream_t stream) {
+  using namespace fa;
+  (void)token_num; (void)num_blocks;
+  Params p = {};
+  p.q = static_cast<const bf16*>(qkv);
+  p.k = static_cast<const bf16*>(key_cache);
+  p.v = static_cast<const bf16*>(value_cache);
+  p.o = static_cast<bf16*>(out);
+  p.ldq = ldq; p.ldo = ldo;
+  p.S = static_cast<int>(max_q_len); p.B = static_cast<int>(B); p.nh = static_cast<int>(num_heads);
+  p.kvh = static_cast<int>(num_kv_heads);
+  p.scale_log2 = softmax_scale * 1.4426950408889634f;
+  p.cu_q = cu_seqlens_q; p.seq_dec = seq_lens_decoder; p.seq_this = seq_lens_this_time; p.seq_enc = seq_lens_encoder;
+  p.block_tables = block_tables;
+  p.max_blocks = static_cast<int>(max_blocks_per_seq); p.block_size = static_cast<int>(block_size);
+  return launch<8, PAGED>(p, static_cast<int>(max_q_len), stream);
+}
+
 }  // namespace b200
 
 extern "C" int b200_fa_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int64_t B, int64_t S,
@@ -346,32 +289,19 @@ extern "C" int b200_fa_fwd_flashmask(const void* q, const void* k, const void* v
                  "fa_fwd: bad shape B=%lld S=%lld nh=%lld kvh=%lld", (long long)B, (long long)S, (long long)num_heads,
                  (long long)num_kv_heads);
   B200_CHECK_ARG(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0, "fa_fwd: token strides must be multiples of 8");
-  if (fa_fwd_impl() == 2)     // two q tiles per CTA, P in TMEM (fa_fwd2.cu); plain causal or FlashMask start rows
-    return launch_fa_fwd2(q, k, v, o, lse, mask_start_rows, B, S, num_heads, num_kv_heads, ldq, ldk, ldv, ldo, softmax_scale, stream);
-  CUtensorMap tmQ, tmK, tmV, tmO;
-  int rc;
-  if ((rc = make_map(&tmQ, q, B, S, num_heads, ldq)) != 0) return rc;
-  if ((rc = make_map(&tmK, k, B, S, num_kv_heads, ldk)) != 0) return rc;
-  if ((rc = make_map(&tmV, v, B, S, num_kv_heads, ldv)) != 0) return rc;
-  if ((rc = make_map(&tmO, o, B, S, num_heads, ldo)) != 0) return rc;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(fa_fwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(fa_fwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-    if (e != cudaSuccess) {
-      set_last_error("fa_fwd smem attr: %s", cudaGetErrorString(e));
-      return static_cast<int>(e);
-    }
-    attr_set = true;
-  }
-  Params p;
+  Params p = {};
+  p.q = static_cast<const bf16*>(q);
+  p.k = static_cast<const bf16*>(k);
+  p.v = static_cast<const bf16*>(v);
+  p.o = static_cast<bf16*>(o);
+  p.lse = lse;
+  p.ldq = ldq; p.ldk = ldk; p.ldv = ldv; p.ldo = ldo;
   p.S = static_cast<int>(S); p.B = static_cast<int>(B); p.nh = static_cast<int>(num_heads);
   p.kvh = static_cast<int>(num_kv_heads);
   p.scale_log2 = softmax_scale * 1.4426950408889634f;
-  p.lse = lse;
   p.mask_start = mask_start_rows;
-  dim3 grid(static_cast<unsigned>((S + BQ - 1) / BQ), static_cast<unsigned>(num_heads), static_cast<unsigned>(B));
-  if (mask_start_rows != nullptr) fa_fwd_kernel<true><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(tmQ, tmK, tmV, tmO, p);
-  else fa_fwd_kernel<false><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(tmQ, tmK, tmV, tmO, p);
-  return check_launch("fa_fwd");
+  const int rows = static_cast<int>(S);
+  if (fa_fwd_impl() == 1)
+    return mask_start_rows ? launch<4, MASK>(p, rows, stream) : launch<4, DENSE>(p, rows, stream);
+  return mask_start_rows ? launch<8, MASK>(p, rows, stream) : launch<8, DENSE>(p, rows, stream);
 }

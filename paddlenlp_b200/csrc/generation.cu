@@ -1468,8 +1468,8 @@ extern "C" int b200_save_output_stream(const int64_t* next_tokens, const int32_t
 //     idle slot               (seq_lens_this_time[b] == 0)
 //   1. append_rope_write_kernel  RoPE (rotate-half) on q, k of EVERY new row in place + k, v appended to the pages (one launch
 //                                for prompt and decode rows alike); decode rows' q are also gathered into a dense [B, ld] buffer
-//   2. fa_fwd2_kernel<PAGED>     prompt rows: tcgen05 flash attention, q tiles of 2 x 128 rows, K/V tiles gathered page by page
-//                                with TMA, causal band offset by the cached prefix (chunked prefill)
+//   2. fa_fwd_kernel<8, PAGED>   prompt rows: flash attention, q tiles of 128 rows, K/V rows gathered page by page with
+//                                cp.async, causal band offset by the cached prefix (chunked prefill)
 //   3. decode_attention_tc<PAGED> decode rows (the decode step's kernel; sequences of the other kinds have length -1 = no work)
 //   4. scatter of the decode rows' outputs back to their token rows
 // No host synchronisation: each kernel decides from the device-resident length arrays which sequences are its own (the

@@ -15,21 +15,9 @@ int fail_arg(const char* fmt, ...);   // records message, returns -1
 int check_launch(const char* what);  // cudaGetLastError() -> return code
 
 int sm_count();  // multiprocessors of the current device (cached per device)
-int skinny_gemm_impl();   // b200_set_skinny_gemm(): 1 = swapped-operand two-CTA/SM kernel (gemm_skinny.cu), 0 = the 128x256 persistent kernel
-int fa_fwd_impl();         // b200_set_fa_fwd_impl(): 2 = two-q-tile kernel (fa_fwd2.cu), 1 = fa_fwd.cu
-// fa_fwd2.cu: causal forward, optional FlashMask start rows (same argument meaning as b200_fa_fwd_flashmask)
-int launch_fa_fwd2(const void* q, const void* k, const void* v, void* o, float* lse, const int32_t* mask_start_rows, int64_t B, int64_t S, int64_t num_heads,
-                   int64_t num_kv_heads, int64_t ldq, int64_t ldk, int64_t ldv, int64_t ldo, float softmax_scale,
-                   cudaStream_t stream);
-int l2_prefetch_mb();      // MB of weights a decode-step GEMM requests into L2 before griddepcontrol.wait (B200_L2_PREFETCH_MB, default 8)
-int fa_exp_poly();        // b200_set_fa_exp_poly(): 0 / 1 / 2 = none / a quarter / half of the forward exponentials on the FMA pipe
-int fa_bwd_impl();         // b200_set_fa_bwd_impl(): 2 = transposed pipelined kernel (fa_bwd2.cu), 1 = fa_bwd.cu
-// fa_bwd2.cu: causal backward, optional FlashMask start rows (same argument meaning as b200_fa_bwd_flashmask)
-int launch_fa_bwd2(const void* q, const void* k, const void* v, const void* o, const void* dout, const float* lse,
-                   const int32_t* mask_start_rows, void* dq, void* dk, void* dv, void* workspace, int64_t B, int64_t S, int64_t num_heads, int64_t num_kv_heads,
-                   int64_t ldq, int64_t ldk, int64_t ldv, int64_t ldo, int64_t lddo, int64_t lddq, int64_t lddk, int64_t lddv,
-                   float softmax_scale, cudaStream_t stream);
-// fa_fwd2.cu, PAGED instantiation: prefill half of b200_append_attention
+int fa_fwd_impl();         // b200_set_fa_fwd_impl(): 2 = 128-row q tiles (8 warps), 1 = 64-row q tiles (4 warps)
+int fa_bwd_impl();         // b200_set_fa_bwd_impl(): 2 = 128-row q tiles, 1 = 64-row q tiles (64-row kv tiles either way)
+// fa_fwd.cu, paged instantiation: prefill half of b200_append_attention
 int launch_fa_prefill_paged(const void* qkv, const void* key_cache, const void* value_cache, void* out, const int32_t* cu_seqlens_q,
                             const int32_t* seq_lens_encoder, const int32_t* seq_lens_decoder, const int32_t* seq_lens_this_time,
                             const int32_t* block_tables, int64_t B, int64_t token_num, int64_t max_q_len, int64_t num_heads,

@@ -1,6 +1,6 @@
 """FusedMultiTransformer — the stacked-layer inference block of
 paddlenlp/experimental/transformers/fused_transformer_layers.py (:205-345 config, :348-792 weights, :1027-1182 forward)
-for the bf16, non-quantised, rmsnorm + swiglu + rotate-half-RoPE case, on the native sm_100a kernels.
+for the bf16, non-quantised, rmsnorm + swiglu + rotate-half-RoPE case, on the native sm_90a kernels.
 
 Weight layouts are the reference's (SURVEY.md Appendix B):
     qkv_weight    [(nh + 2*kvh) * d, h]   (transposed, trans_qkvw=True)      -> GEMM with B stored [N, K]
@@ -80,14 +80,9 @@ class FusedMultiTransformerBase:
         self.ffn1_weights = [z(self.h, 2 * self.I) for _ in range(self.L)]
         self.ffn2_weights = [z(self.I, self.h) for _ in range(self.L)]
         self._bias_f32 = [None] * self.L
-        # decode-step ffn1 + SwiGLU (see the measurement note in forward()): "persistent" = 128x256-tile kernel with the SwiGLU
-        # epilogue, "skinny" = swapped-operand two-CTA/SM kernel with the SwiGLU epilogue, "unfused" = GEMM + SwiGLU kernel
+        # decode-step ffn1 + SwiGLU: "skinny" / "persistent" = the wgmma GEMM with the SwiGLU epilogue (through the decode-step
+        # and the general entry point), "unfused" = GEMM + SwiGLU kernel
         self.ffn1_impl = os.environ.get("B200_DECODE_FFN1", "skinny")
-        # decode step: out-linear .. next layer's qkv as ONE persistent kernel per layer (ops.decode_layer_chain) instead of six
-        # programmatically chained launches.  OFF by default: measured 108 us against 89 us per layer for the six kernels
-        # (tools/decode_probe.py chain, profiles/r02_decode_chain_probe.log) — the grid barriers are cheap (0.25 us) but the two
-        # norm phases take 8 us each under the weight-prefetch traffic, and the chained launches already overlap their prologues
-        self.layer_chain = os.environ.get("B200_DECODE_CHAIN", "0") != "0"
         self.rope = ops.rope_tables(self.d, c.max_position_embeddings, float(c.rope_theta), self.device)
 
     def ensure_rope(self, positions: int):
@@ -163,19 +158,6 @@ class FusedMultiTransformerBase:
         residual = src
         ln_out, _ = ops.add_rmsnorm(src, None, self.ln_scales[0], eps, want_residual=False)   # compute_layernorm_before_qkv
         fused = decode and src.shape[0] <= self.SKINNY_M and not getattr(self.config, "append_attn", False)
-        if (fused and self.layer_chain and src.shape[0] <= 64 and self.I % 64 == 0 and self.h % 128 == 0 and self.h <= 8192
-                and self.qkv_n % 128 == 0):
-            # one persistent kernel per layer for everything between two attention calls; the residual stream lives in one buffer
-            residual = src.clone()
-            acc = ops.gemm_skinny_f32(ln_out, self.qkv_weights[0], trans_b=True, tag="splitk_qkv")
-            for i in range(self.L):
-                qkv = self._rope_append(None, acc, caches, i, seq_lens_decoder, kw)
-                attn = self._attend(qkv, caches, i, seq_lens_decoder, kw)
-                last = i == self.L - 1
-                acc = ops.decode_layer_chain(attn, self.linear_weights[i], self.ffn_ln_scales[i], self.ffn1_weights[i],
-                                             self.ffn2_weights[i], None if last else self.ln_scales[i + 1],
-                                             None if last else self.qkv_weights[i + 1], residual, eps)
-            return residual
         for i in range(self.L):
             if fused:
                 # decode step: the split-K GEMMs leave fp32 sums that the next kernel rounds once (same rounding points,
@@ -185,13 +167,8 @@ class FusedMultiTransformerBase:
                 attn = self._attend(qkv, caches, i, seq_lens_decoder, kw)
                 acc = ops.gemm_skinny_f32(attn, self.linear_weights[i], tag="splitk_h")
                 ln_out, residual = ops.add_rmsnorm_f32(acc, residual, self.ffn_ln_scales[i], eps)
-                # ffn1 + SwiGLU, measured in the 32-layer chain at context 1024 (tools/decode_ablation.py B200_FFN1=fused|epi|plain,
-                # profiles/r02_decode_ablation_ffn1.log): swapped-operand kernel with the SwiGLU epilogue 4.458 ms, persistent
-                # 128x256-tile kernel with the SwiGLU epilogue 4.533 ms, GEMM + SwiGLU kernel 4.630 ms.  (Both epilogues use
-                # swiglu_fwd_pair: with an IEEE division + expf per element the persistent epilogue alone took 6.5 us per layer.)
                 if self.ffn1_impl == "skinny" and ln_out.shape[0] <= 64 and self.I % 64 == 0:
-                    # swapped-operand kernel, tile = 64 gate columns + the 64 up columns of the same channels, straight from the
-                    # reference-layout weight; the activation leaves as one TMA store per tile
+                    # the SwiGLU GEMM's decode-step entry point (gate|up are not stored), straight from the reference-layout weight
                     act = ops.gemm_swiglu_skinny(ln_out, self.ffn1_weights[i])
                 elif self.ffn1_impl != "unfused" and self.I % 128 == 0:
                     # SwiGLU in the ffn1 epilogue of the persistent kernel: the 256-column tile pairs 128 gate columns with the

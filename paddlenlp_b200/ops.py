@@ -89,7 +89,7 @@ def gemm(a: torch.Tensor, b: torch.Tensor, out: Optional[torch.Tensor] = None, *
 
 def gemm_swiglu(x: torch.Tensor, w_gate_up: torch.Tensor, gate_up: Optional[torch.Tensor] = None,
                 out: Optional[torch.Tensor] = None, cta_group: int = 2, store_gate_up: bool = True):
-    """(gate_up [M, 2I], m [M, I]) = fused gate|up projection + SwiGLU (one tcgen05 GEMM; the epilogue holds gate and up of the
+    """(gate_up [M, 2I], m [M, I]) = fused gate|up projection + SwiGLU (one wgmma GEMM; the epilogue holds gate and up of the
     same channels).  w_gate_up is the reference-layout fused weight [K, 2I] (gate | up).  Requires I % 128 == 0.
     store_gate_up=False (inference): only m is written and (None, m) is returned."""
     _chk(x, "x"); _chk(w_gate_up, "w_gate_up")
@@ -308,39 +308,6 @@ def gemm_swiglu_skinny(x: torch.Tensor, w_gate_up: torch.Tensor, out: Optional[t
     return out
 
 
-def decode_layer_chain(attn: torch.Tensor, w_o: torch.Tensor, w_ffn_ln: torch.Tensor, w_ffn1: torch.Tensor, w_ffn2: torch.Tensor,
-                       w_next_ln: Optional[torch.Tensor], w_next_qkv: Optional[torch.Tensor], residual: torch.Tensor, eps: float,
-                       qkv_tag: str = "splitk_qkv"):
-    """One persistent kernel for the GEMM chain of a decode layer (M <= 64 rows): out-linear, residual + ffn RMSNorm, ffn1 +
-    SwiGLU, ffn2, residual + the next layer's RMSNorm, the next layer's QKV projection (see b200_decode_layer_chain).
-    `residual` [M, h] is updated IN PLACE.  Returns the fp32 QKV accumulation [M, qkv_n] of the next layer (the workspace
-    decode_rope_append_f32 consumes and re-zeroes) or None for the last layer (w_next_qkv None)."""
-    for t, n in ((attn, "attn"), (w_o, "w_o"), (w_ffn_ln, "w_ffn_ln"), (w_ffn1, "w_ffn1"), (w_ffn2, "w_ffn2"), (residual, "residual")):
-        _chk(t, n)
-    M, aw = attn.shape
-    h = w_o.shape[1]
-    inter = w_ffn2.shape[0]
-    assert w_o.shape == (aw, h) and w_ffn1.shape == (h, 2 * inter) and w_ffn2.shape == (inter, h) and residual.shape == (M, h)
-    assert all(t.is_contiguous() for t in (attn, w_o, w_ffn1, w_ffn2, residual))
-    dev = attn.device
-    ln_buf = _workspace(M * h * 2, dev, "chain_ln")
-    act_buf = _workspace(M * inter * 2, dev, "chain_act")
-    acc_h = _zero_workspace(M * h * 4, dev, "chain_h")
-    sync = _zero_workspace(_lib.load().b200_decode_layer_chain_workspace_bytes(), dev, "chain_sync")
-    acc_qkv, qkv_n = None, 0
-    if w_next_qkv is not None:
-        _chk(w_next_qkv, "w_next_qkv"); _chk(w_next_ln, "w_next_ln")
-        qkv_n = w_next_qkv.shape[0]
-        assert w_next_qkv.shape == (qkv_n, h) and w_next_qkv.is_contiguous()
-        acc_qkv = _zero_workspace(M * qkv_n * 4, dev, qkv_tag)
-    call("b200_decode_layer_chain", ptr(attn), ptr(w_o), ptr(w_ffn_ln), ptr(w_ffn1), ptr(w_ffn2), ptr(w_next_ln), ptr(w_next_qkv),
-         ptr(residual), ptr(ln_buf), ptr(act_buf), ptr(acc_h), ptr(acc_qkv), ptr(sync), M, h, aw, inter, qkv_n, float(eps),
-         stream_ptr())
-    if acc_qkv is None:
-        return None
-    return acc_qkv[: M * qkv_n * 4].view(torch.float32).view(M, qkv_n)
-
-
 def swiglu_bwd(gate_up: torch.Tensor, dout: torch.Tensor, dgate_up: Optional[torch.Tensor] = None):
     _chk(gate_up, "gate_up"); _chk(dout, "dout")
     rows, two_i = gate_up.shape
@@ -543,7 +510,7 @@ def decode_rope_append(qkv, cache, cos, sin, seq_lens, nh, kvh, d):
 
 
 def decode_attention(qkv, cache, seq_lens, nh, kvh, d, softmax_scale=None, out=None, num_splits: int = 0, impl: str = "tc"):
-    """impl "tc": persistent tcgen05 kernel (TMA-streamed cache); "simt": the CUDA-core kernel (half-warp per cache row)."""
+    """impl "tc" / "simt": both run the streaming CUDA-core kernel (half-warp per cache row); "tc" keeps its split heuristic."""
     _chk(qkv, "qkv"); _chk(cache, "cache"); _chk(seq_lens, "seq_lens", torch.int32)
     B = qkv.shape[0]
     if out is None:
@@ -555,12 +522,12 @@ def decode_attention(qkv, cache, seq_lens, nh, kvh, d, softmax_scale=None, out=N
         if num_splits <= 0:
             # persistent CTAs walk (split, b, kv head) items round-robin; split only when there are too few (b, kv head)
             # pairs to give every SM ~3 items (a split costs partial traffic, a merge launch and an item boundary)
-            num_splits = max(1, min((max_len + 127) // 128, (3 * 148 + B * kvh - 1) // (B * kvh)))
+            num_splits = max(1, min((max_len + 127) // 128, (3 * 132 + B * kvh - 1) // (B * kvh)))
         fn = "b200_decode_attention_tc"
     elif impl == "simt":
         if num_splits <= 0:
             # enough CTAs for ~8 per SM without making the ranges shorter than ~64 cache rows at full length
-            num_splits = max(1, min(max_len // 64, (8 * 148 + B * kvh - 1) // (B * kvh)))
+            num_splits = max(1, min(max_len // 64, (8 * 132 + B * kvh - 1) // (B * kvh)))
         fn = "b200_decode_attention"
     else:
         raise ValueError(f"decode_attention impl {impl!r}")
@@ -611,7 +578,7 @@ def decode_attention_paged(qkv, key_cache, value_cache, block_tables, seq_lens, 
         softmax_scale = 1.0 / math.sqrt(d)
     max_len = mb * bs
     if num_splits <= 0:
-        num_splits = max(1, min((max_len + 127) // 128, (3 * 148 + B * kvh - 1) // (B * kvh)))
+        num_splits = max(1, min((max_len + 127) // 128, (3 * 132 + B * kvh - 1) // (B * kvh)))
     ws = None
     if num_splits > 1:
         ws = _workspace(_lib.load().b200_decode_attention_workspace_bytes(B, nh, num_splits), qkv.device, "decode_attn")
@@ -656,7 +623,7 @@ def append_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_dec
     if softmax_scale is None:
         softmax_scale = 1.0 / math.sqrt(d)
     if num_splits <= 0:
-        num_splits = max(1, min((mb * bs + 127) // 128, (3 * 148 + B * kvh - 1) // (B * kvh)))
+        num_splits = max(1, min((mb * bs + 127) // 128, (3 * 132 + B * kvh - 1) // (B * kvh)))
     ws = _workspace(_lib.load().b200_append_attention_workspace_bytes(B, nh, kvh, d, num_splits), qkv.device, "append_attn")
     call("b200_append_attention", ptr(qkv), ptr(key_cache), ptr(value_cache), ptr(seq_lens_encoder), ptr(seq_lens_decoder),
          ptr(seq_lens_this_time), ptr(cu_seqlens_q), ptr(block_tables), ptr(cos), ptr(sin), ptr(out), ptr(ws), B, token_num,

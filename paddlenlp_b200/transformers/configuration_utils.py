@@ -12,7 +12,7 @@ import os
 from typing import Any, Dict
 
 # Runtime switches the reference copies from TrainingArguments (configuration_utils.py:231-314).  They are accepted
-# and stored; on this implementation every one of them maps onto the single native sm_100a path.
+# and stored; on this implementation every one of them maps onto the single native sm_90a path.
 LLM_META_SWITCHES = {
     "use_flash_attention": True,
     "use_fused_rms_norm": True,

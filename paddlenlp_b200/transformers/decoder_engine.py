@@ -1,6 +1,6 @@
 """DecoderEngine: the Llama/Qwen2 decoder hot path (forward, backward, flat parameter/gradient buffers).
 
-This is the host-side orchestration of the sm_100a kernels behind the C-ABI.  It replaces the per-op eager execution
+This is the host-side orchestration of the sm_90a kernels behind the C-ABI.  It replaces the per-op eager execution
 of the reference's
     LlamaModel.forward            paddlenlp/transformers/llama/modeling.py:1588-1774
     LlamaDecoderLayer.forward     paddlenlp/transformers/llama/modeling.py:1138-1232
@@ -10,7 +10,7 @@ of the reference's
 and their autograd backward with an explicit saved-tensor plan.  Per layer, forward is
     rmsnorm -> QKV GEMM(+bias) -> RoPE (in place) -> flash attention -> O GEMM(+residual epilogue)
             -> rmsnorm -> gate|up GEMM -> SwiGLU -> down GEMM(+residual epilogue)
-i.e. 4 tcgen05 GEMMs, 1 tcgen05 attention and 4 HBM-bound fusions; the residual adds live in GEMM epilogues.
+i.e. 4 wgmma GEMMs, 1 mma.sync attention and 4 HBM-bound fusions; the residual adds live in GEMM epilogues.
 
 Data layout in HBM
   * ONE flat bf16 parameter buffer and ONE flat bf16 gradient buffer (the buffer the data-parallel all-reduce and
@@ -61,9 +61,8 @@ class DecoderEngine:
         # SwiGLU fused into the gate|up GEMM epilogue (needs 128-channel tiles); B200_FUSE_SWIGLU=0 selects GEMM + swiglu kernel
         import os as _os
         self.fuse_swiglu = (self.I % 128 == 0) and _os.environ.get("B200_FUSE_SWIGLU", "1") != "0"
-        # the backward twin: SwiGLU backward in the down-proj dX epilogue (bit-identical to GEMM + swiglu_bwd kernel).  The epilogue
-        # streams the saved gate|up tile through a 4-deep TMA pipeline of 16-channel slabs: 0.70 ms against 0.61 ms for the bare GEMM
-        # and 0.88 ms for GEMM + kernel (tools/epilogue_bench.py, profiles/r02_swiglu_bwd_epilogue.md).  B200_FUSE_SWIGLU_BWD=0 unfuses
+        # the backward twin: SwiGLU backward in the down-proj dX epilogue (bit-identical to GEMM + swiglu_bwd kernel; the epilogue reads
+        # the saved gate|up values of its accumulator's rows and columns).  B200_FUSE_SWIGLU_BWD=0 unfuses
         self.fuse_swiglu_bwd = (self.I % 64 == 0) and _os.environ.get("B200_FUSE_SWIGLU_BWD", "1") != "0"
         # recompute (llama/modeling.py:1706-1733 `recompute_training_full`): keep only each layer's input and re-run the
         # layer forward inside backward.  Only the "full" granularity exists here (the "full_attn" / "core_attn" splits

@@ -6,7 +6,7 @@ Surface of paddlenlp/transformers/gpt/modeling.py: GPTEmbeddings :715-774 (word 
 GPTDecoderLayer :567-712 (pre-LN, tanh-GELU MLP), final LayerNorm(eps 1e-5) :455, GPTLMHead :1461-1503 (tied to the word
 embeddings), GPTPretrainingCriterion :1323-1363 (ignore_index defaults to 0; mean over loss > 0), GPTForCausalLM :1506-1620.
 This path is plain fp32 torch by design: the reference runs it on the CPU through Paddle's CPU kernels, there is nothing
-to accelerate and no B200 kernel is involved.  Linear weights keep Paddle's [in, out] layout and parameter names.
+to accelerate and no GPU kernel is involved.  Linear weights keep Paddle's [in, out] layout and parameter names.
 """
 from __future__ import annotations
 

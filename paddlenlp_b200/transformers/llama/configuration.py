@@ -56,6 +56,15 @@ class LlamaConfig(PretrainedConfig):
 
     # public presets used by bench / tests (hyper-parameters from the public model cards, SURVEY.md §8)
     @classmethod
+    def llama3_2_3b(cls, **kw):
+        """Llama-3.2-3B shapes (head_dim 128, GQA 24/8) with untied input and output embeddings."""
+        base = dict(vocab_size=128256, hidden_size=3072, intermediate_size=8192, num_hidden_layers=28,
+                    num_attention_heads=24, num_key_value_heads=8, rms_norm_eps=1e-5, rope_theta=500000.0,
+                    max_position_embeddings=8192, seq_length=4096, bos_token_id=128000, eos_token_id=128001)
+        base.update(kw)
+        return cls(**base)
+
+    @classmethod
     def llama3_8b(cls, **kw):
         base = dict(vocab_size=128256, hidden_size=4096, intermediate_size=14336, num_hidden_layers=32,
                     num_attention_heads=32, num_key_value_heads=8, rms_norm_eps=1e-5, rope_theta=500000.0,

@@ -1,4 +1,4 @@
-"""Llama modeling classes — API surface of paddlenlp/transformers/llama/modeling.py on the native sm_100a engine.
+"""Llama modeling classes — API surface of paddlenlp/transformers/llama/modeling.py on the native sm_90a engine.
 
     LlamaPretrainingCriterion   :1777-1825     LlamaModel        :1440-1774
     LlamaForCausalLM            :1924-2071     LlamaPretrainedModel :1235-1436

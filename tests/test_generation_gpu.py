@@ -159,7 +159,7 @@ def test_decode_rope_append_and_attention(nh, kvh, impl):
                                                      (8, 1, 200, 300, 0), (28, 4, 5, 1100, 0), (4, 1, 1, 4096, 0), (2, 2, 3, 130, 0),
                                                      (32, 8, 64, 1100, 0), (16, 2, 300, 2100, 0)])
 def test_decode_attention_tc_long(nh, kvh, B, max_len, splits):
-    """The persistent tcgen05 kernel over many work items per CTA, several 128-row tiles per item, ragged lengths (incl. 0
+    """The decode attention kernel over many work items, several 128-row tiles per item, ragged lengths (incl. 0
     cached tokens and a full cache), vs an fp32 reference and vs the CUDA-core kernel.  splits 0 = the library's own choice.
     Partial last tiles are fetched in 32-row boxes: lengths just past / just short of a tile boundary are in the ragged draw."""
     o = ops()
@@ -436,69 +436,6 @@ def test_generate_edge_cases(block_attn):
         m.generate(ids, max_length=29, cache_kvs=caches)
 
 
-@pytest.mark.parametrize("M,h,aw,inter,qkv_n,last", [(64, 4096, 4096, 14336, 6144, False), (5, 256, 256, 704, 512, False),
-                                                      (33, 3584, 3584, 18944, 4608, False), (64, 4096, 4096, 14336, 6144, True),
-                                                      (1, 128, 256, 64, 128, False)])
-def test_decode_layer_chain_matches_the_unfused_kernels(M, h, aw, inter, qkv_n, last):
-    """ops.decode_layer_chain (out-linear .. next layer's qkv as ONE persistent kernel with grid-wide barriers) against the six
-    kernels it replaces: same tiles, same K ranges, same rounding points; only the order of the fp32 split-K reduce-adds differs
-    between any two runs (of either path).  Two launches in a row: the barrier counters are handed back zeroed."""
-    o = ops()
-    g = torch.Generator().manual_seed(M + h)
-    r = lambda *s, scale=1.0: (torch.randn(*s, generator=g) * scale).to(BF16).to(DEV)
-    attn, res0 = r(M, aw), r(M, h)
-    w_o, w1, w2 = r(aw, h, scale=aw ** -0.5), r(h, 2 * inter, scale=h ** -0.5), r(inter, h, scale=inter ** -0.5)
-    wq = r(qkv_n, h, scale=h ** -0.5)
-    ln1, ln2 = (1 + 0.1 * torch.randn(h, generator=g)).to(BF16).to(DEV), (1 + 0.1 * torch.randn(h, generator=g)).to(BF16).to(DEV)
-    eps = 1e-5
-    # unfused reference path (the kernels of the default decode step before the chain)
-    acc = o.gemm_skinny_f32(attn, w_o, tag="t_h")
-    ln, res = o.add_rmsnorm_f32(acc, res0, ln1, eps)
-    act = o.gemm_swiglu_skinny(ln, w1)
-    acc = o.gemm_skinny_f32(act, w2, tag="t_h")
-    if last:
-        _, res_ref = o.add_rmsnorm_f32(acc, res, None, eps, want_normed=False)
-        accq_ref = None
-    else:
-        lnq, res_ref = o.add_rmsnorm_f32(acc, res, ln2, eps)
-        ws = o.gemm_skinny_f32(lnq, wq, trans_b=True, tag="t_q")
-        accq_ref = ws.clone()
-        ws.zero_()                                                        # the consumer's job (decode_rope_append_f32)
-    for _ in range(2):
-        res = res0.clone()
-        accq = o.decode_layer_chain(attn, w_o, ln1, w1, w2, None if last else ln2, None if last else wq, res, eps, qkv_tag="t_chain_q")
-        torch.cuda.synchronize()
-        scale = res_ref.float().abs().max().item()
-        assert (res.float() - res_ref.float()).abs().max().item() <= 2 ** -6 * scale
-        assert (res != res_ref).float().mean().item() < 0.1
-        if last:
-            assert accq is None
-        else:
-            qs = accq_ref.abs().max().item()
-            assert (accq - accq_ref).abs().max().item() <= 2e-2 * qs, ((accq - accq_ref).abs().max().item(), qs)
-            accq.zero_()                                                  # the consumer's job (decode_rope_append_f32)
-    from paddlenlp_b200 import ops as _ops
-    for tag in ("chain_h", "chain_sync"):
-        assert int(_ops._workspaces[(attn.device, tag)].view(torch.int32).abs().sum()) == 0   # handed back zeroed
-
-
-def test_generate_with_layer_chain_option():
-    """FusedMultiTransformerBase.layer_chain (one persistent kernel per layer for out-linear .. next qkv; off by default: measured
-    slower) generates the same tokens as the default chain of launches, with and without the CUDA graph."""
-    cfg = R.RefConfig(vocab_size=512, hidden_size=256, intermediate_size=704, num_hidden_layers=3, num_attention_heads=2,
-                      num_key_value_heads=1, rope_theta=10000.0, max_position_embeddings=128, rms_norm_eps=1e-5)
-    w = R.init_weights(cfg, seed=19)
-    w = {k: (v * 4).to(BF16).float() if k.endswith("weight") and "norm" not in k else v for k, v in w.items()}
-    m, _ = _infer_model(cfg, w)
-    ids = torch.randint(1, cfg.vocab_size, (4, 16), generator=torch.Generator().manual_seed(18))
-    a, _, _ = m.generate(ids, max_length=12)
-    m.transformer_block.layer_chain = True
-    b, _, _ = m.generate(ids, max_length=12)
-    c, _, _ = m.generate(ids, max_length=12, use_cuda_graph=False)
-    assert (a == b).float().mean().item() > 0.9 and torch.equal(a[:, :3], b[:, :3])
-    assert (a == c).float().mean().item() > 0.9 and torch.equal(a[:, :3], c[:, :3])
-
-
 def test_generate_with_fused_ffn1_swiglu_option():
     """FusedMultiTransformerBase.ffn1_impl: "skinny" (default: swapped-operand ffn1 + SwiGLU kernel) and "persistent" (128x256-tile
     kernel with the SwiGLU epilogue) generate the same tokens."""
@@ -518,7 +455,7 @@ def test_generate_with_fused_ffn1_swiglu_option():
 def test_full_width_decode_matches_uncached_forward():
     """KV-cache consistency (tests/transformers/llama/test_modeling.py:171-219) at the FULL Llama-3-8B layer width, batch 64:
     prefill logits match the training-path forward, and three decode steps (swapped-operand GEMMs at N = 6144 / 4096 /
-    28672, K = 14336; tcgen05 decode attention with 4 query heads per kv head) reproduce the uncached forward of the grown
+    28672, K = 14336; decode attention with 4 query heads per kv head) reproduce the uncached forward of the grown
     sequence within bf16 noise, with identical decisive arg-max."""
     import paddlenlp_b200.transformers as T
     from paddlenlp_b200.experimental.transformers import LlamaForCausalLMInferenceModel

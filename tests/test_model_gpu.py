@@ -186,7 +186,7 @@ def test_flashmask_packing_invariance(model_type, request):
     from paddlenlp_b200.datasets import ZeroPaddingMapDataset
 
     # the "same tiles, same order -> same bits" property below compares packed (FlashMask) and one-by-one (plain causal) runs
-    # of the SAME attention kernel generation: both instantiations live in fa_fwd2.cu (the default)
+    # of the SAME attention kernel: both instantiations live in fa_fwd.cu
     cfg = tiny_cfg(model_type)
     w = make_weights(cfg)
     model = build(cfg, w)

@@ -85,7 +85,7 @@ def test_gemm_residual_epilogue():
 @pytest.mark.parametrize("cg", [2, 1])
 @pytest.mark.parametrize("M,inter,K", [(520, 384, 328), (8192, 14336, 4096), (300, 128, 64), (64, 14336, 4096)])
 def test_gemm_swiglu_fused_epilogue(M, inter, K, cg):
-    """gate|up projection + SwiGLU in one tcgen05 GEMM (tile = 128 gate columns | the 128 up columns of the same channels) is
+    """gate|up projection + SwiGLU in one wgmma GEMM (tile = 128 gate columns | the 128 up columns of the same channels) is
     bit-identical to GEMM followed by the SwiGLU kernel: same accumulation order per element, same rounding points."""
     o = ops()
     x = rand_bf16(M, K, seed=51, scale=0.7).to(DEV)
@@ -128,26 +128,6 @@ def test_gemm_skinny_splitk(M, N, K, split, tb):
     out = o.gemm_skinny(A.to(DEV), b_d, trans_b=tb, bias=bias.to(DEV), split_k=split)
     ref = A.float().to(DEV) @ B.float().to(DEV) + bias.to(DEV)
     assert maxerr(out, ref) < 2 ** -7 and relerr(out, ref) < 4e-3
-
-
-@pytest.mark.parametrize("impl", [0, 2])
-def test_gemm_skinny_alternative_kernels(impl):
-    """b200_set_skinny_gemm: the 128x256 split-K kernel (0) and the stream-K variant (2) give the default kernel's result up to
-    fp32 summation order."""
-    from paddlenlp_b200 import _lib
-    o = ops()
-    lib = _lib.load()
-    try:
-        for M, N, K, tb in ((64, 4096, 4096, False), (64, 6144, 4096, True), (17, 1024, 14336, False), (64, 28672, 512, False)):
-            a = rand_bf16(M, K, seed=41).to(DEV)
-            w = rand_bf16(N, K, seed=42).to(DEV) if tb else rand_bf16(K, N, seed=42).to(DEV)
-            lib.b200_set_skinny_gemm(1)
-            want = o.gemm_skinny(a, w, trans_b=tb).float()
-            lib.b200_set_skinny_gemm(impl)
-            got = o.gemm_skinny(a, w, trans_b=tb).float()
-            assert maxerr(got, want) < 2 ** -7, (M, N, K, tb)
-    finally:
-        lib.b200_set_skinny_gemm(1)
 
 
 @pytest.mark.parametrize("M,inter,K", [(64, 14336, 4096), (5, 192, 328), (33, 18944, 3584)])
@@ -275,8 +255,8 @@ def test_embedding():
 # ------------------------------------------------------------------------------------------------
 @pytest.fixture
 def fa_fwd_impl(request):
-    """Select the plain-causal attention kernel generation (b200_set_fa_fwd_impl / b200_set_fa_bwd_impl: 2 = fa_fwd2.cu +
-    fa_bwd2.cu, 1 = fa_fwd.cu + fa_bwd.cu) for one test, then restore."""
+    """Select the attention tile height (b200_set_fa_fwd_impl / b200_set_fa_bwd_impl: 2 = 128-row q tiles, 1 = 64-row q tiles)
+    for one test, then restore."""
     from paddlenlp_b200 import _lib
 
     lib = _lib.load()

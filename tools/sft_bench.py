@@ -1,4 +1,5 @@
-"""Config 4: Qwen2-7B full-parameter SFT, bf16, seq 2048, through the Trainer API with synthetic instruction pairs.
+"""Config 4: Qwen2-1.5B full-parameter SFT, bf16, seq 2048, through the Trainer API with synthetic instruction pairs
+(Qwen2-7B, the BASELINE.json size, needs 122 GB of weights and AdamW state: more than one H100 holds).
 
     python tools/sft_bench.py [--steps 4 --micro-batch 4 --accum 2]           # 1 GPU
     python -m torch.distributed.run --nproc-per-node N tools/sft_bench.py     # pure data parallel
@@ -50,7 +51,7 @@ def run(steps=4, warmup=2, micro_batch=4, accum=2, layers=0, zero_padding=False,
     args = TrainingArguments(output_dir="/tmp/sft_out", per_device_train_batch_size=micro_batch,
                              gradient_accumulation_steps=accum, max_steps=steps + warmup, learning_rate=3e-5,
                              weight_decay=0.01, warmup_steps=1, logging_steps=1, max_seq_length=S, lr_scheduler_type="linear")
-    cfg = T.Qwen2Config.qwen2_7b(num_hidden_layers=layers) if layers else T.Qwen2Config.qwen2_7b()
+    cfg = T.Qwen2Config.qwen2_1_5b(num_hidden_layers=layers) if layers else T.Qwen2Config.qwen2_1_5b()
     model = T.AutoModelForCausalLM.from_config(cfg, dtype="bfloat16")
     n = (steps + warmup) * micro_batch * accum * args.world_size
     collator = None
@@ -79,9 +80,9 @@ def run(steps=4, warmup=2, micro_batch=4, accum=2, layers=0, zero_padding=False,
     if args.process_index == 0:
         sps = sum(h["interval_samples_per_second"] for h in hist) / len(hist)
         nonpad = sum(it[2] for it in ds.items) / len(ds.items)
-        rec = dict(workload="Qwen2-7B full-parameter SFT bf16 through Trainer.train(), synthetic instruction pairs "
+        rec = dict(workload="Qwen2-1.5B full-parameter SFT bf16 through Trainer.train(), synthetic instruction pairs "
                             "(BASELINE.json configs[3])",
-                   model="Qwen2-7B" if not layers else f"Qwen2-7B width, {layers} layers", n_gpus=args.world_size,
+                   model="Qwen2-1.5B" if not layers else f"Qwen2-1.5B width, {layers} layers", n_gpus=args.world_size,
                    seq_len=S, zero_padding=bool(zero_padding), micro_batch=micro_batch, grad_accum=accum, steps=steps,
                    global_batch=micro_batch * accum * args.world_size,
                    tokens_per_s=sps * S, nonpad_tokens_per_s=sps * nonpad, loss_first=hist[0]["loss"], loss_last=hist[-1]["loss"],

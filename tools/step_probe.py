@@ -1,4 +1,4 @@
-"""Probe: full-width Llama-3-8B layers (reduced depth) fwd+bwd timing on one B200, with extrapolation to 32 layers."""
+"""Probe: full-width Llama-3-8B layers (reduced depth) fwd+bwd timing on one H100, with extrapolation to 32 layers."""
 import argparse
 import json
 import os
