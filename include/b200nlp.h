@@ -43,8 +43,9 @@ int b200_set_pdl(int enable);
  * rows (8 warps) per CTA, 1 = 64 rows (4 warps).  Same rounding points; kept switchable for A/B measurements.  The initial
  * value can be set with the environment variable B200_FA_FWD_IMPL. */
 int b200_set_fa_fwd_impl(int impl);
-/* Same for b200_fa_bwd / b200_fa_bwd_flashmask: 2 (default) = 128-row q steps per 64-row kv tile, 1 = 64-row q steps.
- * Environment override: B200_FA_BWD_IMPL. */
+/* Kernel of b200_fa_bwd / b200_fa_bwd_flashmask (returns the previous setting): 2 (default) = the warp-specialised wgmma
+ * kernel (128-row kv tiles, TMA-fed 64-row q tiles, TMA reduce-adds), 1 = the mma.sync kernel (64-row kv and q tiles), kept as
+ * the cross-check.  Same rounding points.  Environment override: B200_FA_BWD_IMPL. */
 int b200_set_fa_bwd_impl(int impl);
 
 /* ---- GEMM: replaces paddle.matmul / nn.Linear (cuBLASLt) --------------------------------------------------

@@ -16,7 +16,7 @@ int check_launch(const char* what);  // cudaGetLastError() -> return code
 
 int sm_count();  // multiprocessors of the current device (cached per device)
 int fa_fwd_impl();         // b200_set_fa_fwd_impl(): 2 = 128-row q tiles (8 warps), 1 = 64-row q tiles (4 warps)
-int fa_bwd_impl();         // b200_set_fa_bwd_impl(): 2 = 128-row q tiles, 1 = 64-row q tiles (64-row kv tiles either way)
+int fa_bwd_impl();         // b200_set_fa_bwd_impl(): 2 = wgmma kernel, 1 = mma.sync kernel (cross-check)
 // fa_fwd.cu, paged instantiation: prefill half of b200_append_attention
 int launch_fa_prefill_paged(const void* qkv, const void* key_cache, const void* value_cache, void* out, const int32_t* cu_seqlens_q,
                             const int32_t* seq_lens_encoder, const int32_t* seq_lens_decoder, const int32_t* seq_lens_this_time,

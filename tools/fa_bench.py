@@ -1,14 +1,23 @@
-"""Time the flash-attention forward/backward at the Llama-3-8B attention shape on an H100."""
+"""Time the flash-attention forward and both backward kernels (b200_set_fa_bwd_impl 2 = wgmma, 1 = mma.sync) on an H100.
+
+Shapes: the two benchmarked models, Llama-3.2-3B (1 x 4096, 24 / 8 heads) and the Qwen2-1.5B SFT micro-batch (4 x 2048,
+12 / 2 heads), then the Llama-3-8B and Qwen2-7B layouts.  The two backward kernels are timed alternately in one process
+(REPEATS rounds each), so clock and neighbour drift hit both alike; each line gives the median and the spread (min, max).
+"""
 import json
-import math
 import os
+import statistics
+import subprocess
 import sys
 
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-from paddlenlp_b200 import ops  # noqa: E402
+from paddlenlp_b200 import _lib, ops  # noqa: E402
+
+REPEATS = 5
+SHAPES = [(1, 4096, 24, 8), (4, 2048, 12, 2), (1, 4096, 32, 8), (2, 4096, 32, 8), (1, 2048, 28, 4)]
 
 
 def timeit(fn, iters=10, warm=3):
@@ -24,9 +33,22 @@ def timeit(fn, iters=10, warm=3):
     return e0.elapsed_time(e1) / iters
 
 
+def gpu_info():
+    q = "name,power.limit,clocks.sm,clocks.max.sm"
+    r = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True)
+    return dict(zip(q.split(","), (x.strip() for x in r.stdout.splitlines()[0].split(",")))) if r.returncode == 0 else {}
+
+
+def summary(ts):
+    return dict(median_ms=statistics.median(ts), min_ms=min(ts), max_ms=max(ts))
+
+
 def main():
     dev = "cuda:0"
-    for (B, S, nh, kvh) in [(1, 4096, 32, 8), (2, 4096, 32, 8), (1, 2048, 28, 4)]:
+    lib = _lib.load()
+    print(json.dumps(dict(gpu=gpu_info())), flush=True)
+    old_impl = lib.b200_set_fa_bwd_impl(2)
+    for (B, S, nh, kvh) in SHAPES:
         d = 128
         ld = (nh + 2 * kvh) * d
         qkv = torch.randn(B, S, ld, device=dev).to(torch.bfloat16)
@@ -40,21 +62,21 @@ def main():
         dk = dqkv[:, :, nh * d: (nh + kvh) * d].view(B, S, kvh, d)
         dv = dqkv[:, :, (nh + kvh) * d:].view(B, S, kvh, d)
         t_f = timeit(lambda: ops.flash_attn_fwd(q, k, v, out=out))
-        t_b = timeit(lambda: ops.flash_attn_bwd(q, k, v, out, dout, lse, dq, dk, dv))
+        t_b = {1: [], 2: []}
+        for _ in range(REPEATS):
+            for impl in (2, 1):
+                lib.b200_set_fa_bwd_impl(impl)
+                t_b[impl].append(timeit(lambda: ops.flash_attn_bwd(q, k, v, out, dout, lse, dq, dk, dv)))
+        lib.b200_set_fa_bwd_impl(2)
         fl_f = 4.0 * B * nh * S * S * d / 2        # causal
         fl_b = 2.5 * fl_f
-        rec = dict(shape=[B, S, nh, kvh], fwd_ms=t_f, fwd_tflops=fl_f / t_f / 1e9, bwd_ms=t_b, bwd_tflops=fl_b / t_b / 1e9)
-        try:
-            from flash_attn import flash_attn_func
-
-            qq, kk, vv = (t.contiguous().requires_grad_(True) for t in (q, k, v))
-            t_ff = timeit(lambda: flash_attn_func(qq, kk, vv, causal=True))
-            o2 = flash_attn_func(qq, kk, vv, causal=True)
-            t_fb = timeit(lambda: torch.autograd.grad(o2, (qq, kk, vv), dout, retain_graph=True))
-            rec.update(fa2_fwd_ms=t_ff, fa2_bwd_ms=t_fb, fa2_fwd_tflops=fl_f / t_ff / 1e9, fa2_bwd_tflops=fl_b / t_fb / 1e9)
-        except Exception as e:  # library comparison only
-            rec["fa2_error"] = str(e)[:200]
+        rec = dict(shape=[B, S, nh, kvh], fwd_ms=t_f, fwd_tflops=fl_f / t_f / 1e9)
+        for impl in (2, 1):
+            sm = summary(t_b[impl])
+            rec[f"bwd_impl{impl}"] = dict(sm, tflops=fl_b / sm["median_ms"] / 1e9)
+        rec["bwd_impl1_over_impl2"] = rec["bwd_impl1"]["median_ms"] / rec["bwd_impl2"]["median_ms"]
         print(json.dumps(rec), flush=True)
+    lib.b200_set_fa_bwd_impl(old_impl)
     # FlashMask (packed samples): Qwen2-7B SFT row of 2048 tokens holding documents of 700 / 900 / 448 tokens; useful flops only
     B, S, nh, kvh, d = 4, 2048, 28, 4, 128
     docs = [700, 900, 448]
