@@ -68,8 +68,10 @@ class DataParallel(torch.nn.Module):
     """paddle.DataParallel stand-in: forwards to the wrapped model, owns the gradient exchange.
 
     The reference's reducer all-reduces 25 MB buckets while backward is still running (SURVEY.md §8a a12).  Here the
-    gradients live in one flat buffer that is final piecewise — lm_head first, then decoder layer L-1 ... 0, then the
-    embedding and the norm/bias vectors — during the backward of the LAST micro-batch of an optimizer step.  The engine
+    gradients live in one flat buffer that is final piecewise — lm_head first (untied models only), then decoder layer
+    L-1 ... 0, then the embedding and the norm/bias vectors — during the backward of the LAST micro-batch of an optimizer step.
+    With tied embeddings there is no head range: the head's term goes into the embedding gradient at the start of backward,
+    and that range is reported once, after the lookup's scatter has added to it.  The engine
     reports each finished range (`grad_ready_hook`); the range is all-reduced on a side stream while the remaining layers
     are still being differentiated, and `sync_gradients()` reduces whatever is left and joins.  Micro-batches run under
     `no_sync()` accumulate locally, exactly like the reference (trainer.py:1049-1075)."""

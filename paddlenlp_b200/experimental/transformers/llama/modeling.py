@@ -36,13 +36,17 @@ class LlamaForCausalLMInferenceModel(GenerationInferenceModel):
         self.device = self.transformer_block.device
         self.embed_tokens = torch.zeros(c.vocab_size, c.hidden_size, dtype=BF16, device=self.device)
         self.norm_weight = torch.ones(c.hidden_size, dtype=BF16, device=self.device)
-        self.lm_head_weight = torch.zeros(c.hidden_size, c.vocab_size, dtype=BF16, device=self.device)
+        # tied embeddings (llama/modeling.py:1924-1938): the head reads embed_tokens [V, h] as the GEMM's K-major operand
+        self.tied = bool(getattr(c, "tie_word_embeddings", False))
+        self.lm_head_weight = (None if self.tied else
+                               torch.zeros(c.hidden_size, c.vocab_size, dtype=BF16, device=self.device))
 
     # ---- weights (experimental/transformers/llama/modeling.py:901-1060) ----
     @torch.no_grad()
     def set_state_dict(self, sd: Dict[str, torch.Tensor]):
         """Accepts the training-format names (`llama.layers.N.self_attn.q_proj.weight` [in,out], ...) and fuses them into
-        the FusedMultiTransformer layouts: qkv_weight = concat([Wq,Wk,Wv],-1).T, ffn1_weight = concat([Wg,Wu],-1)."""
+        the FusedMultiTransformer layouts: qkv_weight = concat([Wq,Wk,Wv],-1).T, ffn1_weight = concat([Wg,Wu],-1).
+        A tied model reads no `lm_head.weight` (one in `sd` is ignored)."""
         t = self.transformer_block
         pre = self.prefix
         dev = self.device
@@ -52,7 +56,8 @@ class LlamaForCausalLMInferenceModel(GenerationInferenceModel):
 
         self.embed_tokens.copy_(g(f"{pre}.embed_tokens.weight"))
         self.norm_weight.copy_(g(f"{pre}.norm.weight"))
-        self.lm_head_weight.copy_(g("lm_head.weight"))
+        if not self.tied:
+            self.lm_head_weight.copy_(g("lm_head.weight"))
         for i in range(t.L):
             lp = f"{pre}.layers.{i}."
             qkv = torch.cat([g(lp + "self_attn.q_proj.weight"), g(lp + "self_attn.k_proj.weight"),
@@ -74,7 +79,8 @@ class LlamaForCausalLMInferenceModel(GenerationInferenceModel):
         gen = torch.Generator(device=self.device)
         gen.manual_seed(seed)
         t = self.transformer_block
-        for w in [self.embed_tokens, self.lm_head_weight] + t.qkv_weights + t.linear_weights + t.ffn1_weights + t.ffn2_weights:
+        head = [] if self.tied else [self.lm_head_weight]
+        for w in [self.embed_tokens] + head + t.qkv_weights + t.linear_weights + t.ffn1_weights + t.ffn2_weights:
             w.normal_(0.0, std, generator=gen)
         t.weights_changed()
 
@@ -108,6 +114,8 @@ class LlamaForCausalLMInferenceModel(GenerationInferenceModel):
     # ---- forward ----
     def _head(self, hidden):
         hn, _ = ops.add_rmsnorm(hidden, None, self.norm_weight, self.config.rms_norm_eps, want_residual=False)
+        if self.tied:
+            return self.transformer_block._mm(hn, self.embed_tokens, trans_b=True)
         return self.transformer_block._mm(hn, self.lm_head_weight)
 
     def _prefill(self, input_ids, seq_lens_encoder, caches):

@@ -32,23 +32,29 @@ def _is_linear(name: str) -> bool:
     return bool(_TRANSPOSED.search(name))
 
 
-def hf_to_paddle_state_dict(sd: Dict[str, torch.Tensor], model_type: str) -> Dict[str, torch.Tensor]:
+def hf_to_paddle_state_dict(sd: Dict[str, torch.Tensor], model_type: str,
+                            tie_word_embeddings: bool = False) -> Dict[str, torch.Tensor]:
     """`model.X` -> `<model_type>.X`, Linear weights transposed to `[in, out]`; `lm_head.weight` kept at top level.
-    A tied-embedding checkpoint (no lm_head.weight) gets the head materialised from the embedding."""
+    Tied embeddings (llama/modeling.py:1270-1271): the mapping has no lm_head, so a stray `lm_head.weight` is dropped.
+    Untied: a tied-embedding checkpoint (no lm_head.weight) gets a separate head materialised from the embedding."""
     out: Dict[str, torch.Tensor] = {}
     for k, v in sd.items():
-        if _IGNORED.search(k):
+        if _IGNORED.search(k) or (tie_word_embeddings and k == "lm_head.weight"):
             continue
         nk = (model_type + k[len("model"):]) if k.startswith("model.") else k
         out[nk] = v.t().contiguous() if _is_linear(nk) else v
-    if "lm_head.weight" not in out and f"{model_type}.embed_tokens.weight" in out:
+    if not tie_word_embeddings and "lm_head.weight" not in out and f"{model_type}.embed_tokens.weight" in out:
         out["lm_head.weight"] = out[f"{model_type}.embed_tokens.weight"].t().contiguous()
     return out
 
 
-def paddle_to_hf_state_dict(sd: Dict[str, torch.Tensor], model_type: str) -> Dict[str, torch.Tensor]:
+def paddle_to_hf_state_dict(sd: Dict[str, torch.Tensor], model_type: str,
+                            tie_word_embeddings: bool = False) -> Dict[str, torch.Tensor]:
+    """Inverse of hf_to_paddle_state_dict; a tied model's state dict maps to one without `lm_head.weight`."""
     out: Dict[str, torch.Tensor] = {}
     for k, v in sd.items():
+        if tie_word_embeddings and k == "lm_head.weight":
+            continue
         nk = ("model" + k[len(model_type):]) if k.startswith(model_type + ".") else k
         out[nk] = v.t().contiguous() if _is_linear(k) else v
     return out

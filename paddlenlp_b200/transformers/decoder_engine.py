@@ -15,6 +15,8 @@ i.e. 4 wgmma GEMMs, 1 mma.sync attention and 4 HBM-bound fusions; the residual a
 Data layout in HBM
   * ONE flat bf16 parameter buffer and ONE flat bf16 gradient buffer (the buffer the data-parallel all-reduce and
     the AdamW kernel operate on).  Matrices first (weight-decayed), then norm weights and biases (not decayed).
+  * config.tie_word_embeddings: the layout has no `head` entry; the logits are hf @ E^T with E = embed [V, h]
+    (llama/modeling.py:1924-1938, LlamaLMHead(transpose_y=True)) and both gradient terms land in the one embed gradient.
   * q/k/v weights are stored fused as [hidden, (nh + 2*kvh) * d] (= concat of the reference's three [in,out]
     matrices along out) and gate/up as [hidden, 2*I]; the reference names are exposed as column-slice views.
   * activations are token-major [T, features] bf16; q/k/v are strided views of the packed QKV projection.
@@ -53,6 +55,7 @@ class DecoderEngine:
         self.L = config.num_hidden_layers
         self.eps = config.rms_norm_eps
         self.qkv_bias = config.model_type == "qwen2"
+        self.tied = bool(getattr(config, "tie_word_embeddings", False))
         if self.d != 128:
             raise NotImplementedError(f"head_dim {self.d}: the attention kernels are written for head_dim 128")
         if self.h % 8 or self.I % 8 or self.V % 8:
@@ -81,7 +84,8 @@ class DecoderEngine:
             vecs += [(f"l{i}.ln1", (self.h,)), (f"l{i}.ln2", (self.h,))]
             if self.qkv_bias:
                 vecs += [(f"l{i}.qkv_b", (self.qkv_n,))]
-        mats += [("head", (self.h, self.V))]
+        if not self.tied:
+            mats += [("head", (self.h, self.V))]
         vecs += [("norm", (self.h,))]
         self._offsets: Dict[str, Tuple[int, Tuple[int, ...]]] = {}
         off = 0
@@ -114,7 +118,8 @@ class DecoderEngine:
         lm_head weight, o_proj and down_proj scaled by 1/sqrt(2L), RMSNorm weights 1, biases 0.
 
         on_host=True draws every tensor in fp32 from ONE seeded CPU generator in the reference's parameter order
-        (embed_tokens, then per layer q, k, v, o[, q/k/v bias = 0], gate, up, down, then lm_head), applies the 1/sqrt(2L)
+        (embed_tokens, then per layer q, k, v, o[, q/k/v bias = 0], gate, up, down, then lm_head unless the embeddings are
+        tied: a tied model's parameter list has no lm_head), applies the 1/sqrt(2L)
         factor in fp32 and rounds to bf16 once — so a CPU restatement that draws the same way holds the same bits
         (SURVEY.md §8a row a10).  Default: host for models below 2^28 parameters, device draws (bf16 normals straight
         into the flat buffer, same distribution, no 30 GB fp32 host round trip) above."""
@@ -170,7 +175,8 @@ class DecoderEngine:
                 if self.qkv_bias:
                     self.p[f"l{i}.qkv_b"].zero_()
             self.p["norm"].fill_(1.0)
-            self.p["head"].copy_(draw(self.h, self.V))
+            if not self.tied:
+                self.p["head"].copy_(draw(self.h, self.V))
         self._bias_f32.clear()
 
     def named_views(self, grads: bool = False, flat: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
@@ -202,10 +208,13 @@ class DecoderEngine:
             out[lp + "input_layernorm.weight"] = src[f"l{i}.ln1"]
             out[lp + "post_attention_layernorm.weight"] = src[f"l{i}.ln2"]
         out[f"{pre}.norm.weight"] = src["norm"]
-        out["lm_head.weight"] = src["head"]
+        if not self.tied:
+            out["lm_head.weight"] = src["head"]
         return out
 
     def load_state_dict(self, sd: Dict[str, torch.Tensor]):
+        """Copies every named view from `sd`.  Entries without a view are ignored: a tied model takes a state dict that
+        still carries `lm_head.weight` and keeps its embedding (the reference's tie_weights() after load)."""
         views = self.named_views()
         missing = [k for k in views if k not in sd]
         if missing:
@@ -322,12 +331,18 @@ class DecoderEngine:
         hf, rstd_f = ops.rmsnorm_fwd(x, self.p["norm"], self.eps)
         return B, S, ids, pos, x, hf, rstd_f
 
+    def _logits(self, hf: torch.Tensor) -> torch.Tensor:
+        """[T, V] = hf @ head, or hf @ E^T when tied (E [V, h] is the GEMM's K-major B operand)."""
+        if self.tied:
+            return ops.gemm(hf, self.p["embed"], trans_b=True)
+        return ops.gemm(hf, self.p["head"])
+
     @torch.no_grad()
     def forward_logits(self, input_ids, position_ids=None, attn_mask_startend_row_indices=None) -> torch.Tensor:
         """Inference forward: logits [B, S, V] (bf16).  Nothing is saved for backward."""
         B, S, ids, pos, x, hf, _ = self.hidden_states(input_ids, position_ids, save=None,
                                                       attn_mask_startend_row_indices=attn_mask_startend_row_indices)
-        logits = ops.gemm(hf, self.p["head"])
+        logits = self._logits(hf)
         return logits.view(B, S, self.V)
 
     @torch.no_grad()
@@ -339,7 +354,7 @@ class DecoderEngine:
         save: Optional[list] = [] if keep_for_backward else None
         B, S, ids, pos, x, hf, rstd_f = self.hidden_states(input_ids, position_ids, save=save,
                                                            attn_mask_startend_row_indices=attn_mask_startend_row_indices)
-        logits = ops.gemm(hf, self.p["head"])
+        logits = self._logits(hf)
         lab = labels.to(device=self.device, dtype=torch.int64, non_blocking=True).contiguous().view(-1)
         loss_out, loss_tok, lse = ops.ce_fwd(logits, lab, ignore_index)
         if keep_for_backward:
@@ -354,7 +369,7 @@ class DecoderEngine:
         save: list = []
         B, S, ids, pos, x, hf, rstd_f = self.hidden_states(input_ids, position_ids, save=save,
                                                            attn_mask_startend_row_indices=attn_mask_startend_row_indices)
-        logits = ops.gemm(hf, self.p["head"])
+        logits = self._logits(hf)
         self._saved = dict(B=B, S=S, ids=ids, pos=pos, mask=self._mask, layers=save, x_last=x, hf=hf, rstd_f=rstd_f,
                            logits=None, labels=None)
         return logits.view(B, S, self.V)
@@ -387,10 +402,16 @@ class DecoderEngine:
             dlogits = ops.ce_bwd_(st["logits"], st["labels"], st["loss_tok"], st["lse"], st["loss_out"], grad_scale,
                                   grad_scale_dev)
         hook, self.grad_ready_hook = self.grad_ready_hook, None      # one backward per arming
-        dhf = ops.gemm(dlogits, p["head"], trans_b=True)
-        ops.gemm(st["hf"], dlogits, out=g["head"], trans_a=True, accumulate=acc)
-        if hook is not None:
-            hook(*self._range("head", "head"))
+        if self.tied:
+            # dhf = dlogits @ E; the head's term dlogits^T @ hf starts (or adds to) the embedding gradient, and the token
+            # scatter of embedding_bwd adds on top after the layers
+            dhf = ops.gemm(dlogits, p["embed"])
+            ops.gemm(dlogits, st["hf"], out=g["embed"], trans_a=True, accumulate=acc)
+        else:
+            dhf = ops.gemm(dlogits, p["head"], trans_b=True)
+            ops.gemm(st["hf"], dlogits, out=g["head"], trans_a=True, accumulate=acc)
+            if hook is not None:
+                hook(*self._range("head", "head"))
         del dlogits
         st["logits"] = None
         dx = ops.rmsnorm_bwd(dhf, st["x_last"], p["norm"], st["rstd_f"], g["norm"], accumulate_dw=acc)
@@ -401,7 +422,7 @@ class DecoderEngine:
             layers[i] = None
             if hook is not None:
                 hook(*self._range(f"l{i}.qkv_w", f"l{i}.down_w"))       # this layer's four matrices are contiguous
-        if not acc:
+        if not acc and not self.tied:
             g["embed"].zero_()
         ops.embedding_bwd(st["ids"], dx, g["embed"])
         if hook is not None:

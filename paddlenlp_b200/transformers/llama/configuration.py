@@ -35,8 +35,6 @@ class LlamaConfig(PretrainedConfig):
             raise ValueError(f"Unknown RoPE scaling type {rope_scaling_type}")      # llama/modeling.py:864
         if alibi:
             raise NotImplementedError("alibi attention bias is outside the hot path this build covers")
-        if tie_word_embeddings:
-            raise NotImplementedError("tie_word_embeddings: Llama-3 / Qwen2-7B use an untied lm_head")
         super().__init__(pad_token_id=pad_token_id, bos_token_id=bos_token_id, eos_token_id=eos_token_id,
                          tie_word_embeddings=tie_word_embeddings, **kwargs)
 
@@ -57,7 +55,9 @@ class LlamaConfig(PretrainedConfig):
     # public presets used by bench / tests (hyper-parameters from the public model cards, SURVEY.md §8)
     @classmethod
     def llama3_2_3b(cls, **kw):
-        """Llama-3.2-3B shapes (head_dim 128, GQA 24/8) with untied input and output embeddings."""
+        """Llama-3.2-3B shapes (head_dim 128, GQA 24/8).  The released model ties its input and output embeddings; the preset
+        keeps a separate lm_head by default (the benchmarked model).  Pass `tie_word_embeddings=True` for the released layout:
+        the logits then read the embedding matrix, and its V x h parameters, gradients and optimizer state exist once."""
         base = dict(vocab_size=128256, hidden_size=3072, intermediate_size=8192, num_hidden_layers=28,
                     num_attention_heads=24, num_key_value_heads=8, rms_norm_eps=1e-5, rope_theta=500000.0,
                     max_position_embeddings=8192, seq_length=4096, bos_token_id=128000, eos_token_id=128001)

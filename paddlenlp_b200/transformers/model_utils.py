@@ -106,28 +106,21 @@ class PretrainedModel(nn.Module):
         views = self.engine.named_views()
         mt = self.engine.prefix
         seen = set()
-        embed = None
         with torch.no_grad():
             for k, v in items:
                 if convert_from_hf:
-                    conv = cu.hf_to_paddle_state_dict({k: v}, mt)
+                    conv = cu.hf_to_paddle_state_dict({k: v}, mt, tie_word_embeddings=self.engine.tied)
                     if k != "lm_head.weight":
-                        conv.pop("lm_head.weight", None)      # tied-head fallback is resolved after the loop
+                        conv.pop("lm_head.weight", None)      # one tensor at a time: no head materialised from the embedding
                 else:
                     conv = {k: v}
                 for nk, nv in conv.items():
                     if nk not in views:
-                        continue                      # e.g. rotary inv_freq buffers (llama/modeling.py:1240)
+                        continue                      # rotary inv_freq buffers (llama/modeling.py:1240), a tied model's lm_head
                     if tuple(nv.shape) != tuple(views[nk].shape):
                         raise ValueError(f"{nk}: shape {tuple(nv.shape)} != {tuple(views[nk].shape)}")
                     views[nk].copy_(nv.to(device=self.engine.device, dtype=torch.bfloat16))
                     seen.add(nk)
-                    if nk.endswith("embed_tokens.weight"):
-                        embed = nk
-        if "lm_head.weight" not in seen and embed is not None and getattr(self.config, "tie_word_embeddings", False):
-            with torch.no_grad():
-                views["lm_head.weight"].copy_(views[embed].t())
-            seen.add("lm_head.weight")
         missing = [k for k in views if k not in seen]
         if missing:
             raise KeyError(f"checkpoint is missing {len(missing)} tensors, e.g. {missing[:3]}")
@@ -136,7 +129,8 @@ class PretrainedModel(nn.Module):
     def save_pretrained(self, save_directory: str, max_shard_size="5GB", safe_serialization: bool = True,
                         hf_format: bool = False, unified_checkpoint: bool = False):
         """config.json + safetensors shards + index (model_utils.py save_pretrained / shard_checkpoint :562-640).
-        `hf_format=True` writes HuggingFace names and `[out, in]` Linear layouts instead of the Paddle ones."""
+        `hf_format=True` writes HuggingFace names and `[out, in]` Linear layouts instead of the Paddle ones.  A model with
+        tied embeddings writes no `lm_head.weight`."""
         from . import conversion_utils as cu
 
         os.makedirs(save_directory, exist_ok=True)
@@ -146,7 +140,7 @@ class PretrainedModel(nn.Module):
             torch.save({k: v.cpu().contiguous() for k, v in sd.items()}, os.path.join(save_directory, "model_state.pt"))
             return
         if hf_format:
-            sd = cu.paddle_to_hf_state_dict(sd, self.engine.prefix)
+            sd = cu.paddle_to_hf_state_dict(sd, self.engine.prefix, tie_word_embeddings=self.engine.tied)
         # unified_checkpoint: always `model-0000i-of-0000N.safetensors` + index, even for one shard (the Trainer's layout)
         cu.save_sharded(sd, save_directory, max_shard_size=max_shard_size, always_index=unified_checkpoint)
 

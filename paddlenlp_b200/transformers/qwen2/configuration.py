@@ -29,15 +29,14 @@ class Qwen2Config(PretrainedConfig):
         self.attention_dropout = attention_dropout
         if use_sliding_window:
             raise NotImplementedError("sliding-window attention is outside the hot path this build covers")
-        if tie_word_embeddings:
-            raise NotImplementedError("tie_word_embeddings: Qwen2-7B uses an untied lm_head")
         super().__init__(pad_token_id=pad_token_id, bos_token_id=bos_token_id, eos_token_id=eos_token_id,
                          tie_word_embeddings=tie_word_embeddings, **kwargs)
 
     @classmethod
     def qwen2_1_5b(cls, **kw):
-        """Qwen2-1.5B shapes (head_dim 128, GQA 12/2).  The released model ties its input and output embeddings; this
-        implementation keeps an untied lm_head (the same shapes and FLOPs, 0.23 G more parameters)."""
+        """Qwen2-1.5B shapes (head_dim 128, GQA 12/2).  The released model ties its input and output embeddings; the preset
+        keeps a separate lm_head by default (the benchmarked model: the same shapes and FLOPs, 0.23 G more parameters).  Pass
+        `tie_word_embeddings=True` for the released layout."""
         base = dict(vocab_size=151936, hidden_size=1536, intermediate_size=8960, num_hidden_layers=28,
                     num_attention_heads=12, num_key_value_heads=2, rms_norm_eps=1e-6, rope_theta=1000000.0,
                     max_position_embeddings=32768, seq_length=2048)
