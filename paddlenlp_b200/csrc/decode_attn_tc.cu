@@ -233,9 +233,9 @@ static int launch(const Params& p, int G, int64_t num_splits, cudaStream_t strea
     launch_pdl(decode_attention_bulk_kernel<GG, PAGED>, grid, dim3(NUM_THREADS), SMEM_BYTES, stream, p);             \
   } break;
   switch (G) {
-    B200_DAB(1) B200_DAB(2) B200_DAB(4) B200_DAB(7) B200_DAB(8)
+    B200_DAB(1) B200_DAB(2) B200_DAB(3) B200_DAB(4) B200_DAB(5) B200_DAB(6) B200_DAB(7) B200_DAB(8)
     default:
-      return fail_arg("decode_attention_tc: GQA group size %d not instantiated (1, 2, 4, 7, 8)", G);
+      return fail_arg("decode_attention_tc: GQA group size %d not instantiated (1 to 8)", G);
   }
 #undef B200_DAB
   int rc = check_launch("decode_attention_tc");

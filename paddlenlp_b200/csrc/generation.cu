@@ -963,9 +963,9 @@ extern "C" int b200_decode_attention(const void* qkv, const void* cache, const i
                                                             (int)num_kv_heads, (int)max_len, ld, sl2);              \
     break;
   switch (G) {
-    B200_DA(1) B200_DA(2) B200_DA(4) B200_DA(7) B200_DA(8)
+    B200_DA(1) B200_DA(2) B200_DA(3) B200_DA(4) B200_DA(5) B200_DA(6) B200_DA(7) B200_DA(8)
     default:
-      return fail_arg("decode_attention: GQA group size %d not instantiated (1, 2, 4, 7, 8)", G);
+      return fail_arg("decode_attention: GQA group size %d not instantiated (1 to 8)", G);
   }
 #undef B200_DA
   int rc = check_launch("decode_attention");
@@ -1470,7 +1470,8 @@ extern "C" int b200_save_output_stream(const int64_t* next_tokens, const int32_t
 //                                for prompt and decode rows alike); decode rows' q are also gathered into a dense [B, ld] buffer
 //   2. fa_fwd_kernel<8, PAGED>   prompt rows: flash attention, q tiles of 128 rows, K/V rows gathered page by page with
 //                                cp.async, causal band offset by the cached prefix (chunked prefill)
-//   3. decode_attention_tc<PAGED> decode rows (the decode step's kernel; sequences of the other kinds have length -1 = no work)
+//   3. decode_attention_tc<PAGED> decode rows (the decode step's kernel; sequences of the other kinds, idle slots included,
+//                                have length -1 = no work)
 //   4. scatter of the decode rows' outputs back to their token rows
 // No host synchronisation: each kernel decides from the device-resident length arrays which sequences are its own (the
 // reference plans tiles on the device too, but copies the plan sizes to the host).
@@ -1485,6 +1486,11 @@ __global__ void append_rope_write_kernel(bf16* __restrict__ qkv, const CacheView
                                          int nh, int max_pos, int64_t ld) {
   const int kvh = cv.kvh, d = cv.d;
   const int tok = blockIdx.x;
+  // an idle slot owns no token row, so no block below writes its decode length: mark it here, or the decode kernel and the
+  // scatter would act on whatever length the workspace held from an earlier call (and write into the next sequence's row)
+  if (tok == 0)
+    for (int bb = threadIdx.x; bb < B; bb += blockDim.x)
+      if (__ldg(seq_this + bb) <= 0) dec_len[bb] = -1;
   // which sequence owns this token row: the last b with cu_q[b] <= tok
   int lo = 0, hi = B;
   while (hi - lo > 1) {

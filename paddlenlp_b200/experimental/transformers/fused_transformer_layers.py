@@ -58,6 +58,14 @@ class FusedMultiTransformerConfig:
 
 class FusedMultiTransformerBase:
     def __init__(self, config: FusedMultiTransformerConfig, device=None):
+        # every cache path ends in the decode-attention kernels: refuse a head layout they do not cover now, not at the
+        # first decode step after a prefill
+        nh, kvh = config.num_heads, config.kv_num_heads
+        if nh % kvh:
+            raise ValueError(f"num_heads {nh} is not a multiple of kv_num_heads {kvh}")
+        if nh // kvh not in ops.DECODE_GQA_GROUPS:
+            raise ValueError(f"GQA group size {nh // kvh} (num_heads {nh} / kv_num_heads {kvh}) is not supported by the decode "
+                             f"attention kernels ({ops.DECODE_GQA_GROUPS.start} to {ops.DECODE_GQA_GROUPS.stop - 1})")
         if device is None:
             if not torch.cuda.is_available():
                 raise RuntimeError("FusedMultiTransformer needs a CUDA device: there is no CPU implementation")

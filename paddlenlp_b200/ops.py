@@ -14,6 +14,10 @@ from . import _lib
 from ._lib import call, ptr, stream_ptr
 
 BF16 = torch.bfloat16
+# The decode-attention kernels (dense, paged and the decode rows of append_attention) are compiled for these GQA group sizes
+# (query heads per kv head) and accept at most this many split-KV partials per (sequence, head).
+DECODE_GQA_GROUPS = range(1, 9)
+DECODE_MAX_SPLITS = 64
 
 
 def _chk(t: torch.Tensor, name: str, dtype=BF16):
@@ -510,7 +514,10 @@ def decode_rope_append(qkv, cache, cos, sin, seq_lens, nh, kvh, d):
 
 
 def decode_attention(qkv, cache, seq_lens, nh, kvh, d, softmax_scale=None, out=None, num_splits: int = 0, impl: str = "tc"):
-    """impl "tc" / "simt": both run the streaming CUDA-core kernel (half-warp per cache row); "tc" keeps its split heuristic."""
+    """Attention of one query row per sequence over the dense cache [2, B, kvh, max_len, d]: sequence b attends to its first
+    min(seq_lens[b] + 1, max_len) rows (the new token was appended at row seq_lens[b]).  GQA group nh / kvh in 1..8,
+    d = 128.  impl "tc": the bulk-copy kernel (decode_attn_tc.cu); "simt": the CUDA-core kernel of generation.cu with plain
+    global loads, the cross-check.  num_splits <= 0 lets each pick its split-KV count (at most 64)."""
     _chk(qkv, "qkv"); _chk(cache, "cache"); _chk(seq_lens, "seq_lens", torch.int32)
     B = qkv.shape[0]
     if out is None:
@@ -520,14 +527,14 @@ def decode_attention(qkv, cache, seq_lens, nh, kvh, d, softmax_scale=None, out=N
     max_len = cache.shape[3]
     if impl == "tc":
         if num_splits <= 0:
-            # persistent CTAs walk (split, b, kv head) items round-robin; split only when there are too few (b, kv head)
-            # pairs to give every SM ~3 items (a split costs partial traffic, a merge launch and an item boundary)
-            num_splits = max(1, min((max_len + 127) // 128, (3 * 132 + B * kvh - 1) // (B * kvh)))
+            # split only when there are too few (b, kv head) pairs to give every SM ~3 CTAs (a split costs partial traffic,
+            # a merge launch and a CTA boundary)
+            num_splits = max(1, min((max_len + 127) // 128, (3 * 132 + B * kvh - 1) // (B * kvh), DECODE_MAX_SPLITS))
         fn = "b200_decode_attention_tc"
     elif impl == "simt":
         if num_splits <= 0:
             # enough CTAs for ~8 per SM without making the ranges shorter than ~64 cache rows at full length
-            num_splits = max(1, min(max_len // 64, (8 * 132 + B * kvh - 1) // (B * kvh)))
+            num_splits = max(1, min(max_len // 64, (8 * 132 + B * kvh - 1) // (B * kvh), DECODE_MAX_SPLITS))
         fn = "b200_decode_attention"
     else:
         raise ValueError(f"decode_attention impl {impl!r}")
@@ -569,6 +576,8 @@ def decode_rope_append_paged(qkv, key_cache, value_cache, block_tables, cos, sin
 
 def decode_attention_paged(qkv, key_cache, value_cache, block_tables, seq_lens, nh, softmax_scale=None, out=None,
                            num_splits: int = 0):
+    """decode_attention over the paged cache: sequence b's row t lives in page block_tables[b, t // block_size] (entries
+    past a sequence's pages may be -1); it attends to min(seq_lens[b] + 1, max_blocks_per_seq * block_size) rows."""
     _chk(qkv, "qkv"); _chk(seq_lens, "seq_lens", torch.int32)
     nb, kvh, bs, d, mb = _paged_geom(key_cache, value_cache, block_tables)
     B = qkv.shape[0]
@@ -578,7 +587,7 @@ def decode_attention_paged(qkv, key_cache, value_cache, block_tables, seq_lens, 
         softmax_scale = 1.0 / math.sqrt(d)
     max_len = mb * bs
     if num_splits <= 0:
-        num_splits = max(1, min((max_len + 127) // 128, (3 * 132 + B * kvh - 1) // (B * kvh)))
+        num_splits = max(1, min((max_len + 127) // 128, (3 * 132 + B * kvh - 1) // (B * kvh), DECODE_MAX_SPLITS))
     ws = None
     if num_splits > 1:
         ws = _workspace(_lib.load().b200_decode_attention_workspace_bytes(B, nh, num_splits), qkv.device, "decode_attn")
@@ -623,7 +632,7 @@ def append_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_dec
     if softmax_scale is None:
         softmax_scale = 1.0 / math.sqrt(d)
     if num_splits <= 0:
-        num_splits = max(1, min((mb * bs + 127) // 128, (3 * 132 + B * kvh - 1) // (B * kvh)))
+        num_splits = max(1, min((mb * bs + 127) // 128, (3 * 132 + B * kvh - 1) // (B * kvh), DECODE_MAX_SPLITS))
     ws = _workspace(_lib.load().b200_append_attention_workspace_bytes(B, nh, kvh, d, num_splits), qkv.device, "append_attn")
     call("b200_append_attention", ptr(qkv), ptr(key_cache), ptr(value_cache), ptr(seq_lens_encoder), ptr(seq_lens_decoder),
          ptr(seq_lens_this_time), ptr(cu_seqlens_q), ptr(block_tables), ptr(cos), ptr(sin), ptr(out), ptr(ws), B, token_num,
