@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define B200NLP_ABI_VERSION 1
+#define B200NLP_ABI_VERSION 2
 
 #ifndef __CUDA_RUNTIME_API_H__
 typedef struct CUstream_st* cudaStream_t;
@@ -40,12 +40,11 @@ int b200_device_check(void);
  * touching operands or outputs.  Used for the decode-step chain. */
 int b200_set_pdl(int enable);
 /* q-tile height of b200_fa_fwd / b200_fa_fwd_flashmask (returns the previous setting; NOT an error code): 2 (default) = 128
- * rows (8 warps) per CTA, 1 = 64 rows (4 warps).  Same rounding points; kept switchable for A/B measurements.  The initial
- * value can be set with the environment variable B200_FA_FWD_IMPL. */
+ * rows (8 warps) per CTA, 1 = 64 rows (4 warps).  Same rounding points; kept switchable for A/B measurements. */
 int b200_set_fa_fwd_impl(int impl);
 /* Kernel of b200_fa_bwd / b200_fa_bwd_flashmask (returns the previous setting): 2 (default) = the warp-specialised wgmma
  * kernel (128-row kv tiles, TMA-fed 64-row q tiles, TMA reduce-adds), 1 = the mma.sync kernel (64-row kv and q tiles), kept as
- * the cross-check.  Same rounding points.  Environment override: B200_FA_BWD_IMPL. */
+ * the cross-check.  Same rounding points. */
 int b200_set_fa_bwd_impl(int impl);
 
 /* ---- GEMM: replaces paddle.matmul / nn.Linear (cuBLASLt) --------------------------------------------------
@@ -63,15 +62,14 @@ int b200_set_fa_bwd_impl(int impl);
 int b200_gemm_bf16(const void* A, const void* B, void* C, const float* bias, int64_t M, int64_t N, int64_t K,
                    int64_t lda, int64_t ldb, int64_t ldc, int a_mn_major, int b_mn_major, int accumulate,
                    cudaStream_t stream);
-/* Same with a fused residual epilogue and tuning knobs.
+/* Same with a fused residual epilogue and a limit on the persistent grid.
  *   residual (bf16 [M,N], leading dimension ldr; exclusive with accumulate):
  *       C = bf16( bf16(acc + bias) + residual )  — the Linear-output rounding followed by the decoder layer's residual
  *       add (llama/modeling.py:1212, 1218), i.e. the reference's two rounding points in one kernel.
- *   cta_group 1 or 2: accepted for compatibility; H100 has no CTA-pair MMA, both run one CTA per 128x256 tile;
  *   max_ctas > 0 limits the persistent grid (used to leave SMs to a concurrent kernel). */
 int b200_gemm_bf16_ex(const void* A, const void* B, void* C, const float* bias, const void* residual, int64_t M,
                       int64_t N, int64_t K, int64_t lda, int64_t ldb, int64_t ldc, int64_t ldr, int a_mn_major,
-                      int b_mn_major, int accumulate, int cta_group, int max_ctas, cudaStream_t stream);
+                      int b_mn_major, int accumulate, int max_ctas, cudaStream_t stream);
 
 /* Weight-streaming GEMM for the decode step (M <= ~128 tokens): same math as b200_gemm_bf16 (C = op(A) op(B) + bias, one
  * rounding), but K is split over CTAs (split_k, 0 = auto) so that every SM streams part of the weight matrix; fp32 partial
@@ -88,14 +86,16 @@ int b200_gemm_bf16_splitk(const void* A, const void* B, void* C, const float* bi
  *   GU[M, 2I] = bf16(X[M,K] * W[K,2I])  (gate columns [0,I), up columns [I,2I); kept for the backward),
  *   Mout[M, I] = bf16(silu(gate) * up)  with gate/up rounded to bf16 first (the unfused rounding points).
  * A 256-column wgmma tile is formed from 128 gate columns and the 128 up columns of the same channels, so no interleaved
- * weight layout is needed; requires I % 128 == 0.  Bit-identical to b200_gemm_bf16 followed by b200_swiglu_fwd. */
+ * weight layout is needed; requires I % 64 == 0 (a last tile of 64 channels leaves half of it unused).  GU == NULL: gate|up are
+ * not stored (the decode step's ffn1 + fused_bias_act("swiglu"), fused_transformer_layers.py:100-168).  Bit-identical to
+ * b200_gemm_bf16 followed by b200_swiglu_fwd. */
 int b200_gemm_swiglu_bf16(const void* X, const void* W, void* GU, void* Mout, int64_t M, int64_t inter, int64_t K, int64_t ldx,
-                          int64_t ldw, int64_t ldgu, int64_t ldm, int cta_group, cudaStream_t stream);
+                          int64_t ldw, int64_t ldgu, int64_t ldm, cudaStream_t stream);
 /* Backward twin: the down-projection dX GEMM with the SwiGLU backward in its epilogue.
  *   d(m) = dY[M,K] * Wdown[I,K]^T (never written);  DGU[M, 2I] = [ d(m) * up * silu'(gate) | d(m) * silu(gate) ],
  * GU = the saved gate|up projection [M, 2I].  Bit-identical to b200_gemm_bf16 (b_mn_major = 0) + b200_swiglu_bwd.  I % 64 == 0. */
 int b200_gemm_swiglu_bwd_bf16(const void* dY, const void* Wdown, const void* GU, void* DGU, int64_t M, int64_t inter, int64_t K,
-                              int64_t lddy, int64_t ldw, int64_t ldgu, int64_t lddgu, int cta_group, cudaStream_t stream);
+                              int64_t lddy, int64_t ldw, int64_t ldgu, int64_t lddgu, cudaStream_t stream);
 
 /* ---- RMSNorm: replaces fused_ln.fused_rms_norm / fast_ln (apex-derived custom ops) --------------------------
  * fwd : y = bf16( bf16(x * rstd) * w ), rstd[row] = rsqrt(mean(x^2) + eps) in fp32 (saved for the backward).
@@ -130,12 +130,6 @@ int b200_swiglu_fwd(const void* gate_up, void* out, int64_t rows, int64_t inter,
 /* Same, gate|up given as the fp32 split-K workspace [rows, 2*inter] of the producing GEMM (rounded to bf16 here, workspace
  * re-zeroed): the decode step's ffn1 -> fused_bias_act("swiglu") pair (fused_transformer_layers.py:100-168). */
 int b200_swiglu_fwd_f32(float* gate_up_f32_ws, void* out, int64_t rows, int64_t inter, cudaStream_t stream);
-/* Decode-step ffn1 + SwiGLU in one kernel (M <= 64 token rows): act[M, inter] = bf16(silu(g) * u) with g|u = bf16(X W).
- * W [K, 2*inter] is the reference-layout fused ffn1 weight (gate | up): the wgmma GEMM with 64-row tiles streams 128 gate
- * columns and the up columns of the same channels per tile and applies the SwiGLU in its epilogue; gate|up are not stored
- * (fused_transformer_layers.py:100-168 fused_bias_act("swiglu") after ffn1).  inter % 64 == 0; ldact = row stride of act. */
-int b200_gemm_swiglu_skinny(const void* X, const void* W_gate_up, void* act, int64_t M, int64_t inter, int64_t K,
-                            int64_t ldx, int64_t ldw, int64_t ldact, cudaStream_t stream);
 int b200_swiglu_bwd(const void* gate_up, const void* dout, void* dgate_up, int64_t rows, int64_t inter,
                     cudaStream_t stream);
 /* ---- Embedding gather / scatter-add (nn.Embedding, llama/modeling.py:1465-1468, 1634). ids are int64. */

@@ -27,9 +27,9 @@ _SIGNATURES = {
     "b200_set_fa_fwd_impl": [I],
     "b200_set_fa_bwd_impl": [I],
     "b200_gemm_bf16": [P, P, P, P, I64, I64, I64, I64, I64, I64, I, I, I, P],
-    "b200_gemm_bf16_ex": [P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I, I, I, I, I, P],
-    "b200_gemm_swiglu_bf16": [P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I, P],
-    "b200_gemm_swiglu_bwd_bf16": [P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I, P],
+    "b200_gemm_bf16_ex": [P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I, I, I, I, P],
+    "b200_gemm_swiglu_bf16": [P, P, P, P, I64, I64, I64, I64, I64, I64, I64, P],
+    "b200_gemm_swiglu_bwd_bf16": [P, P, P, P, I64, I64, I64, I64, I64, I64, I64, P],
     "b200_gemm_splitk_workspace_bytes": [I64, I64],
     "b200_gemm_bf16_splitk": [P, P, P, P, P, I64, I64, I64, I64, I64, I64, I, I, I, P],
     "b200_rmsnorm_fwd": [P, P, P, P, I64, I64, F, P],
@@ -40,7 +40,6 @@ _SIGNATURES = {
     "b200_rope_inplace": [P, P, P, P, I64, I64, I64, I64, I64, I, P],
     "b200_swiglu_fwd": [P, P, I64, I64, P],
     "b200_swiglu_fwd_f32": [P, P, I64, I64, P],
-    "b200_gemm_swiglu_skinny": [P, P, P, I64, I64, I64, I64, I64, I64, P],
     "b200_swiglu_bwd": [P, P, P, I64, I64, P],
     "b200_embedding_fwd": [P, P, P, I64, I64, I64, P],
     "b200_embedding_bwd": [P, P, P, I64, I64, I64, P],
@@ -100,12 +99,6 @@ _RESTYPE = {
 def exported_symbols():
     """Names include/b200nlp.h declares (kept in sync by tests/test_abi.py)."""
     return sorted(_SIGNATURES)
-
-
-def register(name, argtypes, restype=None):
-    _SIGNATURES[name] = argtypes
-    if restype is not None:
-        _RESTYPE[name] = restype
 
 
 def load():

@@ -1,5 +1,4 @@
 // C-ABI plumbing: error string, version, device checks, tensor-map encoding.
-#include <stdlib.h>
 #include <string.h>
 
 #include <mutex>
@@ -36,15 +35,10 @@ int check_launch(const char* what) {
 
 static int g_pdl = 0;
 bool pdl_enabled() { return g_pdl != 0; }
-// attention kernel tile sizes (fa_fwd.cu, fa_bwd.cu); the initial value can be overridden with B200_FA_FWD_IMPL /
-// B200_FA_BWD_IMPL for A/B runs of unmodified scripts
-static int env_int(const char* name, int dflt) {
-  const char* v = getenv(name);
-  return (v && *v) ? atoi(v) : dflt;
-}
-static int g_fa_fwd_impl = env_int("B200_FA_FWD_IMPL", 2);
+// attention kernel tile sizes (fa_fwd.cu, fa_bwd.cu): b200_set_fa_fwd_impl / b200_set_fa_bwd_impl
+static int g_fa_fwd_impl = 2;
 int fa_fwd_impl() { return g_fa_fwd_impl; }
-static int g_fa_bwd_impl = env_int("B200_FA_BWD_IMPL", 2);
+static int g_fa_bwd_impl = 2;
 int fa_bwd_impl() { return g_fa_bwd_impl; }
 
 int sm_count() {
@@ -77,7 +71,7 @@ static EncodeTiledFn get_encode_fn() {
 }
 
 static int encode_tmap(CUtensorMap* out, CUtensorMapDataType dtype, const void* base, int rank, const uint64_t* dims,
-                       const uint64_t* strides, const uint32_t* box, CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B);
+                       const uint64_t* strides, const uint32_t* box);
 
 int encode_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides,
                      const uint32_t* box) {
@@ -87,13 +81,9 @@ int encode_tmap_f32(CUtensorMap* out, const void* base, int rank, const uint64_t
                     const uint32_t* box) {
   return encode_tmap(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, base, rank, dims, strides, box);
 }
-int encode_tmap_bf16_linear(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides,
-                            const uint32_t* box) {
-  return encode_tmap(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, base, rank, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE);
-}
 
 static int encode_tmap(CUtensorMap* out, CUtensorMapDataType dtype, const void* base, int rank, const uint64_t* dims,
-                       const uint64_t* strides, const uint32_t* box, CUtensorMapSwizzle swizzle) {
+                       const uint64_t* strides, const uint32_t* box) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) return fail_arg("cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
   cuuint64_t gdim[5];
@@ -110,7 +100,7 @@ static int encode_tmap(CUtensorMap* out, CUtensorMapDataType dtype, const void* 
   for (int i = 0; i < rank - 1; ++i)
     if (gstr[i] % 16 != 0) return fail_arg("tensor map stride %llu not a multiple of 16 bytes", (unsigned long long)gstr[i]);
   CUresult r = fn(out, dtype, static_cast<cuuint32_t>(rank), const_cast<void*>(base), gdim,
-                  gstr, bdim, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
+                  gstr, bdim, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS)
     return fail_arg("cuTensorMapEncodeTiled failed (CUresult %d) rank=%d dims=[%llu,%llu] box=[%u,%u]", (int)r, rank,

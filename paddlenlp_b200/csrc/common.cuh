@@ -20,23 +20,6 @@ typedef __nv_bfloat16 bf16;
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
-__device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31u; }
-
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.u32 %0, 1, 0, P;\n\t}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
@@ -109,17 +92,6 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* tm) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tm)) : "memory");
 }
 // global -> shared, 2D tile, completion on an mbarrier in this CTA.
-// L2 prefetch of one 2-D box (no shared-memory destination, no barrier): warms L2 ahead of the real load.
-__device__ __forceinline__ void tma_prefetch_l2_2d(const CUtensorMap* tm, int c0, int c1) {
-  asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];" ::"l"(reinterpret_cast<uint64_t>(tm)), "r"(c0),
-               "r"(c1)
-               : "memory");
-}
-__device__ __forceinline__ void tma_prefetch_l2_4d(const CUtensorMap* tm, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.prefetch.tensor.4d.L2.global.tile [%0, {%1, %2, %3, %4}];" ::"l"(reinterpret_cast<uint64_t>(tm)),
-               "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-               : "memory");
-}
 __device__ __forceinline__ void tma_load_2d(const CUtensorMap* tm, uint64_t* bar, void* smem_dst, int c0, int c1) {
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
@@ -133,13 +105,6 @@ __device__ __forceinline__ void bulk_load(void* smem_dst, const void* src, uint3
                "l"(src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
-__device__ __forceinline__ void tma_load_3d(const CUtensorMap* tm, uint64_t* bar, void* smem_dst, int c0, int c1,
-                                            int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
 __device__ __forceinline__ void tma_load_4d(const CUtensorMap* tm, uint64_t* bar, void* smem_dst, int c0, int c1,
                                             int c2, int c3) {
   asm volatile(
@@ -147,32 +112,6 @@ __device__ __forceinline__ void tma_load_4d(const CUtensorMap* tm, uint64_t* bar
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2),
       "r"(c3)
       : "memory");
-}
-__device__ __forceinline__ void tma_store_4d(const CUtensorMap* tm, const void* smem_src, int c0, int c1, int c2,
-                                             int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(tm)),
-               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-               : "memory");
-}
-// shared -> global, 2D tile (bulk async group completion).
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* tm, const void* smem_src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(tm)),
-               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_3d(const CUtensorMap* tm, const void* smem_src, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(tm)),
-               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
-               : "memory");
-}
-__device__ __forceinline__ void tma_reduce_add_2d(const CUtensorMap* tm, const void* smem_src, int c0, int c1) {
-  asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(tm)),
-               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
-               : "memory");
 }
 // shared -> global element-wise ADD (fp32 tensor map), 4D tile: the TMA unit performs the reduction in L2.
 __device__ __forceinline__ void tma_reduce_add_4d(const CUtensorMap* tm, const void* smem_src, int c0, int c1, int c2,
@@ -292,8 +231,8 @@ __device__ __forceinline__ float2 unpack_bf16x2(uint32_t u) {
 __device__ __forceinline__ float bf16_round(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
 
 // NOT volatile: a read-only load has no side effects, and `asm volatile` statements are never reordered relative to
-// each other, which serialises "load, compute, store" loops into one memory round trip per iteration (measured: 64-row
-// add_rmsnorm 22 us -> see profiles/).  Only use on data that no thread writes during the kernel.
+// each other, which serialises "load, compute, store" loops into one memory round trip per iteration.  Only use on data that
+// no thread writes during the kernel.
 __device__ __forceinline__ uint4 ld_nc_v4(const void* p) {
   uint4 r;
   asm("ld.global.nc.L1::no_allocate.v4.u32 {%0, %1, %2, %3}, [%4];"
@@ -312,10 +251,6 @@ __device__ __forceinline__ uint4 ld_shared_v4(uint32_t saddr) {
   uint4 r;
   asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "r"(saddr));
   return r;
-}
-__device__ __forceinline__ void st_shared_v4(uint32_t saddr, const uint4& v) {
-  asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w)
-               : "memory");
 }
 
 // 2^x on the SFU (MUFU.EX2), flush-to-zero, no denormal fix-up code around it (exp2f() without fast-math expands to
@@ -378,11 +313,6 @@ __device__ __forceinline__ void swiglu_bwd_pair(uint32_t g2, uint32_t u2, float 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-__device__ __forceinline__ float warp_max(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
 }
 

@@ -351,18 +351,15 @@ static Params base_params(int64_t M, int64_t N, int64_t K) {
 }  // namespace gemm
 }  // namespace b200
 
-// cta_group (1 or 2) is accepted for ABI compatibility; Hopper has no CTA-pair MMA and every call runs the same kernel.
 extern "C" int b200_gemm_bf16_ex(const void* A, const void* B, void* C, const float* bias, const void* residual,
                                  int64_t M, int64_t N, int64_t K, int64_t lda, int64_t ldb, int64_t ldc, int64_t ldr,
-                                 int a_mn_major, int b_mn_major, int accumulate, int cta_group, int max_ctas,
-                                 cudaStream_t stream) {
+                                 int a_mn_major, int b_mn_major, int accumulate, int max_ctas, cudaStream_t stream) {
   using namespace b200;
   using namespace b200::gemm;
   B200_CHECK_ARG(A && B && C, "gemm: null pointer");
   B200_CHECK_ARG(M > 0 && N > 0 && K > 0, "gemm: non-positive dimension M=%lld N=%lld K=%lld", (long long)M,
                  (long long)N, (long long)K);
   B200_CHECK_ARG(lda % 8 == 0 && ldb % 8 == 0 && ldc % 8 == 0, "gemm: leading dimensions must be multiples of 8");
-  B200_CHECK_ARG(cta_group == 1 || cta_group == 2, "gemm: cta_group must be 1 or 2");
   B200_CHECK_ARG(!(residual && accumulate), "gemm: residual and accumulate are mutually exclusive");
   B200_CHECK_ARG(!residual || ldr % 8 == 0, "gemm: ldr must be a multiple of 8");
   B200_CHECK_ARG(M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31), "gemm: dimension too large");
@@ -386,14 +383,13 @@ extern "C" int b200_gemm_bf16_ex(const void* A, const void* B, void* C, const fl
 // The 256-column tile is formed from 128 gate columns and the 128 up columns of the same channels (TMA boxes at different
 // column coordinates of the SAME row-major weight), so the epilogue holds both halves of every channel.
 extern "C" int b200_gemm_swiglu_bf16(const void* X, const void* W, void* GU, void* Mout, int64_t M, int64_t inter, int64_t K,
-                                     int64_t ldx, int64_t ldw, int64_t ldgu, int64_t ldm, int cta_group, cudaStream_t stream) {
+                                     int64_t ldx, int64_t ldw, int64_t ldgu, int64_t ldm, cudaStream_t stream) {
   using namespace b200;
   using namespace b200::gemm;
   B200_CHECK_ARG(X && W && Mout, "gemm_swiglu: null pointer");     // GU may be null: gate|up are then not written (inference)
   B200_CHECK_ARG(M > 0 && inter > 0 && K > 0 && inter % 64 == 0, "gemm_swiglu: intermediate size must be a multiple of 64 (got %lld)",
                  (long long)inter);
   B200_CHECK_ARG(ldx % 8 == 0 && ldw % 8 == 0 && ldgu % 8 == 0 && ldm % 8 == 0, "gemm_swiglu: leading dimensions must be multiples of 8");
-  B200_CHECK_ARG(cta_group == 1 || cta_group == 2, "gemm_swiglu: cta_group must be 1 or 2");
   B200_CHECK_ARG(M < (1ll << 31) && inter < (1ll << 30) && K < (1ll << 31), "gemm_swiglu: dimension too large");
   CUtensorMap tmA, tmB;
   int rc;
@@ -414,15 +410,13 @@ extern "C" int b200_gemm_swiglu_bf16(const void* X, const void* W, void* GU, voi
 //   d(m)[M, I] = dY[M, h] * W_down[I, h]^T   (never written),   DGU[M, 2I] = [ d(m) * up * silu'(gate) | d(m) * silu(gate) ]
 // GU is the saved gate|up projection [M, 2I].  Bit-identical to b200_gemm_bf16 (dX) followed by b200_swiglu_bwd.  I % 64 == 0.
 extern "C" int b200_gemm_swiglu_bwd_bf16(const void* dY, const void* Wdown, const void* GU, void* DGU, int64_t M, int64_t inter,
-                                         int64_t K, int64_t lddy, int64_t ldw, int64_t ldgu, int64_t lddgu, int cta_group,
-                                         cudaStream_t stream) {
+                                         int64_t K, int64_t lddy, int64_t ldw, int64_t ldgu, int64_t lddgu, cudaStream_t stream) {
   using namespace b200;
   using namespace b200::gemm;
   B200_CHECK_ARG(dY && Wdown && GU && DGU, "gemm_swiglu_bwd: null pointer");
   B200_CHECK_ARG(M > 0 && inter > 0 && K > 0 && inter % 64 == 0, "gemm_swiglu_bwd: intermediate size must be a multiple of 64 (got %lld)",
                  (long long)inter);
   B200_CHECK_ARG(lddy % 8 == 0 && ldw % 8 == 0 && ldgu % 8 == 0 && lddgu % 8 == 0, "gemm_swiglu_bwd: leading dimensions must be multiples of 8");
-  B200_CHECK_ARG(cta_group == 1 || cta_group == 2, "gemm_swiglu_bwd: cta_group must be 1 or 2");
   B200_CHECK_ARG(M < (1ll << 31) && inter < (1ll << 30) && K < (1ll << 31), "gemm_swiglu_bwd: dimension too large");
   CUtensorMap tmA, tmB;
   int rc;
@@ -508,16 +502,9 @@ extern "C" int b200_gemm_bf16_splitk(const void* A, const void* B, void* C, cons
   return check_launch("gemm_splitk(finish)");
 }
 
-// Decode-step gate|up projection + SwiGLU (inference form: gate|up are not kept): the fused GEMM of b200_gemm_swiglu_bf16.
-extern "C" int b200_gemm_swiglu_skinny(const void* X, const void* W_gate_up, void* act, int64_t M, int64_t inter, int64_t K,
-                                       int64_t ldx, int64_t ldw, int64_t ldact, cudaStream_t stream) {
-  B200_CHECK_ARG(X && W_gate_up && act, "gemm_swiglu_skinny: null pointer");
-  return b200_gemm_swiglu_bf16(X, W_gate_up, nullptr, act, M, inter, K, ldx, ldw, 2 * inter, ldact, 1, stream);
-}
-
 extern "C" int b200_gemm_bf16(const void* A, const void* B, void* C, const float* bias, int64_t M, int64_t N, int64_t K,
                               int64_t lda, int64_t ldb, int64_t ldc, int a_mn_major, int b_mn_major, int accumulate,
                               cudaStream_t stream) {
   return b200_gemm_bf16_ex(A, B, C, bias, nullptr, M, N, K, lda, ldb, ldc, 0, a_mn_major, b_mn_major, accumulate,
-                           /*cta_group=*/1, /*max_ctas=*/0, stream);
+                           /*max_ctas=*/0, stream);
 }

@@ -50,9 +50,6 @@ inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, siz
 // Returns 0 on success, <0 on failure (message recorded).
 int encode_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides,
                      const uint32_t* box);
-// bf16, no shared-memory swizzle: the box lands as plain rows of box[0] elements (small staging boxes read row-wise by one thread)
-int encode_tmap_bf16_linear(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides,
-                            const uint32_t* box);
 // Same for fp32 elements (box[0] * 4 must be <= 128); used for TMA reduce-add into fp32 accumulation buffers.
 int encode_tmap_f32(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides,
                     const uint32_t* box);

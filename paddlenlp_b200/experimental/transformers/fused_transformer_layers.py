@@ -12,7 +12,6 @@ Layer loop (:1126-1174): the output norm of layer i is fused with the residual a
 from __future__ import annotations
 
 import math
-import os
 from dataclasses import dataclass
 from typing import List, Optional
 
@@ -88,9 +87,6 @@ class FusedMultiTransformerBase:
         self.ffn1_weights = [z(self.h, 2 * self.I) for _ in range(self.L)]
         self.ffn2_weights = [z(self.I, self.h) for _ in range(self.L)]
         self._bias_f32 = [None] * self.L
-        # decode-step ffn1 + SwiGLU: "skinny" / "persistent" = the wgmma GEMM with the SwiGLU epilogue (through the decode-step
-        # and the general entry point), "unfused" = GEMM + SwiGLU kernel
-        self.ffn1_impl = os.environ.get("B200_DECODE_FFN1", "skinny")
         self.rope = ops.rope_tables(self.d, c.max_position_embeddings, float(c.rope_theta), self.device)
 
     def ensure_rope(self, positions: int):
@@ -117,7 +113,7 @@ class FusedMultiTransformerBase:
         n = w.shape[0] if trans_b else w.shape[1]
         if a.shape[0] <= self.SKINNY_M:
             if n >= 100 * 256:        # enough 256-wide column tiles to keep most SMs streaming: no split-K needed
-                return ops.gemm(a, w, trans_b=trans_b, bias=bias, cta_group=1)
+                return ops.gemm(a, w, trans_b=trans_b, bias=bias)
             return ops.gemm_skinny(a, w, trans_b=trans_b, bias=bias)
         return ops.gemm(a, w, trans_b=trans_b, bias=bias)
 
@@ -175,13 +171,10 @@ class FusedMultiTransformerBase:
                 attn = self._attend(qkv, caches, i, seq_lens_decoder, kw)
                 acc = ops.gemm_skinny_f32(attn, self.linear_weights[i], tag="splitk_h")
                 ln_out, residual = ops.add_rmsnorm_f32(acc, residual, self.ffn_ln_scales[i], eps)
-                if self.ffn1_impl == "skinny" and ln_out.shape[0] <= 64 and self.I % 64 == 0:
-                    # the SwiGLU GEMM's decode-step entry point (gate|up are not stored), straight from the reference-layout weight
-                    act = ops.gemm_swiglu_skinny(ln_out, self.ffn1_weights[i])
-                elif self.ffn1_impl != "unfused" and self.I % 128 == 0:
+                if self.I % 64 == 0:
                     # SwiGLU in the ffn1 epilogue of the persistent kernel: the 256-column tile pairs 128 gate columns with the
                     # 128 up columns of the same channels straight from the reference-layout weight; only the activation is stored
-                    _, act = ops.gemm_swiglu(ln_out, self.ffn1_weights[i], cta_group=1, store_gate_up=False)
+                    _, act = ops.gemm_swiglu(ln_out, self.ffn1_weights[i], store_gate_up=False)
                 else:
                     ffn1 = self._mm(ln_out, self.ffn1_weights[i])
                     act = ops.swiglu_fwd(ffn1)

@@ -55,7 +55,7 @@ def _zero_workspace(nbytes: int, device, tag: str) -> torch.Tensor:
 # ----------------------------------------------------------------------------------------------------------
 def gemm(a: torch.Tensor, b: torch.Tensor, out: Optional[torch.Tensor] = None, *, trans_a: bool = False,
          trans_b: bool = False, accumulate: bool = False, bias: Optional[torch.Tensor] = None,
-         residual: Optional[torch.Tensor] = None, cta_group: int = 2, max_ctas: int = 0) -> torch.Tensor:
+         residual: Optional[torch.Tensor] = None, max_ctas: int = 0) -> torch.Tensor:
     """out (+)= op(a) @ op(b) (+ bias)   or   out = bf16(bf16(op(a) @ op(b) + bias) + residual).
     a, b 2-D bf16 with unit inner stride.
     trans_a: a is stored [K, M];  trans_b: b is stored [N, K].  Default b layout [K, N] is Paddle's nn.Linear weight."""
@@ -86,15 +86,14 @@ def gemm(a: torch.Tensor, b: torch.Tensor, out: Optional[torch.Tensor] = None, *
         assert residual.shape == (M, N) and residual.stride(1) == 1 and not accumulate
         ldr = residual.stride(0)
     call("b200_gemm_bf16_ex", ptr(a), ptr(b), ptr(out), ptr(bias), ptr(residual), M, N, K, a.stride(0), b.stride(0),
-         out.stride(0), ldr, 1 if trans_a else 0, 0 if trans_b else 1, 1 if accumulate else 0, cta_group, max_ctas,
-         stream_ptr())
+         out.stride(0), ldr, 1 if trans_a else 0, 0 if trans_b else 1, 1 if accumulate else 0, max_ctas, stream_ptr())
     return out
 
 
 def gemm_swiglu(x: torch.Tensor, w_gate_up: torch.Tensor, gate_up: Optional[torch.Tensor] = None,
-                out: Optional[torch.Tensor] = None, cta_group: int = 2, store_gate_up: bool = True):
+                out: Optional[torch.Tensor] = None, store_gate_up: bool = True):
     """(gate_up [M, 2I], m [M, I]) = fused gate|up projection + SwiGLU (one wgmma GEMM; the epilogue holds gate and up of the
-    same channels).  w_gate_up is the reference-layout fused weight [K, 2I] (gate | up).  Requires I % 128 == 0.
+    same channels).  w_gate_up is the reference-layout fused weight [K, 2I] (gate | up).  Requires I % 64 == 0.
     store_gate_up=False (inference): only m is written and (None, m) is returned."""
     _chk(x, "x"); _chk(w_gate_up, "w_gate_up")
     assert x.dim() == 2 and w_gate_up.dim() == 2 and x.stride(1) == 1 and w_gate_up.stride(1) == 1
@@ -108,12 +107,12 @@ def gemm_swiglu(x: torch.Tensor, w_gate_up: torch.Tensor, gate_up: Optional[torc
     if out is None:
         out = torch.empty(M, inter, dtype=BF16, device=x.device)
     call("b200_gemm_swiglu_bf16", ptr(x), ptr(w_gate_up), ptr(gate_up) if store_gate_up else 0, ptr(out), M, inter, K, x.stride(0),
-         w_gate_up.stride(0), gate_up.stride(0) if store_gate_up else two_i, out.stride(0), cta_group, stream_ptr())
+         w_gate_up.stride(0), gate_up.stride(0) if store_gate_up else two_i, out.stride(0), stream_ptr())
     return (gate_up if store_gate_up else None), out
 
 
-def gemm_swiglu_bwd(dy: torch.Tensor, w_down: torch.Tensor, gate_up: torch.Tensor, dgate_up: Optional[torch.Tensor] = None,
-                    cta_group: int = 2) -> torch.Tensor:
+def gemm_swiglu_bwd(dy: torch.Tensor, w_down: torch.Tensor, gate_up: torch.Tensor,
+                    dgate_up: Optional[torch.Tensor] = None) -> torch.Tensor:
     """dgate_up [M, 2I] = SwiGLU backward of d(m) = dy @ w_down^T, computed in the GEMM epilogue (d(m) is never written).
     w_down is the reference-layout down_proj weight [I, h]; gate_up the saved projection [M, 2I].  Requires I % 64 == 0."""
     _chk(dy, "dy"); _chk(w_down, "w_down"); _chk(gate_up, "gate_up")
@@ -123,7 +122,7 @@ def gemm_swiglu_bwd(dy: torch.Tensor, w_down: torch.Tensor, gate_up: torch.Tenso
     if dgate_up is None:
         dgate_up = torch.empty_like(gate_up)
     call("b200_gemm_swiglu_bwd_bf16", ptr(dy), ptr(w_down), ptr(gate_up), ptr(dgate_up), M, inter, K, dy.stride(0), w_down.stride(0),
-         gate_up.stride(0), dgate_up.stride(0), cta_group, stream_ptr())
+         gate_up.stride(0), dgate_up.stride(0), stream_ptr())
     return dgate_up
 
 
@@ -294,21 +293,6 @@ def swiglu_fwd_f32(acc_f32: torch.Tensor, out: Optional[torch.Tensor] = None):
     if out is None:
         out = torch.empty(rows, inter, dtype=BF16, device=acc_f32.device)
     call("b200_swiglu_fwd_f32", ptr(acc_f32), ptr(out), rows, inter, stream_ptr())
-    return out
-
-
-def gemm_swiglu_skinny(x: torch.Tensor, w_gate_up: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """Decode-step ffn1 + SwiGLU (M <= 64 token rows) in one weight-streaming kernel (two CTAs per SM, swapped operands);
-    w_gate_up is the reference-layout fused weight [K, 2I] (gate | up), I % 64 == 0."""
-    _chk(x, "x"); _chk(w_gate_up, "w_gate_up")
-    M, K = x.shape
-    inter = w_gate_up.shape[1] // 2
-    assert w_gate_up.shape[0] == K and x.stride(1) == 1 and w_gate_up.stride(1) == 1
-    if out is None:
-        out = torch.empty(M, inter, dtype=BF16, device=x.device)
-    assert out.shape == (M, inter) and out.stride(1) == 1
-    call("b200_gemm_swiglu_skinny", ptr(x), ptr(w_gate_up), ptr(out), M, inter, K, x.stride(0), w_gate_up.stride(0),
-         out.stride(0), stream_ptr())
     return out
 
 
@@ -513,6 +497,13 @@ def decode_rope_append(qkv, cache, cos, sin, seq_lens, nh, kvh, d):
          qkv.stride(0), stream_ptr())
 
 
+def _decode_splits(B: int, kvh: int, max_len: int) -> int:
+    """Split-KV count of the bulk-copy decode-attention kernels (dense, paged and append_attention's decode rows): split only
+    when there are too few (b, kv head) pairs to give every SM ~3 CTAs (a split costs partial traffic, a merge launch and a
+    CTA boundary), with at most one split per 128 cache rows."""
+    return max(1, min((max_len + 127) // 128, (3 * 132 + B * kvh - 1) // (B * kvh), DECODE_MAX_SPLITS))
+
+
 def decode_attention(qkv, cache, seq_lens, nh, kvh, d, softmax_scale=None, out=None, num_splits: int = 0, impl: str = "tc"):
     """Attention of one query row per sequence over the dense cache [2, B, kvh, max_len, d]: sequence b attends to its first
     min(seq_lens[b] + 1, max_len) rows (the new token was appended at row seq_lens[b]).  GQA group nh / kvh in 1..8,
@@ -527,9 +518,7 @@ def decode_attention(qkv, cache, seq_lens, nh, kvh, d, softmax_scale=None, out=N
     max_len = cache.shape[3]
     if impl == "tc":
         if num_splits <= 0:
-            # split only when there are too few (b, kv head) pairs to give every SM ~3 CTAs (a split costs partial traffic,
-            # a merge launch and a CTA boundary)
-            num_splits = max(1, min((max_len + 127) // 128, (3 * 132 + B * kvh - 1) // (B * kvh), DECODE_MAX_SPLITS))
+            num_splits = _decode_splits(B, kvh, max_len)
         fn = "b200_decode_attention_tc"
     elif impl == "simt":
         if num_splits <= 0:
@@ -585,9 +574,8 @@ def decode_attention_paged(qkv, key_cache, value_cache, block_tables, seq_lens, 
         out = torch.empty(B, nh * d, dtype=BF16, device=qkv.device)
     if softmax_scale is None:
         softmax_scale = 1.0 / math.sqrt(d)
-    max_len = mb * bs
     if num_splits <= 0:
-        num_splits = max(1, min((max_len + 127) // 128, (3 * 132 + B * kvh - 1) // (B * kvh), DECODE_MAX_SPLITS))
+        num_splits = _decode_splits(B, kvh, mb * bs)
     ws = None
     if num_splits > 1:
         ws = _workspace(_lib.load().b200_decode_attention_workspace_bytes(B, nh, num_splits), qkv.device, "decode_attn")
@@ -632,7 +620,7 @@ def append_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_dec
     if softmax_scale is None:
         softmax_scale = 1.0 / math.sqrt(d)
     if num_splits <= 0:
-        num_splits = max(1, min((mb * bs + 127) // 128, (3 * 132 + B * kvh - 1) // (B * kvh), DECODE_MAX_SPLITS))
+        num_splits = _decode_splits(B, kvh, mb * bs)
     ws = _workspace(_lib.load().b200_append_attention_workspace_bytes(B, nh, kvh, d, num_splits), qkv.device, "append_attn")
     call("b200_append_attention", ptr(qkv), ptr(key_cache), ptr(value_cache), ptr(seq_lens_encoder), ptr(seq_lens_decoder),
          ptr(seq_lens_this_time), ptr(cu_seqlens_q), ptr(block_tables), ptr(cos), ptr(sin), ptr(out), ptr(ws), B, token_num,

@@ -61,12 +61,10 @@ class DecoderEngine:
         if self.h % 8 or self.I % 8 or self.V % 8:
             raise ValueError("hidden_size, intermediate_size and vocab_size must be multiples of 8")
         self.qkv_n = (self.nh + 2 * self.kvh) * self.d
-        # SwiGLU fused into the gate|up GEMM epilogue (needs 128-channel tiles); B200_FUSE_SWIGLU=0 selects GEMM + swiglu kernel
-        import os as _os
-        self.fuse_swiglu = (self.I % 128 == 0) and _os.environ.get("B200_FUSE_SWIGLU", "1") != "0"
-        # the backward twin: SwiGLU backward in the down-proj dX epilogue (bit-identical to GEMM + swiglu_bwd kernel; the epilogue reads
-        # the saved gate|up values of its accumulator's rows and columns).  B200_FUSE_SWIGLU_BWD=0 unfuses
-        self.fuse_swiglu_bwd = (self.I % 64 == 0) and _os.environ.get("B200_FUSE_SWIGLU_BWD", "1") != "0"
+        # SwiGLU fused into the gate|up GEMM epilogue and, in the backward, into the down-proj dX epilogue (which reads the saved
+        # gate|up values of its accumulator's rows and columns).  Both kernels need I % 64 == 0 and give the same bits as GEMM +
+        # swiglu kernel, the path taken otherwise.
+        self.fuse_swiglu = self.I % 64 == 0
         # recompute (llama/modeling.py:1706-1733 `recompute_training_full`): keep only each layer's input and re-run the
         # layer forward inside backward.  Only the "full" granularity exists here (the "full_attn" / "core_attn" splits
         # exist to trade memory against the reference's unfused attention; the fused attention keeps no S x S tensor).
@@ -446,7 +444,7 @@ class DecoderEngine:
         T = B * S
         qn, kn = self.nh * self.d, self.kvh * self.d
         # ---- MLP ----
-        if self.fuse_swiglu_bwd:
+        if self.fuse_swiglu:
             dgu = ops.gemm_swiglu_bwd(dx2, p[f"l{i}.down_w"], gu)      # SwiGLU backward in the dX GEMM's epilogue
             ops.gemm(m, dx2, out=g[f"l{i}.down_w"], trans_a=True, accumulate=acc)
             del m

@@ -21,7 +21,7 @@ def test_library_loads_and_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(lib, name), f"{name} declared in include/b200nlp.h but not exported"
     assert sorted(_lib.exported_symbols()) == declared, "ctypes signature table out of sync with the header"
-    assert lib.b200_abi_version() == 1
+    assert lib.b200_abi_version() == 2
 
 
 def test_no_cuda_device_is_a_loud_error():

@@ -436,22 +436,6 @@ def test_generate_edge_cases(block_attn):
         m.generate(ids, max_length=29, cache_kvs=caches)
 
 
-def test_generate_with_fused_ffn1_swiglu_option():
-    """FusedMultiTransformerBase.ffn1_impl: "skinny" (default: swapped-operand ffn1 + SwiGLU kernel) and "persistent" (128x256-tile
-    kernel with the SwiGLU epilogue) generate the same tokens."""
-    cfg = R.RefConfig(vocab_size=512, hidden_size=256, intermediate_size=704, num_hidden_layers=2, num_attention_heads=2,
-                      num_key_value_heads=1, rope_theta=10000.0, max_position_embeddings=128, rms_norm_eps=1e-5)
-    w = R.init_weights(cfg, seed=9)
-    w = {k: (v * 4).to(BF16).float() if k.endswith("weight") and "norm" not in k else v for k, v in w.items()}
-    m, _ = _infer_model(cfg, w)
-    ids = torch.randint(1, cfg.vocab_size, (4, 16), generator=torch.Generator().manual_seed(8))
-    a, _, _ = m.generate(ids, max_length=12)
-    assert m.transformer_block.ffn1_impl == "skinny"
-    m.transformer_block.ffn1_impl = "persistent"
-    b, _, _ = m.generate(ids, max_length=12)
-    assert (a == b).float().mean().item() > 0.9 and torch.equal(a[:, :3], b[:, :3])
-
-
 def test_full_width_decode_matches_uncached_forward():
     """KV-cache consistency (tests/transformers/llama/test_modeling.py:171-219) at the FULL Llama-3-8B layer width, batch 64:
     prefill logits match the training-path forward, and three decode steps (swapped-operand GEMMs at N = 6144 / 4096 /

@@ -39,16 +39,16 @@ def rand_bf16(*shape, seed=0, scale=1.0):
 
 
 # ------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("cg", [1, 2])
+@pytest.mark.parametrize("M", [520, 40])    # two-warpgroup (128-row) and one-warpgroup (64-row) tiles
 @pytest.mark.parametrize("ta,tb", [(False, False), (False, True), (True, False), (True, True)])
-def test_gemm_layouts(cg, ta, tb):
+def test_gemm_layouts(M, ta, tb):
     o = ops()
-    M, N, K = 520, 776, 328   # ragged against every tile dimension
+    N, K = 776, 328           # ragged against every tile dimension
     A = rand_bf16(M, K, seed=1, scale=0.5)
     B = rand_bf16(K, N, seed=2, scale=0.5)
     a_d = (A.t().contiguous() if ta else A).to(DEV)
     b_d = (B.t().contiguous() if tb else B).to(DEV)
-    out = o.gemm(a_d, b_d, trans_a=ta, trans_b=tb, cta_group=cg)
+    out = o.gemm(a_d, b_d, trans_a=ta, trans_b=tb)
     ref = A.float().to(DEV) @ B.float().to(DEV)
     # one bf16 rounding of an fp32-accumulated result: <= 2^-8 relative to the largest magnitude
     assert maxerr(out, ref) < 2 ** -7
@@ -82,38 +82,40 @@ def test_gemm_residual_epilogue():
     assert mism < 0.02 and maxerr(out, ref) < 2 ** -7           # only fp32 accumulation-order ties may differ
 
 
-@pytest.mark.parametrize("cg", [2, 1])
-@pytest.mark.parametrize("M,inter,K", [(520, 384, 328), (8192, 14336, 4096), (300, 128, 64), (64, 14336, 4096)])
-def test_gemm_swiglu_fused_epilogue(M, inter, K, cg):
+# (5 | 33 | 64, ...): decode-step ffn1 shapes (one-warpgroup tiles); I = 192: a last tile of 64 channels, half used
+@pytest.mark.parametrize("M,inter,K", [(520, 384, 328), (8192, 14336, 4096), (300, 128, 64), (64, 14336, 4096), (5, 192, 328),
+                                       (33, 18944, 3584), (100, 192, 328), (520, 192, 328)])
+def test_gemm_swiglu_fused_epilogue(M, inter, K):
     """gate|up projection + SwiGLU in one wgmma GEMM (tile = 128 gate columns | the 128 up columns of the same channels) is
-    bit-identical to GEMM followed by the SwiGLU kernel: same accumulation order per element, same rounding points."""
+    bit-identical to GEMM followed by the SwiGLU kernel: same accumulation order per element, same rounding points.  The
+    inference form (gate|up not stored) is the decode step's ffn1."""
     o = ops()
     x = rand_bf16(M, K, seed=51, scale=0.7).to(DEV)
     w = rand_bf16(K, 2 * inter, seed=52, scale=0.3).to(DEV)
-    gu_ref = o.gemm(x, w, cta_group=cg)
+    gu_ref = o.gemm(x, w)
     m_ref = o.swiglu_fwd(gu_ref)
-    gu, m = o.gemm_swiglu(x, w, cta_group=cg)
+    gu, m = o.gemm_swiglu(x, w)
     assert torch.equal(gu, gu_ref)
     assert torch.equal(m, m_ref)
     ref = R.swiglu((x.float() @ w.float())[:, :inter].to(BF16).float(), (x.float() @ w.float())[:, inter:].to(BF16).float(), "bf16")
     assert maxerr(m, ref) < 2 ** -6
-    _, m_only = o.gemm_swiglu(x, w, cta_group=cg, store_gate_up=False)       # inference form: gate|up are not written
+    _, m_only = o.gemm_swiglu(x, w, store_gate_up=False)       # inference form: gate|up are not written
     assert torch.equal(m_only, m_ref)
     with pytest.raises(Exception):
-        o.gemm_swiglu(x, w[:, : 2 * 72].contiguous())              # I = 72 is not a multiple of 128
+        o.gemm_swiglu(x, w[:, : 2 * 72].contiguous())              # I = 72 is not a multiple of 64
 
 
-@pytest.mark.parametrize("cg", [2, 1])
-@pytest.mark.parametrize("M,inter,K", [(520, 320, 328), (8192, 14336, 4096), (300, 64, 64)])
-def test_gemm_swiglu_bwd_fused_epilogue(M, inter, K, cg):
+@pytest.mark.parametrize("M,inter,K", [(520, 320, 328), (8192, 14336, 4096), (300, 64, 64), (5, 192, 328), (100, 192, 328),
+                                       (520, 192, 328)])
+def test_gemm_swiglu_bwd_fused_epilogue(M, inter, K):
     """The down-projection dX GEMM with the SwiGLU backward in its epilogue is bit-identical to GEMM (dX) + swiglu_bwd kernel."""
     o = ops()
     dy = rand_bf16(M, K, seed=53, scale=0.5).to(DEV)
     wd = rand_bf16(inter, K, seed=54, scale=0.3).to(DEV)
     gu = rand_bf16(M, 2 * inter, seed=55, scale=1.5).to(DEV)
-    dm = o.gemm(dy, wd, trans_b=True, cta_group=cg)
+    dm = o.gemm(dy, wd, trans_b=True)
     ref = o.swiglu_bwd(gu, dm)
-    got = o.gemm_swiglu_bwd(dy, wd, gu, cta_group=cg)
+    got = o.gemm_swiglu_bwd(dy, wd, gu)
     assert torch.equal(got, ref)
 
 
@@ -128,21 +130,6 @@ def test_gemm_skinny_splitk(M, N, K, split, tb):
     out = o.gemm_skinny(A.to(DEV), b_d, trans_b=tb, bias=bias.to(DEV), split_k=split)
     ref = A.float().to(DEV) @ B.float().to(DEV) + bias.to(DEV)
     assert maxerr(out, ref) < 2 ** -7 and relerr(out, ref) < 4e-3
-
-
-@pytest.mark.parametrize("M,inter,K", [(64, 14336, 4096), (5, 192, 328), (33, 18944, 3584)])
-def test_gemm_swiglu_skinny(M, inter, K):
-    """Decode ffn1 + SwiGLU in one swapped-operand kernel == GEMM (bf16 output) followed by the SwiGLU kernel, straight from the
-    reference-layout [K, 2I] weight."""
-    o = ops()
-    x = rand_bf16(M, K, seed=51).to(DEV)
-    w = rand_bf16(K, 2 * inter, seed=52, scale=0.05).to(DEV)
-    got = o.gemm_swiglu_skinny(x, w)
-    want = o.swiglu_fwd(o.gemm(x, w, cta_group=1))
-    ref = R.swiglu(R.linear(x.float().cpu(), w[:, :inter].float().cpu(), None, "bf16"),
-                   R.linear(x.float().cpu(), w[:, inter:].float().cpu(), None, "bf16"), "bf16")
-    assert maxerr(got.cpu(), ref) < 2 ** -6
-    assert (got != want).float().mean().item() < 0.02          # same rounding points; fp32 summation order may flip a few ulps
 
 
 def test_gemm_argument_errors():

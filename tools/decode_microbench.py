@@ -43,8 +43,8 @@ def main():
         for split in (0, 1):
             us = timeit(lambda: ops.gemm_skinny(a, wt, trans_b=tb, split_k=split))
             print(json.dumps(dict(op=f"gemm_skinny[{name} 64x{N}x{K}] split={split}", us=us, gbs=K * N * 2 / us / 1e3)))
-        us = timeit(lambda: ops.gemm(a, wt, trans_b=tb, cta_group=1))
-        print(json.dumps(dict(op=f"gemm cg1 [{name}]", us=us, gbs=K * N * 2 / us / 1e3)))
+        us = timeit(lambda: ops.gemm(a, wt, trans_b=tb))
+        print(json.dumps(dict(op=f"gemm [{name}]", us=us, gbs=K * N * 2 / us / 1e3)))
     max_len = 2048
     cache = torch.randn(2, B, kvh, max_len, d, device=dev).to(torch.bfloat16)
     qkv = torch.randn(B, (nh + 2 * kvh) * d, device=dev).to(torch.bfloat16)

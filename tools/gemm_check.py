@@ -1,7 +1,7 @@
 """Bring-up / regression check of the wgmma GEMM on an H100.
 
-    python tools/gemm_check.py            # driver: one subprocess per (cta_group, a_major, b_major) case
-    python tools/gemm_check.py --case 2,0,1
+    python tools/gemm_check.py            # driver: one subprocess per (a_major, b_major) case
+    python tools/gemm_check.py --case 0,1
 
 Each case checks correctness against torch.matmul (fp32 accumulate reference on the same bf16 inputs) on
 single-tile, ragged and multi-tile shapes, then times a large shape.  Output is appended to <--log-dir>/gemm_check.log.
@@ -17,7 +17,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 
-def run_case(cg, a_mn, b_mn, big):
+def run_case(a_mn, b_mn, big):
     import torch
 
     from paddlenlp_b200 import _lib
@@ -28,7 +28,7 @@ def run_case(cg, a_mn, b_mn, big):
 
     def gemm(A, B, C, M, N, K, acc=0, bias=None):
         _lib.call("b200_gemm_bf16_ex", _lib.ptr(A), _lib.ptr(B), _lib.ptr(C), _lib.ptr(bias), None, M, N, K,
-                  A.stride(0), B.stride(0), C.stride(0), 0, a_mn, b_mn, acc, cg, 0, _lib.stream_ptr())
+                  A.stride(0), B.stride(0), C.stride(0), 0, a_mn, b_mn, acc, 0, _lib.stream_ptr())
 
     def check(M, N, K, acc=0, use_bias=False, seed=0):
         g = torch.Generator(device="cpu").manual_seed(seed)
@@ -54,7 +54,7 @@ def run_case(cg, a_mn, b_mn, big):
         # bf16 rounding of the result: half-ulp relative 2^-9
         tol = scale * 2.0 ** -8 + 1e-3
         ok = bool(maxerr <= tol) and bool(torch.isfinite(got).all())
-        info = dict(case=[cg, a_mn, b_mn], M=M, N=N, K=K, acc=acc, bias=use_bias, maxerr=maxerr, scale=scale, ok=ok)
+        info = dict(case=[a_mn, b_mn], M=M, N=N, K=K, acc=acc, bias=use_bias, maxerr=maxerr, scale=scale, ok=ok)
         if not ok:
             bad = err > tol
             rows = bad.any(dim=1).nonzero().flatten()
@@ -69,7 +69,7 @@ def run_case(cg, a_mn, b_mn, big):
         return ok
 
     shapes = [
-        (128 * cg, 256, 64), (128 * cg, 256, 128), (128 * cg, 256, 512),
+        (128, 256, 64), (128, 256, 128), (128, 256, 512),
         (256, 512, 256), (512, 768, 320), (384, 256, 64),
         (1024, 1024, 1024), (136, 264, 72), (2048, 6144, 4096),
     ]
@@ -111,7 +111,7 @@ def run_case(cg, a_mn, b_mn, big):
             torch.cuda.synchronize()
             ms2 = e0.elapsed_time(e1) / iters
             tf2 = 2.0 * M * N * K / ms2 / 1e9
-            info = dict(case=[cg, a_mn, b_mn], perf=[M, N, K], ms=ms, tflops=tf, cublas_ms=ms2, cublas_tflops=tf2)
+            info = dict(case=[a_mn, b_mn], perf=[M, N, K], ms=ms, tflops=tf, cublas_ms=ms2, cublas_tflops=tf2)
             print(json.dumps(info), flush=True)
     return allok
 
@@ -120,34 +120,34 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--case", default=None)
     ap.add_argument("--no-big", action="store_true")
-    ap.add_argument("--cases", default=None, help="semicolon separated list of cg,a,b")
+    ap.add_argument("--cases", default=None, help="semicolon separated list of a,b")
     ap.add_argument("--log-dir", default=".", help="directory of gemm_check.log")
     a = ap.parse_args()
     if a.case:
-        cg, am, bm = [int(x) for x in a.case.split(",")]
-        ok = run_case(cg, am, bm, not a.no_big)
+        am, bm = [int(x) for x in a.case.split(",")]
+        ok = run_case(am, bm, not a.no_big)
         sys.exit(0 if ok else 1)
     os.makedirs(a.log_dir, exist_ok=True)
     log = open(os.path.join(a.log_dir, "gemm_check.log"), "a")
     if a.cases:
         cases = [tuple(int(x) for x in c.split(",")) for c in a.cases.split(";")]
     else:
-        cases = [(cg, am, bm) for cg in (1, 2) for am in (0, 1) for bm in (0, 1)]
+        cases = [(am, bm) for am in (0, 1) for bm in (0, 1)]
     summary = {}
-    for (cg, am, bm) in cases:
-        cmd = [sys.executable, os.path.abspath(__file__), "--case", f"{cg},{am},{bm}"] + (["--no-big"] if a.no_big else [])
+    for (am, bm) in cases:
+        cmd = [sys.executable, os.path.abspath(__file__), "--case", f"{am},{bm}"] + (["--no-big"] if a.no_big else [])
         t0 = time.time()
         try:
             r = subprocess.run(cmd, capture_output=True, text=True, timeout=240)
             out, rc = r.stdout + r.stderr[-3000:], r.returncode
         except subprocess.TimeoutExpired as e:
             out, rc = (e.stdout or b"").decode(errors="replace") + "\nTIMEOUT", -9
-        hdr = f"=== case cg={cg} a_mn={am} b_mn={bm} rc={rc} ({time.time() - t0:.1f}s)"
+        hdr = f"=== case a_mn={am} b_mn={bm} rc={rc} ({time.time() - t0:.1f}s)"
         print(hdr)
         print(out[-6000:])
         log.write(hdr + "\n" + out + "\n")
         log.flush()
-        summary[f"{cg},{am},{bm}"] = rc
+        summary[f"{am},{bm}"] = rc
     print("SUMMARY", json.dumps(summary))
     log.write("SUMMARY " + json.dumps(summary) + "\n")
 

@@ -69,11 +69,11 @@ def gemms(rounds):
     head, E = rnd(H, V, s=0.02), rnd(V, H, s=0.02)
     g_head, g_E = torch.zeros(H, V, dtype=BF16, device=dev), torch.zeros(V, H, dtype=BF16, device=dev)
     hn = rnd(DECODE_M, H)
-    # FusedMultiTransformerBase._mm at M <= SKINNY_M and N = V (>= 100 column tiles): the persistent GEMM, cta_group 1
+    # FusedMultiTransformerBase._mm at M <= SKINNY_M and N = V (>= 100 column tiles): the persistent GEMM
     assert DECODE_M <= FusedMultiTransformerBase.SKINNY_M and V >= 100 * 256
 
     def mm(a, w, trans_b=False):
-        return ops.gemm(a, w, trans_b=trans_b, cta_group=1)
+        return ops.gemm(a, w, trans_b=trans_b)
 
     cases = {
         "logits": (lambda: ops.gemm(hf, head), lambda: ops.gemm(hf, E, trans_b=True)),
