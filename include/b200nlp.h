@@ -138,9 +138,9 @@ int b200_embedding_fwd(const int64_t* ids, const void* table, void* out, int64_t
 int b200_embedding_bwd(const int64_t* ids, const void* dout, void* dtable, int64_t tokens, int64_t h, int64_t vocab,
                        cudaStream_t stream);
 
-/* ---- Flash attention, causal, GQA, head_dim 128: replaces F.scaled_dot_product_attention(is_causal=True)
+/* ---- Flash attention, causal, GQA, head_dim 64 or 128 (anything else: argument error): replaces F.scaled_dot_product_attention(is_causal=True)
  * (fusion_ops.py:147-267; Paddle-vendored FlashAttention-2) and its gradient (csrc/gpu/flash_attn_bwd.cc:22-92).
- * q [B,S,nh,128], k/v [B,S,kvh,128], o [B,S,nh,128]; ld* = token stride in elements (the tensors may be views into a
+ * q [B,S,nh,d], k/v [B,S,kvh,d], o [B,S,nh,d]; ld* = token stride in elements (the tensors may be views into a
  * packed QKV projection).  lse [B,nh,S] fp32 (natural log).  Backward workspace: b200_fa_bwd_workspace_bytes(). */
 int b200_fa_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int64_t B, int64_t S,
                 int64_t num_heads, int64_t num_kv_heads, int64_t head_dim, int64_t ldq, int64_t ldk, int64_t ldv,
@@ -218,7 +218,7 @@ int b200_decode_rope_append(void* qkv, void* cache, const float* cos_table, cons
 int b200_decode_rope_append_f32(void* qkv, float* acc_f32_ws, const float* bias, void* cache, const float* cos_table,
                                 const float* sin_table, const int32_t* seq_lens, int64_t B, int64_t num_heads,
                                 int64_t num_kv_heads, int64_t head_dim, int64_t max_len, int64_t ld, cudaStream_t stream);
-/* Decode attention of one query token per sequence over cache positions [0, seq_lens[b]] (GQA, head_dim 128);
+/* Decode attention of one query token per sequence over cache positions [0, seq_lens[b]] (GQA, head_dim 64 or 128);
  * out [B, nh*d].  num_splits > 1 splits each sequence's cache range over that many CTAs (split-KV, merged by a second
  * kernel through `workspace`), as the reference's append_attention does (append_attention_c16_impl.cuh:826-1000).
  * Replaces the attention half of masked_multihead_attention / append_attention decode
@@ -227,9 +227,9 @@ int64_t b200_decode_attention_workspace_bytes(int64_t B, int64_t num_heads, int6
 int b200_decode_attention(const void* qkv, const void* cache, const int32_t* seq_lens, void* out, void* workspace, int64_t B,
                           int64_t num_heads, int64_t num_kv_heads, int64_t head_dim, int64_t max_len, int64_t ld,
                           float softmax_scale, int64_t num_splits, cudaStream_t stream);
-/* Same contract, Hopper streaming kernel: a producer warp moves 32-row K/V chunks with cp.async.bulk into a 4-stage shared-memory
- * ring on mbarriers, four consumer warps compute (a half-warp per cache row, the G heads of a group sharing each row); GQA group
- * size 1, 2, 4, 7 or 8.
+/* Same contract, Hopper streaming kernel: a producer warp moves 8 KB K/V chunks (32 rows at d = 128, 64 at d = 64) with
+ * cp.async.bulk into a 4-stage shared-memory ring on mbarriers, four consumer warps compute (d / 8 lanes per cache row, the G
+ * heads of a group sharing each row); GQA group size 1 to 8.  Split-KV partial rows are 132 floats at either head_dim.
  * Cache rows past the sequence length must hold finite values (zero-filled allocation, as the reference's paddle.zeros). */
 int b200_decode_attention_tc(const void* qkv, const void* cache, const int32_t* seq_lens, void* out, void* workspace, int64_t B,
                              int64_t num_heads, int64_t num_kv_heads, int64_t head_dim, int64_t max_len, int64_t ld,

@@ -1,4 +1,4 @@
-// Causal GQA flash-attention backward on Hopper tensor cores (head_dim 128).
+// Causal GQA flash-attention backward on Hopper tensor cores (head_dim 64 or 128).
 //
 //   inputs : q, k, v, o, do, lse            outputs: dq, dk, dv (bf16; fp32 accumulation buffers in the workspace)
 //   P = exp(S*scale - lse) ; dP = dO V^T ; dS = P o (dP - D) * scale, D = rowsum(dO o O)
@@ -21,6 +21,12 @@
 //                   dQ = dS K                             (dS^T through shared memory; each warpgroup 64 of the d columns)
 //                   dQ tile -> fp32 staging -> cp.reduce.async.bulk.tensor add into the dQ buffer
 //                   dK / dV -> TMA reduce-adds into the kv head's fp32 buffers once per CTA
+//   head_dim 64: one [128 kv][64 d] swizzled block for K and V, one [64 q][64 d] block for Q and dO; S^T and dP^T take 4
+//   k-steps, dV / dK are m64n64k16.  dQ = dS K is split over the kv rows instead of the d columns: each warpgroup multiplies
+//   its own 64 rows of dS^T by its own 64 rows of K into a full [64 q][64 d] partial and reduce-adds it, so every wgmma keeps
+//   the m64n64k16 shape with swizzle-atom-aligned operands and the warpgroups need no shared barrier for dS^T; the price is
+//   twice the dQ reduce-add bytes (2 x 16 KB per q tile, as at head_dim 128).  (A d split would need m64n32 tiles that start
+//   inside a swizzle row; a q-row split is below wgmma's 64-row M.)
 // impl 1, fa_bwd_kernel: the mma.sync cross-check.  One CTA (8 warps) = (batch, q-head, 64-row kv tile), 64-row q tiles
 // through cp.async; per q tile S and dP per warp in registers -> P, dS as bf16 in shared memory -> dV, dK (ldmatrix.trans
 // operands) and dQ, which it adds to the fp32 dQ buffer with atomics, as it does dK / dV at the end.
@@ -33,7 +39,6 @@
 namespace b200 {
 namespace fab {
 
-constexpr int D = 128;
 constexpr int BKV = 64;
 constexpr int NUM_THREADS = 256;
 
@@ -45,27 +50,29 @@ struct Params {
   const float* lse2;    // [B, nh, Spad]  lse * log2(e); +inf on the padding rows s >= S (P = 0 there)
   const float* delta;   // [B, nh, Spad]  rowsum(dO o O); 0 on the padding rows
   const int* mask_start;   // FlashMask causal-LT start rows [B, S] (see fa_fwd.cu) or nullptr
-  float* dq_acc;        // [B, S, nh, 128]
-  float* dk_acc;        // [B, S, kvh, 128]
+  float* dq_acc;        // [B, S, nh, D]
+  float* dk_acc;        // [B, S, kvh, D]
   float* dv_acc;
 };
 
-// [rows][128] bf16 tiles: 16-byte chunks XOR-swizzled by row & 7 (as fa_fwd.cu); [rows][64] tiles (P, dS): 128-byte rows
-__device__ __forceinline__ uint32_t swz(int row, int chunk) { return static_cast<uint32_t>(row * 256 + ((chunk ^ (row & 7)) << 4)); }
+// [rows][D] bf16 tiles: 16-byte chunks XOR-swizzled by row & 7 (as fa_fwd.cu); [rows][64] tiles (P, dS): 128-byte rows
+template <int D>
+__device__ __forceinline__ uint32_t swz(int row, int chunk) { return static_cast<uint32_t>(row * (D * 2) + ((chunk ^ (row & 7)) << 4)); }
 __device__ __forceinline__ uint32_t swz64(int row, int chunk) { return static_cast<uint32_t>(row * 128 + ((chunk ^ (row & 7)) << 4)); }
 
-template <int BQ, bool MASK>
+template <int D, int BQ, bool MASK>
 __global__ void __launch_bounds__(NUM_THREADS, 1) fa_bwd_kernel(const Params p) {
+  constexpr int DCH = D / 8, DCH_LOG2 = D == 128 ? 4 : 3;   // 16-byte chunks per row of a [rows][D] tile
   constexpr int RG = BQ / 16;            // phase 1: row groups of 16 q rows
   constexpr int CH = 8 / RG;             //          column slices of the 64 kv columns
   constexpr int NT = 8 / CH;             //          8-column n-tiles per warp
   constexpr int QG = BQ / 16;            // dQ: row groups
   constexpr int DH = 8 / QG;             //     d slices
-  constexpr int DTQ = 16 / DH;           //     8-column d tiles per warp
+  constexpr int DTQ = DCH / DH;           //     8-column d tiles per warp
   extern __shared__ __align__(128) uint8_t smem[];
-  const uint32_t sK = smem_u32(smem), sV = sK + BKV * 256, sQ = sV + BKV * 256, sdO = sQ + BQ * 256;
-  const uint32_t sP = sdO + BQ * 256, sdS = sP + BQ * 128;
-  float* s_lse = reinterpret_cast<float*>(smem + 2 * BKV * 256 + 2 * BQ * 256 + 2 * BQ * 128);
+  const uint32_t sK = smem_u32(smem), sV = sK + BKV * D * 2, sQ = sV + BKV * D * 2, sdO = sQ + BQ * D * 2;
+  const uint32_t sP = sdO + BQ * D * 2, sdS = sP + BQ * 128;
+  float* s_lse = reinterpret_cast<float*>(smem + 2 * BKV * D * 2 + 2 * BQ * D * 2 + 2 * BQ * 128);
   float* s_delta = s_lse + BQ;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, tq = lane & 3;
@@ -80,25 +87,25 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fa_bwd_kernel(const Params p) 
     const int last = __ldg(p.mask_start + tok0 + min(kv0 + BKV - 1, p.S - 1));
     q_hi = min(q_hi, (last + BQ - 1) / BQ);
   }
-  for (int i = threadIdx.x; i < BKV * 16; i += NUM_THREADS) {
-    const int r = i >> 4, ch = i & 15;
+  for (int i = threadIdx.x; i < BKV * DCH; i += NUM_THREADS) {
+    const int r = i >> DCH_LOG2, ch = i & (DCH - 1);
     const bool ok = kv0 + r < p.S;
-    cp_async_16(sK + swz(r, ch), ok ? p.k + (tok0 + kv0 + r) * p.ldk + kv_head * D + ch * 8 : p.k, ok ? 16u : 0u);
-    cp_async_16(sV + swz(r, ch), ok ? p.v + (tok0 + kv0 + r) * p.ldv + kv_head * D + ch * 8 : p.v, ok ? 16u : 0u);
+    cp_async_16(sK + swz<D>(r, ch), ok ? p.k + (tok0 + kv0 + r) * p.ldk + kv_head * D + ch * 8 : p.k, ok ? 16u : 0u);
+    cp_async_16(sV + swz<D>(r, ch), ok ? p.v + (tok0 + kv0 + r) * p.ldv + kv_head * D + ch * 8 : p.v, ok ? 16u : 0u);
   }
-  // dK / dV accumulators: warp = 16 kv rows (kg) x 64 d columns (dh)
+  // dK / dV accumulators: warp = 16 kv rows (kg) x D/2 d columns (dh)
   const int kg = warp >> 1, dh = warp & 1;
-  float dk[8][4], dv[8][4];
+  float dk[D / 16][4], dv[D / 16][4];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) dk[i][0] = dk[i][1] = dk[i][2] = dk[i][3] = dv[i][0] = dv[i][1] = dv[i][2] = dv[i][3] = 0.f;
+  for (int i = 0; i < D / 16; ++i) dk[i][0] = dk[i][1] = dk[i][2] = dk[i][3] = dv[i][0] = dv[i][1] = dv[i][2] = dv[i][3] = 0.f;
 
   for (int qt = q_lo; qt < q_hi; ++qt) {
     const int q0 = qt * BQ;
-    for (int i = threadIdx.x; i < BQ * 16; i += NUM_THREADS) {
-      const int r = i >> 4, ch = i & 15;
+    for (int i = threadIdx.x; i < BQ * DCH; i += NUM_THREADS) {
+      const int r = i >> DCH_LOG2, ch = i & (DCH - 1);
       const bool ok = q0 + r < p.S;
-      cp_async_16(sQ + swz(r, ch), ok ? p.q + (tok0 + q0 + r) * p.ldq + head * D + ch * 8 : p.q, ok ? 16u : 0u);
-      cp_async_16(sdO + swz(r, ch), ok ? p.dout + (tok0 + q0 + r) * p.lddo + head * D + ch * 8 : p.dout, ok ? 16u : 0u);
+      cp_async_16(sQ + swz<D>(r, ch), ok ? p.q + (tok0 + q0 + r) * p.ldq + head * D + ch * 8 : p.q, ok ? 16u : 0u);
+      cp_async_16(sdO + swz<D>(r, ch), ok ? p.dout + (tok0 + q0 + r) * p.lddo + head * D + ch * 8 : p.dout, ok ? 16u : 0u);
     }
     cp_async_commit();
     for (int i = threadIdx.x; i < BQ; i += NUM_THREADS) {   // BQ divides Spad
@@ -116,16 +123,16 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fa_bwd_kernel(const Params p) 
 #pragma unroll
       for (int i = 0; i < NT; ++i) s[i][0] = s[i][1] = s[i][2] = s[i][3] = dp[i][0] = dp[i][1] = dp[i][2] = dp[i][3] = 0.f;
 #pragma unroll
-      for (int kc = 0; kc < 8; ++kc) {
+      for (int kc = 0; kc < D / 16; ++kc) {
         uint32_t a[4], ad[4];
-        ldsm_x4(sQ + swz(rg * 16 + (lane & 15), kc * 2 + (lane >> 4)), a);
-        ldsm_x4(sdO + swz(rg * 16 + (lane & 15), kc * 2 + (lane >> 4)), ad);
+        ldsm_x4(sQ + swz<D>(rg * 16 + (lane & 15), kc * 2 + (lane >> 4)), a);
+        ldsm_x4(sdO + swz<D>(rg * 16 + (lane & 15), kc * 2 + (lane >> 4)), ad);
 #pragma unroll
         for (int np = 0; np < NT / 2; ++np) {
           const int kr = cs * NT * 8 + np * 16 + (lane & 7) + ((lane >> 4) << 3);
           uint32_t b[4], bv[4];
-          ldsm_x4(sK + swz(kr, kc * 2 + ((lane >> 3) & 1)), b);
-          ldsm_x4(sV + swz(kr, kc * 2 + ((lane >> 3) & 1)), bv);
+          ldsm_x4(sK + swz<D>(kr, kc * 2 + ((lane >> 3) & 1)), b);
+          ldsm_x4(sV + swz<D>(kr, kc * 2 + ((lane >> 3) & 1)), bv);
           mma_bf16_16816(s[2 * np], a, b[0], b[1]);
           mma_bf16_16816(s[2 * np + 1], a, b[2], b[3]);
           mma_bf16_16816(dp[2 * np], ad, bv[0], bv[1]);
@@ -165,11 +172,11 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fa_bwd_kernel(const Params p) 
       ldsm_x4_t(sP + swz64(pr, pc), ap);
       ldsm_x4_t(sdS + swz64(pr, pc), as);
 #pragma unroll
-      for (int dp2 = 0; dp2 < 4; ++dp2) {
-        const int br = qc * 16 + (lane & 7) + ((lane >> 3) & 1) * 8, bc = dh * 8 + dp2 * 2 + (lane >> 4);
+      for (int dp2 = 0; dp2 < D / 32; ++dp2) {
+        const int br = qc * 16 + (lane & 7) + ((lane >> 3) & 1) * 8, bc = dh * (DCH / 2) + dp2 * 2 + (lane >> 4);
         uint32_t bo[4], bq[4];
-        ldsm_x4_t(sdO + swz(br, bc), bo);
-        ldsm_x4_t(sQ + swz(br, bc), bq);
+        ldsm_x4_t(sdO + swz<D>(br, bc), bo);
+        ldsm_x4_t(sQ + swz<D>(br, bc), bq);
         mma_bf16_16816(dv[2 * dp2], ap, bo[0], bo[1]);
         mma_bf16_16816(dv[2 * dp2 + 1], ap, bo[2], bo[3]);
         mma_bf16_16816(dk[2 * dp2], as, bq[0], bq[1]);
@@ -188,7 +195,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fa_bwd_kernel(const Params p) 
 #pragma unroll
         for (int dp2 = 0; dp2 < DTQ / 2; ++dp2) {
           uint32_t b[4];
-          ldsm_x4_t(sK + swz(kc * 16 + (lane & 7) + ((lane >> 3) & 1) * 8, dsl * (DTQ) + dp2 * 2 + (lane >> 4)), b);
+          ldsm_x4_t(sK + swz<D>(kc * 16 + (lane & 7) + ((lane >> 3) & 1) * 8, dsl * (DTQ) + dp2 * 2 + (lane >> 4)), b);
           mma_bf16_16816(dq[2 * dp2], a, b[0], b[1]);
           mma_bf16_16816(dq[2 * dp2 + 1], a, b[2], b[3]);
         }
@@ -212,9 +219,9 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fa_bwd_kernel(const Params p) 
   for (int h = 0; h < 2; ++h) {
     const int r = kv0 + kg * 16 + g + 8 * h;
     if (r >= p.S) continue;
-    const size_t off = ((tok0 + r) * p.kvh + kv_head) * D + dh * 64 + 2 * tq;
+    const size_t off = ((tok0 + r) * p.kvh + kv_head) * D + dh * (D / 2) + 2 * tq;
 #pragma unroll
-    for (int dt = 0; dt < 8; ++dt) {
+    for (int dt = 0; dt < D / 16; ++dt) {
       atomicAdd(p.dk_acc + off + dt * 8, dk[dt][2 * h]);
       atomicAdd(p.dk_acc + off + dt * 8 + 1, dk[dt][2 * h + 1]);
       atomicAdd(p.dv_acc + off + dt * 8, dv[dt][2 * h]);
@@ -225,14 +232,16 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fa_bwd_kernel(const Params p) 
 
 // Per-row statistics of both kernels, [B, nh, Spad] (Spad = S rounded up to 64, so that every 64-row q tile's rows are one
 // 16-byte-aligned block for any S):
-//   delta[b, h, s] = sum_d dO[b,s,h,d] * O[b,s,h,d]      (16 lanes per row of 128)
+//   delta[b, h, s] = sum_d dO[b,s,h,d] * O[b,s,h,d]      (D / 8 lanes per row)
 //   lse2[b, h, s]  = lse[b, h, s] * log2(e)
 // padding rows s >= S get delta = 0 and lse2 = +inf, so P = 0 there.
+template <int D>
 __global__ void fa_bwd_delta_kernel(const bf16* __restrict__ o, const bf16* __restrict__ dout, const float* __restrict__ lse,
                                     float* __restrict__ lse2, float* __restrict__ delta, int B, int S, int Spad, int nh,
                                     int64_t ldo, int64_t lddo) {
-  const int64_t row = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 4;   // (b, s < Spad, h) flattened
-  const int sub = threadIdx.x & 15;
+  constexpr int LPR = D / 8, LPR_LOG2 = D == 128 ? 4 : 3;   // lanes per row
+  const int64_t row = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> LPR_LOG2;   // (b, s < Spad, h) flattened
+  const int sub = threadIdx.x & (LPR - 1);
   const int64_t total = static_cast<int64_t>(B) * Spad * nh;
   float acc = 0.f;
   int b = 0, s = 0, h = 0;
@@ -243,8 +252,8 @@ __global__ void fa_bwd_delta_kernel(const bf16* __restrict__ o, const bf16* __re
   }
   if (row < total && s < S) {
     const int64_t tok = static_cast<int64_t>(b) * S + s;
-    const uint4 ov = ld_nc_v4(reinterpret_cast<const uint4*>(o + tok * ldo + h * 128) + sub);
-    const uint4 dv = ld_nc_v4(reinterpret_cast<const uint4*>(dout + tok * lddo + h * 128) + sub);
+    const uint4 ov = ld_nc_v4(reinterpret_cast<const uint4*>(o + tok * ldo + h * D) + sub);
+    const uint4 dv = ld_nc_v4(reinterpret_cast<const uint4*>(dout + tok * lddo + h * D) + sub);
     const uint32_t* oi = reinterpret_cast<const uint32_t*>(&ov);
     const uint32_t* di = reinterpret_cast<const uint32_t*>(&dv);
 #pragma unroll
@@ -254,7 +263,7 @@ __global__ void fa_bwd_delta_kernel(const bf16* __restrict__ o, const bf16* __re
     }
   }
 #pragma unroll
-  for (int off = 8; off > 0; off >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, off);
+  for (int off = LPR / 2; off > 0; off >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, off);
   if (row < total && sub == 0) {
     const size_t bh = static_cast<size_t>(b) * nh + h;
     delta[bh * Spad + s] = acc;
@@ -287,21 +296,29 @@ constexpr int BKV = 128;                                  // kv rows per CTA, 64
 constexpr int BQ = 64;                                    // q rows per ring stage
 constexpr int STAGES = 2;
 constexpr int NUM_THREADS = 256;                          // two warpgroups, 64 kv rows each
-constexpr int KV_BYTES = BKV * D * 2;                     // K or V: two [128 rows][64 d] swizzled halves
-constexpr int QT_BYTES = BQ * D * 2;                      // Q or dO tile: two [64 rows][64 d] halves
-constexpr int STAGE_BYTES = 2 * QT_BYTES + 2 * BQ * 4;    // Q, dO, lse2, delta
-constexpr int STAGE_STRIDE = 33 * 1024;                   // keeps every stage 1024-byte aligned (128-byte swizzle atoms)
-constexpr int DS_BYTES = BKV * BQ * 2;                    // dS^T [128 kv][64 q] bf16
-constexpr int DQ_BYTES = BQ * 64 * 4;                     // one warpgroup's fp32 dQ tile: two [64 q][32 d] boxes
-constexpr int OFF_K = 0, OFF_V = KV_BYTES, OFF_RING = 2 * KV_BYTES;
-constexpr int OFF_DS = OFF_RING + STAGES * STAGE_STRIDE;  // two dS^T buffers (alternate q tiles)
-constexpr int OFF_DQ = OFF_DS + 2 * DS_BYTES;
-constexpr int OFF_BAR = OFF_DQ + 2 * DQ_BYTES;
-constexpr int SMEM_BYTES = OFF_BAR + 64 + 1024;           // + barriers + alignment slack
-static_assert(SMEM_BYTES <= 227 * 1024, "fa_bwd_wgmma: shared memory");
-// the final dK / dV staging (64 rows x 128 d fp32 per warpgroup) reuses a ring stage, the dS buffers and the dQ buffers
-static_assert(STAGE_BYTES <= STAGE_STRIDE && 64 * D * 4 <= STAGE_STRIDE && 64 * D * 4 <= 2 * DS_BYTES && 64 * D * 4 <= 2 * DQ_BYTES,
-              "fa_bwd_wgmma: shared-memory layout");
+constexpr int HK = BKV * 64 * 2;                          // one swizzled [128 kv rows][64 d] block of K or V
+constexpr int HQ = BQ * 64 * 2;                           // one swizzled [64 q rows][64 d] block of Q or dO
+
+// shared-memory layout at head_dim D
+template <int D>
+struct Layout {
+  static constexpr int KV_BYTES = BKV * D * 2;                       // K or V: D / 64 blocks of HK bytes
+  static constexpr int QT_BYTES = BQ * D * 2;                        // Q or dO tile: D / 64 blocks of HQ bytes
+  static constexpr int STAGE_BYTES = 2 * QT_BYTES + 2 * BQ * 4;      // Q, dO, lse2, delta
+  static constexpr int STAGE_STRIDE = (STAGE_BYTES + 1023) / 1024 * 1024;   // every stage 1024-byte aligned (swizzle atoms)
+  static constexpr int DS_BYTES = BKV * BQ * 2;                      // dS^T [128 kv][64 q] bf16
+  static constexpr int DQ_BYTES = BQ * 64 * 4;                       // one warpgroup's fp32 dQ tile: two [64 q][32 d] boxes
+  static constexpr int OFF_K = 0, OFF_V = KV_BYTES, OFF_RING = 2 * KV_BYTES;
+  static constexpr int OFF_DS = OFF_RING + STAGES * STAGE_STRIDE;    // two dS^T buffers (alternate q tiles)
+  static constexpr int OFF_DQ = OFF_DS + 2 * DS_BYTES;
+  static constexpr int OFF_BAR = OFF_DQ + 2 * DQ_BYTES;
+  static constexpr int SMEM_BYTES = OFF_BAR + 64 + 1024;             // + barriers + alignment slack
+  static_assert(SMEM_BYTES <= 227 * 1024, "fa_bwd_wgmma: shared memory");
+  // the final dK / dV staging (64 rows x D fp32 per warpgroup) reuses a ring stage, the dS buffers and the dQ buffers
+  static_assert(64 * D * 4 <= STAGE_STRIDE && 64 * D * 4 <= 2 * DS_BYTES && 64 * D * 4 <= 2 * DQ_BYTES,
+                "fa_bwd_wgmma: shared-memory layout");
+};
+static_assert(Layout<128>::STAGE_STRIDE == 33 * 1024, "fa_bwd_wgmma: head_dim 128 layout");
 
 struct Params {
   int S, nh, kvh, Spad;
@@ -335,12 +352,16 @@ __device__ __forceinline__ void stage_f32(uint32_t base, const float (&acc)[4 * 
   }
 }
 
-template <bool MASK>
+template <int D, bool MASK>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 fa_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                     const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO,
                     const __grid_constant__ CUtensorMap tmdQ, const __grid_constant__ CUtensorMap tmdK,
                     const __grid_constant__ CUtensorMap tmdV, const Params p) {
+  using L = Layout<D>;
+  constexpr int KV_BYTES = L::KV_BYTES, QT_BYTES = L::QT_BYTES, STAGE_BYTES = L::STAGE_BYTES, STAGE_STRIDE = L::STAGE_STRIDE;
+  constexpr int DS_BYTES = L::DS_BYTES, DQ_BYTES = L::DQ_BYTES;
+  constexpr int OFF_K = L::OFF_K, OFF_V = L::OFF_V, OFF_RING = L::OFF_RING, OFF_DS = L::OFF_DS, OFF_DQ = L::OFF_DQ, OFF_BAR = L::OFF_BAR;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + OFF_BAR);   // [STAGES]
@@ -375,9 +396,9 @@ fa_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     uint8_t* sq = smem + OFF_RING + st * STAGE_STRIDE;
     mbar_arrive_expect_tx(&full_bar[st], STAGE_BYTES);
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      tma_load_4d(&tmQ, &full_bar[st], sq + h * (QT_BYTES / 2), h * 64, head, qt * BQ, batch);
-      tma_load_4d(&tmdO, &full_bar[st], sq + QT_BYTES + h * (QT_BYTES / 2), h * 64, head, qt * BQ, batch);
+    for (int h = 0; h < D / 64; ++h) {
+      tma_load_4d(&tmQ, &full_bar[st], sq + h * HQ, h * 64, head, qt * BQ, batch);
+      tma_load_4d(&tmdO, &full_bar[st], sq + QT_BYTES + h * HQ, h * 64, head, qt * BQ, batch);
     }
     bulk_load(sq + 2 * QT_BYTES, p.lse2 + stat0 + qt * BQ, BQ * 4, &full_bar[st]);
     bulk_load(sq + 2 * QT_BYTES + BQ * 4, p.delta + stat0 + qt * BQ, BQ * 4, &full_bar[st]);
@@ -385,9 +406,9 @@ fa_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   if (threadIdx.x == 0) {
     mbar_arrive_expect_tx(kv_bar, 2 * KV_BYTES);
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      tma_load_4d(&tmK, kv_bar, smem + OFF_K + h * (KV_BYTES / 2), h * 64, kv_head, kv0, batch);
-      tma_load_4d(&tmV, kv_bar, smem + OFF_V + h * (KV_BYTES / 2), h * 64, kv_head, kv0, batch);
+    for (int h = 0; h < D / 64; ++h) {
+      tma_load_4d(&tmK, kv_bar, smem + OFF_K + h * HK, h * 64, kv_head, kv0, batch);
+      tma_load_4d(&tmV, kv_bar, smem + OFF_V + h * HK, h * 64, kv_head, kv0, batch);
     }
     for (int i = 0; i < STAGES && q_lo + i < q_hi; ++i) load_q_tile(q_lo + i, i);
   }
@@ -404,9 +425,9 @@ fa_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     for (int i = 0; i < 2; ++i)
       if (kv_r + 8 * i < p.S) ms[i] = __ldg(p.mask_start + static_cast<size_t>(batch) * p.S + kv_r + 8 * i);
   }
-  float dk[64], dv[64];
+  float dk[D / 2], dv[D / 2];
 #pragma unroll
-  for (int i = 0; i < 64; ++i) dk[i] = dv[i] = 0.f;
+  for (int i = 0; i < D / 2; ++i) dk[i] = dv[i] = 0.f;
   mbar_wait_nocall(kv_bar, 0);
 
   for (int qt = q_lo, it = 0; qt < q_hi; ++qt, ++it) {
@@ -426,8 +447,8 @@ fa_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     float s[32];
     wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < 8; ++kk) {
-      const uint32_t ko = (kk >> 2) * (KV_BYTES / 2) + cw * 64 * 128 + (kk & 3) * 32, qo = (kk >> 2) * (QT_BYTES / 2) + (kk & 3) * 32;
+    for (int kk = 0; kk < D / 16; ++kk) {
+      const uint32_t ko = (kk >> 2) * HK + cw * 64 * 128 + (kk & 3) * 32, qo = (kk >> 2) * HQ + (kk & 3) * 32;
       wgmma_m64n64k16<0, 0>(s, wgmma_desc_sw128(sK + ko, 16, 1024), wgmma_desc_sw128(sQ + qo, 16, 1024), kk > 0 ? 1u : 0u);
     }
     wgmma_commit();
@@ -453,8 +474,8 @@ fa_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     float dp[32];
     wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < 8; ++kk) {
-      const uint32_t ko = (kk >> 2) * (KV_BYTES / 2) + cw * 64 * 128 + (kk & 3) * 32, qo = (kk >> 2) * (QT_BYTES / 2) + (kk & 3) * 32;
+    for (int kk = 0; kk < D / 16; ++kk) {
+      const uint32_t ko = (kk >> 2) * HK + cw * 64 * 128 + (kk & 3) * 32, qo = (kk >> 2) * HQ + (kk & 3) * 32;
       wgmma_m64n64k16<0, 0>(dp, wgmma_desc_sw128(sV + ko, 16, 1024), wgmma_desc_sw128(sdO + qo, 16, 1024), kk > 0 ? 1u : 0u);
     }
     wgmma_commit();
@@ -482,10 +503,17 @@ fa_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     }
     // dV += P^T dO, dK += dS^T Q: B = dO / Q, MN-major (d contiguous), k = 16 q rows = 2048 bytes
     wgmma_fence();
+    if constexpr (D == 128) {
 #pragma unroll
-    for (int k = 0; k < 4; ++k) wgmma_m64n128k16_rs<1>(dv, pa + 4 * k, wgmma_desc_sw128(sdO + k * 2048, QT_BYTES / 2, 1024), 1u);
+      for (int k = 0; k < 4; ++k) wgmma_m64n128k16_rs<1>(dv, pa + 4 * k, wgmma_desc_sw128(sdO + k * 2048, HQ, 1024), 1u);
 #pragma unroll
-    for (int k = 0; k < 4; ++k) wgmma_m64n128k16_rs<1>(dk, da + 4 * k, wgmma_desc_sw128(sQ + k * 2048, QT_BYTES / 2, 1024), 1u);
+      for (int k = 0; k < 4; ++k) wgmma_m64n128k16_rs<1>(dk, da + 4 * k, wgmma_desc_sw128(sQ + k * 2048, HQ, 1024), 1u);
+    } else {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) wgmma_m64n64k16_rs<1>(dv, pa + 4 * k, wgmma_desc_sw128(sdO + k * 2048, HQ, 1024), 1u);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) wgmma_m64n64k16_rs<1>(dk, da + 4 * k, wgmma_desc_sw128(sQ + k * 2048, HQ, 1024), 1u);
+    }
     wgmma_commit();
     // dS^T -> shared memory, [128 kv][64 q] bf16, 128-byte swizzle: the MN-major A operand of dQ = dS K
     const uint32_t sdS = sbase + OFF_DS + (it & 1) * DS_BYTES;
@@ -497,13 +525,22 @@ fa_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
         asm volatile("st.shared.b32 [%0], %1;" ::"r"(sdS + row * 128 + ((j ^ (row & 7)) << 4) + tq * 4), "r"(da[2 * j + i]) : "memory");
     }
     fence_proxy_async_smem();
-    named_bar_sync(1, 256);   // both warpgroups' dS^T rows are in shared memory
-    // dQ[64 q][64 d of this warpgroup] = dS K: A = dS^T buffer (MN-major), B = K half cw (MN-major), k = 16 kv rows
     float dq[32];   // no initial value: the first wgmma (accumulate = 0) overwrites it
+    if constexpr (D == 128) {
+      named_bar_sync(1, 256);   // both warpgroups' dS^T rows are in shared memory
+      // dQ[64 q][64 d of this warpgroup] = dS K: A = dS^T buffer (MN-major), B = K half cw (MN-major), k = 16 kv rows
 #pragma unroll
-    for (int kk = 0; kk < 8; ++kk)
-      wgmma_m64n64k16<1, 1>(dq, wgmma_desc_sw128(sdS + kk * 2048, DS_BYTES, 1024),
-                            wgmma_desc_sw128(sK + cw * (KV_BYTES / 2) + kk * 2048, KV_BYTES / 2, 1024), kk > 0 ? 1u : 0u);
+      for (int kk = 0; kk < 8; ++kk)
+        wgmma_m64n64k16<1, 1>(dq, wgmma_desc_sw128(sdS + kk * 2048, DS_BYTES, 1024),
+                              wgmma_desc_sw128(sK + cw * HK + kk * 2048, HK, 1024), kk > 0 ? 1u : 0u);
+    } else {
+      named_bar_sync(2 + cw, 128);   // this warpgroup's dS^T rows are in shared memory
+      // dQ partial [64 q][64 d] = dS[:, this warpgroup's 64 kv rows] K[those rows, :]
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk)
+        wgmma_m64n64k16<1, 1>(dq, wgmma_desc_sw128(sdS + cw * 64 * 128 + kk * 2048, DS_BYTES, 1024),
+                              wgmma_desc_sw128(sK + cw * 64 * 128 + kk * 2048, HK, 1024), kk > 0 ? 1u : 0u);
+    }
     wgmma_commit();
     wgmma_wait<0>();
     reg_fence(dq);
@@ -518,8 +555,9 @@ fa_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     fence_proxy_async_smem();
     named_bar_sync(2 + cw, 128);
     if (leader) {
-      tma_reduce_add_4d(&tmdQ, sdq, cw * 64, head, q0, batch);
-      tma_reduce_add_4d(&tmdQ, sdq + DQ_BYTES / 2, cw * 64 + 32, head, q0, batch);
+      const int d0 = D == 128 ? cw * 64 : 0;
+      tma_reduce_add_4d(&tmdQ, sdq, d0, head, q0, batch);
+      tma_reduce_add_4d(&tmdQ, sdq + DQ_BYTES / 2, d0 + 32, head, q0, batch);
       tma_store_commit();
     }
   }
@@ -530,13 +568,13 @@ fa_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   named_bar_sync(1, 256);
   uint8_t* sdk = smem + OFF_RING + cw * STAGE_STRIDE;
   uint8_t* sdv = smem + (cw == 0 ? OFF_DS : OFF_DQ);
-  stage_f32<16>(smem_u32(sdk), dk, wi, lane);
-  stage_f32<16>(smem_u32(sdv), dv, wi, lane);
+  stage_f32<D / 8>(smem_u32(sdk), dk, wi, lane);
+  stage_f32<D / 8>(smem_u32(sdv), dv, wi, lane);
   fence_proxy_async_smem();
   named_bar_sync(2 + cw, 128);
   if (leader) {
 #pragma unroll
-    for (int b = 0; b < 4; ++b) {
+    for (int b = 0; b < D / 32; ++b) {
       tma_reduce_add_4d(&tmdK, sdk + b * (64 * 128), b * 32, kv_head, kv0 + cw * 64, batch);
       tma_reduce_add_4d(&tmdV, sdv + b * (64 * 128), b * 32, kv_head, kv0 + cw * 64, batch);
     }
@@ -545,24 +583,27 @@ fa_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   }
 }
 
-// [B, S, heads, 128] bf16 view with token stride ld, box {64 d, 1 head, rows, 1}: one 128-byte swizzled half of `rows` rows
-static int make_bf16_map(CUtensorMap* tm, const void* base, int64_t B, int64_t S, int64_t heads, int64_t ld, uint32_t rows) {
-  const uint64_t dims[4] = {128, static_cast<uint64_t>(heads), static_cast<uint64_t>(S), static_cast<uint64_t>(B)};
-  const uint64_t strides[3] = {256, static_cast<uint64_t>(ld) * 2, static_cast<uint64_t>(S * ld) * 2};
+// [B, S, heads, D] bf16 view with token stride ld, box {64 d, 1 head, rows, 1}: one 128-byte swizzled block of `rows` rows
+static int make_bf16_map(CUtensorMap* tm, const void* base, int64_t B, int64_t S, int64_t heads, int64_t D, int64_t ld,
+                         uint32_t rows) {
+  const uint64_t dims[4] = {static_cast<uint64_t>(D), static_cast<uint64_t>(heads), static_cast<uint64_t>(S), static_cast<uint64_t>(B)};
+  const uint64_t strides[3] = {static_cast<uint64_t>(D) * 2, static_cast<uint64_t>(ld) * 2, static_cast<uint64_t>(S * ld) * 2};
   const uint32_t box[4] = {64, 1, rows, 1};
   return encode_tmap_bf16(tm, base, 4, dims, strides, box);
 }
-// [B, S, heads, 128] fp32 accumulation buffer, box {32 d, 1 head, 64 rows, 1}
-static int make_f32_map(CUtensorMap* tm, float* base, int64_t B, int64_t S, int64_t heads) {
-  const uint64_t dims[4] = {128, static_cast<uint64_t>(heads), static_cast<uint64_t>(S), static_cast<uint64_t>(B)};
-  const uint64_t strides[3] = {512, static_cast<uint64_t>(heads) * 512, static_cast<uint64_t>(S * heads) * 512};
+// [B, S, heads, D] fp32 accumulation buffer, box {32 d, 1 head, 64 rows, 1}
+static int make_f32_map(CUtensorMap* tm, float* base, int64_t B, int64_t S, int64_t heads, int64_t D) {
+  const uint64_t dims[4] = {static_cast<uint64_t>(D), static_cast<uint64_t>(heads), static_cast<uint64_t>(S), static_cast<uint64_t>(B)};
+  const uint64_t row = static_cast<uint64_t>(D) * 4;
+  const uint64_t strides[3] = {row, static_cast<uint64_t>(heads) * row, static_cast<uint64_t>(S * heads) * row};
   const uint32_t box[4] = {32, 1, 64, 1};
   return encode_tmap_f32(tm, base, 4, dims, strides, box);
 }
 
-template <bool MASK>
+template <int D, bool MASK>
 static int launch(const CUtensorMap (&tm)[7], const Params& p, int B, cudaStream_t stream) {
-  auto kern = fa_bwd_wgmma_kernel<MASK>;
+  constexpr int SMEM_BYTES = Layout<D>::SMEM_BYTES;
+  auto kern = fa_bwd_wgmma_kernel<D, MASK>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
@@ -578,12 +619,12 @@ static int launch(const CUtensorMap (&tm)[7], const Params& p, int B, cudaStream
 }
 }  // namespace wg
 
-template <int BQ, bool MASK>
+template <int D, int BQ, bool MASK>
 static int launch(const Params& p, cudaStream_t stream) {
-  constexpr int SMEM = 2 * BKV * 256 + 2 * BQ * 256 + 2 * BQ * 128 + 2 * BQ * 4;
+  constexpr int SMEM = 2 * BKV * D * 2 + 2 * BQ * D * 2 + 2 * BQ * 128 + 2 * BQ * 4;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(fa_bwd_kernel<BQ, MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
+    cudaError_t e = cudaFuncSetAttribute(fa_bwd_kernel<D, BQ, MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
     if (e != cudaSuccess) {
       set_last_error("fa_bwd smem attr: %s", cudaGetErrorString(e));
       return static_cast<int>(e);
@@ -591,7 +632,7 @@ static int launch(const Params& p, cudaStream_t stream) {
     attr_set = true;
   }
   dim3 grid(static_cast<unsigned>((p.S + BKV - 1) / BKV), static_cast<unsigned>(p.nh), static_cast<unsigned>(p.B));
-  fa_bwd_kernel<BQ, MASK><<<grid, NUM_THREADS, SMEM, stream>>>(p);
+  fa_bwd_kernel<D, BQ, MASK><<<grid, NUM_THREADS, SMEM, stream>>>(p);
   return check_launch("fa_bwd");
 }
 
@@ -622,7 +663,7 @@ extern "C" int b200_fa_bwd_flashmask(const void* q, const void* k, const void* v
   using namespace b200;
   using namespace b200::fab;
   B200_CHECK_ARG(q && k && v && o && dout && lse && dq && dk && dv && workspace, "fa_bwd: null pointer");
-  B200_CHECK_ARG(head_dim == 128, "fa_bwd: head_dim must be 128 (got %lld)", (long long)head_dim);
+  B200_CHECK_ARG(head_dim == 64 || head_dim == 128, "fa_bwd: head_dim must be 64 or 128 (got %lld)", (long long)head_dim);
   B200_CHECK_ARG(B > 0 && S > 0 && num_heads > 0 && num_kv_heads > 0 && num_heads % num_kv_heads == 0, "fa_bwd: bad shape");
   B200_CHECK_ARG(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0 && lddo % 8 == 0 && lddq % 8 == 0 &&
                      lddk % 8 == 0 && lddv % 8 == 0,
@@ -636,21 +677,24 @@ extern "C" int b200_fa_bwd_flashmask(const void* q, const void* k, const void* v
   }
   const int64_t Spad = (S + 63) / 64 * 64;
   float* dq_acc = static_cast<float*>(workspace);
-  float* dk_acc = dq_acc + B * S * num_heads * 128;
-  float* dv_acc = dk_acc + B * S * num_kv_heads * 128;
-  float* lse2 = dq_acc + 3 * B * S * num_heads * 128;
+  float* dk_acc = dq_acc + B * S * num_heads * head_dim;
+  float* dv_acc = dk_acc + B * S * num_kv_heads * head_dim;
+  float* lse2 = dq_acc + 3 * B * S * num_heads * head_dim;
   float* delta = lse2 + B * num_heads * Spad;
-  cudaError_t e = cudaMemsetAsync(dq_acc, 0, static_cast<size_t>(B) * S * (num_heads + 2 * num_kv_heads) * 128 * 4, stream);
+  cudaError_t e = cudaMemsetAsync(dq_acc, 0, static_cast<size_t>(B) * S * (num_heads + 2 * num_kv_heads) * head_dim * 4, stream);
   if (e != cudaSuccess) {
     set_last_error("fa_bwd memset: %s", cudaGetErrorString(e));
     return static_cast<int>(e);
   }
   {
     const int64_t rows = B * Spad * num_heads;
-    const int64_t threads = rows * 16;
-    fa_bwd_delta_kernel<<<static_cast<unsigned>((threads + 255) / 256), 256, 0, stream>>>(
-        static_cast<const bf16*>(o), static_cast<const bf16*>(dout), lse, lse2, delta, (int)B, (int)S, (int)Spad, (int)num_heads,
-        ldo, lddo);
+    const int64_t threads = rows * (head_dim / 8);
+    const unsigned blocks = static_cast<unsigned>((threads + 255) / 256);
+    const bf16 *op = static_cast<const bf16*>(o), *dop = static_cast<const bf16*>(dout);
+    if (head_dim == 64)
+      fa_bwd_delta_kernel<64><<<blocks, 256, 0, stream>>>(op, dop, lse, lse2, delta, (int)B, (int)S, (int)Spad, (int)num_heads, ldo, lddo);
+    else
+      fa_bwd_delta_kernel<128><<<blocks, 256, 0, stream>>>(op, dop, lse, lse2, delta, (int)B, (int)S, (int)Spad, (int)num_heads, ldo, lddo);
     int rc = check_launch("fa_bwd(delta)");
     if (rc) return rc;
   }
@@ -666,28 +710,34 @@ extern "C" int b200_fa_bwd_flashmask(const void* q, const void* k, const void* v
     p.lse2 = lse2; p.delta = delta;
     p.mask_start = mask_start_rows;
     p.dq_acc = dq_acc; p.dk_acc = dk_acc; p.dv_acc = dv_acc;
-    rc = mask_start_rows ? launch<64, true>(p, stream) : launch<64, false>(p, stream);
+    if (head_dim == 64)
+      rc = mask_start_rows ? launch<64, 64, true>(p, stream) : launch<64, 64, false>(p, stream);
+    else
+      rc = mask_start_rows ? launch<128, 64, true>(p, stream) : launch<128, 64, false>(p, stream);
   } else {
     CUtensorMap tm[7];
-    if ((rc = wg::make_bf16_map(&tm[0], q, B, S, num_heads, ldq, wg::BQ)) != 0) return rc;
-    if ((rc = wg::make_bf16_map(&tm[1], k, B, S, num_kv_heads, ldk, wg::BKV)) != 0) return rc;
-    if ((rc = wg::make_bf16_map(&tm[2], v, B, S, num_kv_heads, ldv, wg::BKV)) != 0) return rc;
-    if ((rc = wg::make_bf16_map(&tm[3], dout, B, S, num_heads, lddo, wg::BQ)) != 0) return rc;
-    if ((rc = wg::make_f32_map(&tm[4], dq_acc, B, S, num_heads)) != 0) return rc;
-    if ((rc = wg::make_f32_map(&tm[5], dk_acc, B, S, num_kv_heads)) != 0) return rc;
-    if ((rc = wg::make_f32_map(&tm[6], dv_acc, B, S, num_kv_heads)) != 0) return rc;
+    if ((rc = wg::make_bf16_map(&tm[0], q, B, S, num_heads, head_dim, ldq, wg::BQ)) != 0) return rc;
+    if ((rc = wg::make_bf16_map(&tm[1], k, B, S, num_kv_heads, head_dim, ldk, wg::BKV)) != 0) return rc;
+    if ((rc = wg::make_bf16_map(&tm[2], v, B, S, num_kv_heads, head_dim, ldv, wg::BKV)) != 0) return rc;
+    if ((rc = wg::make_bf16_map(&tm[3], dout, B, S, num_heads, head_dim, lddo, wg::BQ)) != 0) return rc;
+    if ((rc = wg::make_f32_map(&tm[4], dq_acc, B, S, num_heads, head_dim)) != 0) return rc;
+    if ((rc = wg::make_f32_map(&tm[5], dk_acc, B, S, num_kv_heads, head_dim)) != 0) return rc;
+    if ((rc = wg::make_f32_map(&tm[6], dv_acc, B, S, num_kv_heads, head_dim)) != 0) return rc;
     wg::Params p;
     p.S = (int)S; p.nh = (int)num_heads; p.kvh = (int)num_kv_heads; p.Spad = (int)Spad;
     p.scale = softmax_scale;
     p.scale_log2 = softmax_scale * 1.4426950408889634f;
     p.lse2 = lse2; p.delta = delta;
     p.mask_start = mask_start_rows;
-    rc = mask_start_rows ? wg::launch<true>(tm, p, (int)B, stream) : wg::launch<false>(tm, p, (int)B, stream);
+    if (head_dim == 64)
+      rc = mask_start_rows ? wg::launch<64, true>(tm, p, (int)B, stream) : wg::launch<64, false>(tm, p, (int)B, stream);
+    else
+      rc = mask_start_rows ? wg::launch<128, true>(tm, p, (int)B, stream) : wg::launch<128, false>(tm, p, (int)B, stream);
   }
   if (rc) return rc;
   {
     const int64_t tokens = B * S;
-    const int width = static_cast<int>(num_heads * 128);
+    const int width = static_cast<int>(num_heads * head_dim);
     const int64_t total = tokens * (width / 8);
     int64_t blocks = (total + 255) / 256;
     const int64_t cap = static_cast<int64_t>(sm_count()) * 16;
@@ -695,7 +745,7 @@ extern "C" int b200_fa_bwd_flashmask(const void* q, const void* k, const void* v
     fa_bwd_dq_finish_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(dq_acc, static_cast<bf16*>(dq), tokens,
                                                                               width, lddq);
     if ((rc = check_launch("fa_bwd(dq finish)")) != 0) return rc;
-    const int kvw = static_cast<int>(num_kv_heads * 128);
+    const int kvw = static_cast<int>(num_kv_heads * head_dim);
     int64_t kblocks = (tokens * (kvw / 8) + 255) / 256;
     if (kblocks > cap) kblocks = cap;
     fa_bwd_dq_finish_kernel<<<static_cast<unsigned>(kblocks), 256, 0, stream>>>(dk_acc, static_cast<bf16*>(dk), tokens, kvw,

@@ -256,19 +256,22 @@ __global__ void decode_rope_append_kernel(bf16* __restrict__ qkv, float* __restr
 
 // ------------------------------------------------------------------------------------------------
 // Decode attention: one query token per sequence over the cache, GQA group shares each K/V row read.
-//   CTA = (batch, kv head); 4 warps; a half-warp (16 lanes x 16 B) reads one 256-byte K row, so a warp covers two
-//   cache rows per load; every lane keeps its 8 dims of q / o for the G q-heads of the group in registers;
-//   online softmax (exp2, fp32) per half-warp, merged across the 8 half-warps through shared memory.
+//   CTA = (batch, kv head); 4 warps; a row group of D / 8 lanes x 16 B reads one K row (a half-warp at d = 128, a quarter
+//   at d = 64), so a warp covers 2 (4) cache rows per load; every lane keeps its 8 dims of q / o for the G q-heads of the
+//   group in registers; online softmax (exp2, fp32) per row group, merged across the 8 (16) row groups through shared memory.
 // HBM roofline: 2 * len * d * 2 bytes per (b, kv head).
+// Split-KV partials: DECODE_PART_ROW-float rows (common.cuh).
 // ------------------------------------------------------------------------------------------------
-template <int G>
+
+template <int D, int G>
 __global__ void __launch_bounds__(128, (G <= 4 ? 4 : 2)) decode_attention_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ cache,
                                                                const int* __restrict__ seq_lens, bf16* __restrict__ out,
                                                                float* __restrict__ partial, int B, int nh, int kvh,
                                                                int max_len, int64_t ld, float scale_log2) {
-  constexpr int D = 128;
-  __shared__ float s_m[8][G], s_l[8][G];
-  __shared__ float s_o[8][G][D];
+  constexpr int LPR = D / 8, LPR_LOG2 = D == 128 ? 4 : 3;   // lanes per cache row
+  constexpr int NG = 128 / LPR;                              // row groups per CTA
+  __shared__ float s_m[NG][G], s_l[NG][G];
+  __shared__ float s_o[NG][G][D];
   pdl_launch_dependents();
   const int b = blockIdx.x / kvh, kh = blockIdx.x % kvh;
   const int total_len = min(seq_lens[b] + 1, max_len);  // the new token was appended at index seq_lens[b]
@@ -278,9 +281,11 @@ __global__ void __launch_bounds__(128, (G <= 4 ? 4 : 2)) decode_attention_kernel
   const int t_begin = split * chunk;
   const int len = min(total_len, t_begin + chunk);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int hw = warp * 2 + (lane >> 4);               // half-warp id 0..7
-  const int sub = lane & 15;                           // which 8 dims of the row
-  const unsigned hmask = (lane < 16) ? 0x0000ffffu : 0xffff0000u;
+  const int hw = warp * (32 / LPR) + (lane >> LPR_LOG2);   // row group id 0..NG-1
+  const int sub = lane & (LPR - 1);                         // which 8 dims of the row
+  unsigned hmask;
+  if constexpr (D == 128) hmask = (lane < 16) ? 0x0000ffffu : 0xffff0000u;
+  else hmask = 0xffu << (lane & 24);
   float q[G][8], o[G][8], m[G], l[G];
 #pragma unroll
   for (int g = 0; g < G; ++g) {
@@ -298,12 +303,12 @@ __global__ void __launch_bounds__(128, (G <= 4 ? 4 : 2)) decode_attention_kernel
   const size_t half = static_cast<size_t>(B) * kvh * max_len * D;
   const bf16* kbase = cache + (static_cast<size_t>(b) * kvh + kh) * max_len * D;
   const bf16* vbase = kbase + half;
-  constexpr int U = 4;      // rows in flight per half-warp: 8 x 16-byte loads issued before any math (memory-level parallelism)
-  for (int t0 = t_begin + hw; t0 < len; t0 += 8 * U) {
+  constexpr int U = 4;      // rows in flight per row group: 8 x 16-byte loads issued before any math (memory-level parallelism)
+  for (int t0 = t_begin + hw; t0 < len; t0 += NG * U) {
     uint4 kv[U], vv[U];
 #pragma unroll
     for (int u = 0; u < U; ++u) {
-      const int t = t0 + 8 * u;
+      const int t = t0 + NG * u;
       if (t < len) {
         kv[u] = ld_nc_v4(reinterpret_cast<const uint4*>(kbase + static_cast<size_t>(t) * D) + sub);
         vv[u] = ld_nc_v4(reinterpret_cast<const uint4*>(vbase + static_cast<size_t>(t) * D) + sub);
@@ -328,8 +333,8 @@ __global__ void __launch_bounds__(128, (G <= 4 ? 4 : 2)) decode_attention_kernel
       }
     }
 #pragma unroll
-    for (int off = 8; off > 0; off >>= 1) {
-      // the two half-warps of a warp can have different trip counts: shuffle within the half-warp only
+    for (int off = LPR / 2; off > 0; off >>= 1) {
+      // the row groups of a warp can have different trip counts: shuffle within the row group only
 #pragma unroll
       for (int u = 0; u < U; ++u)
 #pragma unroll
@@ -340,7 +345,7 @@ __global__ void __launch_bounds__(128, (G <= 4 ? 4 : 2)) decode_attention_kernel
       float mn = m[g];
 #pragma unroll
       for (int u = 0; u < U; ++u)
-        if (t0 + 8 * u < len) mn = fmaxf(mn, sc[u][g]);
+        if (t0 + NG * u < len) mn = fmaxf(mn, sc[u][g]);
       const float corr = fast_exp2(m[g] - mn);      // m = -inf on the first block -> corr = 0, o and l are still 0
       m[g] = mn;
       l[g] *= corr;
@@ -349,7 +354,7 @@ __global__ void __launch_bounds__(128, (G <= 4 ? 4 : 2)) decode_attention_kernel
     }
 #pragma unroll
     for (int u = 0; u < U; ++u) {
-      if (t0 + 8 * u < len) {                      // uniform within the half-warp
+      if (t0 + NG * u < len) {                     // uniform within the row group
         const uint32_t* vi = reinterpret_cast<const uint32_t*>(&vv[u]);
         float vf[8];
 #pragma unroll
@@ -364,7 +369,7 @@ __global__ void __launch_bounds__(128, (G <= 4 ? 4 : 2)) decode_attention_kernel
       }
     }
   }
-  // merge the 8 half-warp partials
+  // merge the NG row-group partials
 #pragma unroll
   for (int g = 0; g < G; ++g) {
     if (sub == 0) { s_m[hw][g] = m[g]; s_l[hw][g] = l[g]; }
@@ -376,10 +381,10 @@ __global__ void __launch_bounds__(128, (G <= 4 ? 4 : 2)) decode_attention_kernel
     const int g = idx / D, dd = idx % D;
     float mm = -INFINITY;
 #pragma unroll
-    for (int w = 0; w < 8; ++w) mm = fmaxf(mm, s_m[w][g]);
+    for (int w = 0; w < NG; ++w) mm = fmaxf(mm, s_m[w][g]);
     float acc = 0.f, lt = 0.f;
 #pragma unroll
-    for (int w = 0; w < 8; ++w) {
+    for (int w = 0; w < NG; ++w) {
       const float f = (s_m[w][g] == -INFINITY) ? 0.f : exp2f(s_m[w][g] - mm);
       acc += s_o[w][g][dd] * f;
       lt += s_l[w][g] * f;
@@ -387,39 +392,47 @@ __global__ void __launch_bounds__(128, (G <= 4 ? 4 : 2)) decode_attention_kernel
     if (nsplit == 1) {
       out[static_cast<size_t>(b) * nh * D + (kh * G + g) * D + dd] = __float2bfloat16_rn(lt > 0.f ? acc / lt : 0.f);
     } else {
-      // partial[b, head, split, 0:128] = unnormalised o ; [.., 128] = running max (log2 units) ; [.., 129] = sum
-      // (row stride 132 floats keeps the float4 reads of the merge kernel 16-byte aligned)
-      float* dst = partial + ((static_cast<size_t>(b) * nh + kh * G + g) * nsplit + split) * (D + 4);
+      float* dst = partial + ((static_cast<size_t>(b) * nh + kh * G + g) * nsplit + split) * DECODE_PART_ROW;
       dst[dd] = acc;
-      if (dd == 0) { dst[D] = mm; dst[D + 1] = lt; }
+      if (dd == 0) { dst[DECODE_PART_M] = mm; dst[DECODE_PART_M + 1] = lt; }
     }
   }
 }
 
-// merge the split-KV partials: one warp per (b, head)
+// merge the split-KV partials: one warp per (b, head); reads the first D columns of o
+template <int D>
 __global__ void decode_attention_merge_kernel(const float* __restrict__ partial, bf16* __restrict__ out, int rows, int nsplit) {
-  constexpr int D = 128;
+  constexpr int W = DECODE_PART_ROW, M = DECODE_PART_M;
   pdl_launch_dependents();
   pdl_wait();
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (row >= rows) return;
-  const float* base = partial + static_cast<size_t>(row) * nsplit * (D + 4);
+  const float* base = partial + static_cast<size_t>(row) * nsplit * W;
   float mm = -INFINITY;
-  for (int s = 0; s < nsplit; ++s) mm = fmaxf(mm, base[s * (D + 4) + D]);
+  for (int s = 0; s < nsplit; ++s) mm = fmaxf(mm, base[s * W + M]);
   float acc[4] = {0.f, 0.f, 0.f, 0.f}, lt = 0.f;
   for (int s = 0; s < nsplit; ++s) {
-    const float ms = base[s * (D + 4) + D];
+    const float ms = base[s * W + M];
     const float f = (ms == -INFINITY) ? 0.f : exp2f(ms - mm);
-    lt += base[s * (D + 4) + D + 1] * f;
-    const float4 o = *reinterpret_cast<const float4*>(base + s * (D + 4) + lane * 4);
-    acc[0] += o.x * f; acc[1] += o.y * f; acc[2] += o.z * f; acc[3] += o.w * f;
+    lt += base[s * W + M + 1] * f;
+    if constexpr (D == 128) {
+      const float4 o = *reinterpret_cast<const float4*>(base + s * W + lane * 4);
+      acc[0] += o.x * f; acc[1] += o.y * f; acc[2] += o.z * f; acc[3] += o.w * f;
+    } else {
+      const float2 o = *reinterpret_cast<const float2*>(base + s * W + lane * 2);
+      acc[0] += o.x * f; acc[1] += o.y * f;
+    }
   }
   const float inv = lt > 0.f ? 1.f / lt : 0.f;
-  uint2 o2;
-  o2.x = pack_bf16x2(acc[0] * inv, acc[1] * inv);
-  o2.y = pack_bf16x2(acc[2] * inv, acc[3] * inv);
-  *reinterpret_cast<uint2*>(out + static_cast<size_t>(row) * D + lane * 4) = o2;
+  if constexpr (D == 128) {
+    uint2 o2;
+    o2.x = pack_bf16x2(acc[0] * inv, acc[1] * inv);
+    o2.y = pack_bf16x2(acc[2] * inv, acc[3] * inv);
+    *reinterpret_cast<uint2*>(out + static_cast<size_t>(row) * D + lane * 4) = o2;
+  } else {
+    *reinterpret_cast<uint32_t*>(out + static_cast<size_t>(row) * D + lane * 2) = pack_bf16x2(acc[0] * inv, acc[1] * inv);
+  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -932,15 +945,19 @@ extern "C" int b200_decode_rope_append_paged(void* qkv, float* acc_f32_ws, const
 
 namespace b200 {
 // shared with decode_attn_tc.cu
-int launch_decode_attention_merge(const float* partial, void* out, int rows, int nsplit, cudaStream_t stream) {
-  launch_pdl(gen::decode_attention_merge_kernel, dim3((rows + 3) / 4), dim3(128), 0, stream, partial, static_cast<bf16*>(out), rows,
-             nsplit);
+int launch_decode_attention_merge(const float* partial, void* out, int rows, int nsplit, int head_dim, cudaStream_t stream) {
+  if (head_dim == 64)
+    launch_pdl(gen::decode_attention_merge_kernel<64>, dim3((rows + 3) / 4), dim3(128), 0, stream, partial, static_cast<bf16*>(out),
+               rows, nsplit);
+  else
+    launch_pdl(gen::decode_attention_merge_kernel<128>, dim3((rows + 3) / 4), dim3(128), 0, stream, partial, static_cast<bf16*>(out),
+               rows, nsplit);
   return check_launch("decode_attention(merge)");
 }
 }  // namespace b200
 
 extern "C" int64_t b200_decode_attention_workspace_bytes(int64_t B, int64_t num_heads, int64_t num_splits) {
-  return num_splits > 1 ? B * num_heads * num_splits * (128 + 4) * 4 : 0;
+  return num_splits > 1 ? B * num_heads * num_splits * DECODE_PART_ROW * 4 : 0;
 }
 
 extern "C" int b200_decode_attention(const void* qkv, const void* cache, const int32_t* seq_lens, void* out, void* workspace,
@@ -948,7 +965,7 @@ extern "C" int b200_decode_attention(const void* qkv, const void* cache, const i
                                      int64_t ld, float softmax_scale, int64_t num_splits, cudaStream_t stream) {
   B200_CHECK_ARG(qkv && cache && seq_lens && out, "decode_attention: null pointer");
   B200_CHECK_ARG(num_splits >= 1 && num_splits <= 64 && (num_splits == 1 || workspace), "decode_attention: bad num_splits / workspace");
-  B200_CHECK_ARG(head_dim == 128, "decode_attention: head_dim must be 128 (got %lld)", (long long)head_dim);
+  B200_CHECK_ARG(head_dim == 64 || head_dim == 128, "decode_attention: head_dim must be 64 or 128 (got %lld)", (long long)head_dim);
   B200_CHECK_ARG(num_heads % num_kv_heads == 0, "decode_attention: num_heads %% num_kv_heads != 0");
   const int G = static_cast<int>(num_heads / num_kv_heads);
   const float sl2 = softmax_scale * 1.4426950408889634f;
@@ -957,22 +974,28 @@ extern "C" int b200_decode_attention(const void* qkv, const void* cache, const i
   const bf16* c = static_cast<const bf16*>(cache);
   bf16* o = static_cast<bf16*>(out);
   float* part = static_cast<float*>(workspace);
-#define B200_DA(GG)                                                                                                  \
+#define B200_DA(DD, GG)                                                                                              \
   case GG:                                                                                                           \
-    decode_attention_kernel<GG><<<grid, block, 0, stream>>>(q, c, seq_lens, o, part, (int)B, (int)num_heads,         \
-                                                            (int)num_kv_heads, (int)max_len, ld, sl2);              \
+    decode_attention_kernel<DD, GG><<<grid, block, 0, stream>>>(q, c, seq_lens, o, part, (int)B, (int)num_heads,     \
+                                                                (int)num_kv_heads, (int)max_len, ld, sl2);          \
     break;
-  switch (G) {
-    B200_DA(1) B200_DA(2) B200_DA(3) B200_DA(4) B200_DA(5) B200_DA(6) B200_DA(7) B200_DA(8)
-    default:
-      return fail_arg("decode_attention: GQA group size %d not instantiated (1 to 8)", G);
+#define B200_DA_G(DD)                                                                                                \
+  switch (G) {                                                                                                       \
+    B200_DA(DD, 1) B200_DA(DD, 2) B200_DA(DD, 3) B200_DA(DD, 4) B200_DA(DD, 5) B200_DA(DD, 6) B200_DA(DD, 7)          \
+    B200_DA(DD, 8)                                                                                                   \
+    default:                                                                                                         \
+      return fail_arg("decode_attention: GQA group size %d not instantiated (1 to 8)", G);                          \
   }
+  if (head_dim == 64) {
+    B200_DA_G(64)
+  } else {
+    B200_DA_G(128)
+  }
+#undef B200_DA_G
 #undef B200_DA
   int rc = check_launch("decode_attention");
   if (rc || num_splits == 1) return rc;
-  const int rows = static_cast<int>(B * num_heads);
-  launch_pdl(decode_attention_merge_kernel, dim3((rows + 3) / 4), dim3(128), 0, stream, part, o, rows, (int)num_splits);
-  return check_launch("decode_attention(merge)");
+  return launch_decode_attention_merge(part, o, static_cast<int>(B * num_heads), static_cast<int>(num_splits), (int)head_dim, stream);
 }
 
 extern "C" int b200_get_padding_offset(const int64_t* input_ids, const int32_t* cum_offsets, const int32_t* seq_lens,
@@ -1468,7 +1491,7 @@ extern "C" int b200_save_output_stream(const int64_t* next_tokens, const int32_t
 //     idle slot               (seq_lens_this_time[b] == 0)
 //   1. append_rope_write_kernel  RoPE (rotate-half) on q, k of EVERY new row in place + k, v appended to the pages (one launch
 //                                for prompt and decode rows alike); decode rows' q are also gathered into a dense [B, ld] buffer
-//   2. fa_fwd_kernel<8, PAGED>   prompt rows: flash attention, q tiles of 128 rows, K/V rows gathered page by page with
+//   2. fa_fwd_kernel<d, 8, PAGED> prompt rows: flash attention, q tiles of 128 rows, K/V rows gathered page by page with
 //                                cp.async, causal band offset by the cached prefix (chunked prefill)
 //   3. decode_attention_tc<PAGED> decode rows (the decode step's kernel; sequences of the other kinds, idle slots included,
 //                                have length -1 = no work)
@@ -1581,7 +1604,7 @@ extern "C" int b200_append_attention(void* qkv, void* key_cache, void* value_cac
   B200_CHECK_ARG(qkv && key_cache && value_cache && seq_lens_encoder && seq_lens_decoder && seq_lens_this_time && cu_seqlens_q &&
                      block_tables && cos_table && sin_table && out && workspace,
                  "append_attention: null pointer");
-  B200_CHECK_ARG(head_dim == 128, "append_attention: head_dim must be 128 (got %lld)", (long long)head_dim);
+  B200_CHECK_ARG(head_dim == 64 || head_dim == 128, "append_attention: head_dim must be 64 or 128 (got %lld)", (long long)head_dim);
   B200_CHECK_ARG(block_size == 32 || block_size == 64 || block_size == 128, "append_attention: block_size must be 32, 64 or 128");
   B200_CHECK_ARG(B > 0 && token_num > 0 && max_q_len > 0 && num_heads % num_kv_heads == 0 && ldq % 8 == 0 && ldo % 8 == 0 &&
                      num_splits >= 1 && num_splits <= 64,
@@ -1606,7 +1629,7 @@ extern "C" int b200_append_attention(void* qkv, void* key_cache, void* value_cac
   int rc = check_launch("append_attention(rope + cache write)");
   if (rc) return rc;
   rc = launch_fa_prefill_paged(qkv, key_cache, value_cache, out, cu_seqlens_q, seq_lens_encoder, seq_lens_decoder,
-                               seq_lens_this_time, block_tables, B, token_num, max_q_len, num_heads, num_kv_heads, num_blocks,
+                               seq_lens_this_time, block_tables, B, token_num, max_q_len, num_heads, num_kv_heads, head_dim, num_blocks,
                                block_size, max_blocks_per_seq, ldq, ldo, softmax_scale, stream);
   if (rc) return rc;
   rc = b200_decode_attention_paged(q_dec, key_cache, value_cache, block_tables, dec_len, out_dec, num_splits > 1 ? dec_ws : nullptr, B,

@@ -51,8 +51,7 @@ class FusedMultiTransformerConfig:
             raise NotImplementedError("tensor-parallel generation is out of scope (config 5 is single-GPU)")
         if not self.trans_qkvw:
             raise NotImplementedError("trans_qkvw=False")
-        if self.embed_dim // self.num_heads != 128:
-            raise NotImplementedError("head_dim must be 128")
+        ops.check_head_dim(self.embed_dim // self.num_heads, "FusedMultiTransformerConfig")
 
 
 class FusedMultiTransformerBase:

@@ -18,6 +18,15 @@ BF16 = torch.bfloat16
 # (query heads per kv head) and accept at most this many split-KV partials per (sequence, head).
 DECODE_GQA_GROUPS = range(1, 9)
 DECODE_MAX_SPLITS = 64
+# Every attention kernel (training forward / backward, decode, append_attention) is compiled for these head dims.
+ATTENTION_HEAD_DIMS = (64, 128)
+
+
+def check_head_dim(head_dim: int, what: str) -> None:
+    """Raise NotImplementedError unless the attention kernels are compiled for `head_dim`."""
+    if head_dim not in ATTENTION_HEAD_DIMS:
+        raise NotImplementedError(f"{what}: head_dim {head_dim} is not supported; the attention kernels are written for head_dim "
+                                  f"{' and '.join(map(str, ATTENTION_HEAD_DIMS))}")
 
 
 def _chk(t: torch.Tensor, name: str, dtype=BF16):
@@ -348,9 +357,9 @@ def _mask_rows(mask_start, B, S):
 
 def flash_attn_fwd(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, softmax_scale: Optional[float] = None,
                    out: Optional[torch.Tensor] = None, mask_start: Optional[torch.Tensor] = None):
-    """Causal GQA attention.  q [B,S,nh,128], k/v [B,S,kvh,128] (may be strided views of a packed QKV buffer).
+    """Causal GQA attention.  q [B,S,nh,d], k/v [B,S,kvh,d], d = 64 or 128 (may be strided views of a packed QKV buffer).
     mask_start [B,S] int32 (optional): FlashMask start rows — row i sees column c iff c <= i < mask_start[b, c].
-    Returns (o [B,S,nh,128] contiguous, lse [B,nh,S] fp32)."""
+    Returns (o [B,S,nh,d] contiguous, lse [B,nh,S] fp32)."""
     _chk(q, "q"); _chk(k, "k"); _chk(v, "v")
     B, S, nh, d = q.shape
     kvh = k.shape[2]
@@ -366,7 +375,7 @@ def flash_attn_fwd(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, softmax_sc
 
 
 def flash_attn_bwd(q, k, v, o, dout, lse, dq, dk, dv, softmax_scale: Optional[float] = None, mask_start=None):
-    """Gradients written into dq/dk/dv (views allowed, e.g. slices of a packed dQKV buffer)."""
+    """Gradients written into dq/dk/dv (views allowed, e.g. slices of a packed dQKV buffer); head_dim 64 or 128."""
     for name, t in (("q", q), ("k", k), ("v", v), ("o", o), ("dout", dout), ("dq", dq), ("dk", dk), ("dv", dv)):
         _chk(t, name)
     _chk(lse, "lse", torch.float32)
@@ -507,7 +516,7 @@ def _decode_splits(B: int, kvh: int, max_len: int) -> int:
 def decode_attention(qkv, cache, seq_lens, nh, kvh, d, softmax_scale=None, out=None, num_splits: int = 0, impl: str = "tc"):
     """Attention of one query row per sequence over the dense cache [2, B, kvh, max_len, d]: sequence b attends to its first
     min(seq_lens[b] + 1, max_len) rows (the new token was appended at row seq_lens[b]).  GQA group nh / kvh in 1..8,
-    d = 128.  impl "tc": the bulk-copy kernel (decode_attn_tc.cu); "simt": the CUDA-core kernel of generation.cu with plain
+    d = 64 or 128.  impl "tc": the bulk-copy kernel (decode_attn_tc.cu); "simt": the CUDA-core kernel of generation.cu with plain
     global loads, the cross-check.  num_splits <= 0 lets each pick its split-KV count (at most 64)."""
     _chk(qkv, "qkv"); _chk(cache, "cache"); _chk(seq_lens, "seq_lens", torch.int32)
     B = qkv.shape[0]
@@ -566,7 +575,8 @@ def decode_rope_append_paged(qkv, key_cache, value_cache, block_tables, cos, sin
 def decode_attention_paged(qkv, key_cache, value_cache, block_tables, seq_lens, nh, softmax_scale=None, out=None,
                            num_splits: int = 0):
     """decode_attention over the paged cache: sequence b's row t lives in page block_tables[b, t // block_size] (entries
-    past a sequence's pages may be -1); it attends to min(seq_lens[b] + 1, max_blocks_per_seq * block_size) rows."""
+    past a sequence's pages may be -1); it attends to min(seq_lens[b] + 1, max_blocks_per_seq * block_size) rows.
+    d = 64 or 128, block_size 32, 64 or 128."""
     _chk(qkv, "qkv"); _chk(seq_lens, "seq_lens", torch.int32)
     nb, kvh, bs, d, mb = _paged_geom(key_cache, value_cache, block_tables)
     B = qkv.shape[0]

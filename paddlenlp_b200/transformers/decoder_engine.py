@@ -56,8 +56,7 @@ class DecoderEngine:
         self.eps = config.rms_norm_eps
         self.qkv_bias = config.model_type == "qwen2"
         self.tied = bool(getattr(config, "tie_word_embeddings", False))
-        if self.d != 128:
-            raise NotImplementedError(f"head_dim {self.d}: the attention kernels are written for head_dim 128")
+        ops.check_head_dim(self.d, "DecoderEngine")
         if self.h % 8 or self.I % 8 or self.V % 8:
             raise ValueError("hidden_size, intermediate_size and vocab_size must be multiples of 8")
         self.qkv_n = (self.nh + 2 * self.kvh) * self.d

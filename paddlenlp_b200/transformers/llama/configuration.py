@@ -65,6 +65,17 @@ class LlamaConfig(PretrainedConfig):
         return cls(**base)
 
     @classmethod
+    def llama3_2_1b(cls, **kw):
+        """Llama-3.2-1B shapes (head_dim 64, GQA 32/8).  Tied input and output embeddings by default, the released layout (no
+        benchmark uses this preset); pass `tie_word_embeddings=False` for a separate lm_head."""
+        base = dict(vocab_size=128256, hidden_size=2048, intermediate_size=8192, num_hidden_layers=16,
+                    num_attention_heads=32, num_key_value_heads=8, rms_norm_eps=1e-5, rope_theta=500000.0,
+                    max_position_embeddings=8192, seq_length=4096, bos_token_id=128000, eos_token_id=128001,
+                    tie_word_embeddings=True)
+        base.update(kw)
+        return cls(**base)
+
+    @classmethod
     def llama3_8b(cls, **kw):
         base = dict(vocab_size=128256, hidden_size=4096, intermediate_size=14336, num_hidden_layers=32,
                     num_attention_heads=32, num_key_value_heads=8, rms_norm_eps=1e-5, rope_theta=500000.0,

@@ -153,8 +153,7 @@ def fusion_flash_attention(query_states, config, key_states, value_states, atten
         raise NotImplementedError("sep-parallel resharding is outside the data-parallel hot path")
     if output_attentions:
         raise ValueError("flash attention does not return attention weights (fusion_ops.py:209-212)")
-    if head_dim != 128:
-        raise ValueError(f"head_dim {head_dim} unsupported (128 only)")
+    ops.check_head_dim(head_dim, "fusion_flash_attention")
     mask_rows = None
     if attn_mask_startend_row_indices is not None:
         # fusion_ops.py:218-231: F.flashmask_attention(..., startend_row_indices=idx.unsqueeze(-1), causal=True); idx is

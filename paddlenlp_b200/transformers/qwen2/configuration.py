@@ -44,6 +44,16 @@ class Qwen2Config(PretrainedConfig):
         return cls(**base)
 
     @classmethod
+    def qwen2_0_5b(cls, **kw):
+        """Qwen2-0.5B / Qwen2.5-0.5B shapes (head_dim 64, GQA 14/2).  Tied input and output embeddings by default, the released
+        layout (no benchmark uses this preset); pass `tie_word_embeddings=False` for a separate lm_head."""
+        base = dict(vocab_size=151936, hidden_size=896, intermediate_size=4864, num_hidden_layers=24,
+                    num_attention_heads=14, num_key_value_heads=2, rms_norm_eps=1e-6, rope_theta=1000000.0,
+                    max_position_embeddings=32768, seq_length=2048, tie_word_embeddings=True)
+        base.update(kw)
+        return cls(**base)
+
+    @classmethod
     def qwen2_7b(cls, **kw):
         base = dict(vocab_size=152064, hidden_size=3584, intermediate_size=18944, num_hidden_layers=28,
                     num_attention_heads=28, num_key_value_heads=4, rms_norm_eps=1e-6, rope_theta=1000000.0,

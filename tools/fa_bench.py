@@ -1,8 +1,10 @@
 """Time the flash-attention forward and both backward kernels (b200_set_fa_bwd_impl 2 = wgmma, 1 = mma.sync) on an H100.
 
-Shapes: the two benchmarked models, Llama-3.2-3B (1 x 4096, 24 / 8 heads) and the Qwen2-1.5B SFT micro-batch (4 x 2048,
-12 / 2 heads), then the Llama-3-8B and Qwen2-7B layouts.  The two backward kernels are timed alternately in one process
-(REPEATS rounds each), so clock and neighbour drift hit both alike; each line gives the median and the spread (min, max).
+Shapes (B, S, q heads, kv heads, head_dim): the two benchmarked models, Llama-3.2-3B (1 x 4096, 24 / 8 heads) and the
+Qwen2-1.5B SFT micro-batch (4 x 2048, 12 / 2 heads), then the Llama-3-8B and Qwen2-7B layouts, all at head_dim 128; then the
+head_dim 64 models: Llama-3.2-1B (1 x 4096, 32 / 8), a Qwen2-0.5B SFT micro-batch (4 x 2048, 14 / 2) and TinyLlama
+(1 x 2048, 32 / 4).  The forward and the two backward kernels are timed alternately in one process (REPEATS rounds each), so
+clock and neighbour drift hit all alike; each line gives the median and the spread (min, max).
 """
 import json
 import os
@@ -17,7 +19,8 @@ sys.path.insert(0, ROOT)
 from paddlenlp_b200 import _lib, ops  # noqa: E402
 
 REPEATS = 5
-SHAPES = [(1, 4096, 24, 8), (4, 2048, 12, 2), (1, 4096, 32, 8), (2, 4096, 32, 8), (1, 2048, 28, 4)]
+SHAPES = [(1, 4096, 24, 8, 128), (4, 2048, 12, 2, 128), (1, 4096, 32, 8, 128), (2, 4096, 32, 8, 128), (1, 2048, 28, 4, 128),
+          (1, 4096, 32, 8, 64), (4, 2048, 14, 2, 64), (1, 2048, 32, 4, 64)]
 
 
 def timeit(fn, iters=10, warm=3):
@@ -48,8 +51,7 @@ def main():
     lib = _lib.load()
     print(json.dumps(dict(gpu=gpu_info())), flush=True)
     old_impl = lib.b200_set_fa_bwd_impl(2)
-    for (B, S, nh, kvh) in SHAPES:
-        d = 128
+    for (B, S, nh, kvh, d) in SHAPES:
         ld = (nh + 2 * kvh) * d
         qkv = torch.randn(B, S, ld, device=dev).to(torch.bfloat16)
         q = qkv[:, :, : nh * d].view(B, S, nh, d)
@@ -61,16 +63,18 @@ def main():
         dq = dqkv[:, :, : nh * d].view(B, S, nh, d)
         dk = dqkv[:, :, nh * d: (nh + kvh) * d].view(B, S, kvh, d)
         dv = dqkv[:, :, (nh + kvh) * d:].view(B, S, kvh, d)
-        t_f = timeit(lambda: ops.flash_attn_fwd(q, k, v, out=out))
+        t_f = []
         t_b = {1: [], 2: []}
         for _ in range(REPEATS):
+            t_f.append(timeit(lambda: ops.flash_attn_fwd(q, k, v, out=out)))
             for impl in (2, 1):
                 lib.b200_set_fa_bwd_impl(impl)
                 t_b[impl].append(timeit(lambda: ops.flash_attn_bwd(q, k, v, out, dout, lse, dq, dk, dv)))
         lib.b200_set_fa_bwd_impl(2)
         fl_f = 4.0 * B * nh * S * S * d / 2        # causal
         fl_b = 2.5 * fl_f
-        rec = dict(shape=[B, S, nh, kvh], fwd_ms=t_f, fwd_tflops=fl_f / t_f / 1e9)
+        sm = summary(t_f)
+        rec = dict(shape=[B, S, nh, kvh], head_dim=d, fwd=dict(sm, tflops=fl_f / sm["median_ms"] / 1e9))
         for impl in (2, 1):
             sm = summary(t_b[impl])
             rec[f"bwd_impl{impl}"] = dict(sm, tflops=fl_b / sm["median_ms"] / 1e9)

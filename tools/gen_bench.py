@@ -1,4 +1,5 @@
 """Config 5: Llama-3-8B generation decode, 1xH100, batch 64, prompt 128 -> gen 1920 (FusedMultiTransformer KV-cache path).
+`--preset llama3_2_1b` / `qwen2_0_5b` runs the same workload on the head_dim 64 models (tied embeddings, as released).
 
 Reports prefill time, decode tokens/s = B * (gen - 1) / decode time, and the HBM roofline of the decode step
 (weights 15.01 GB + KV read 8.39 MB * t per step; SURVEY.md §8d)."""
@@ -16,16 +17,21 @@ import paddlenlp_b200.transformers as T  # noqa: E402
 from paddlenlp_b200.experimental.transformers import LlamaForCausalLMInferenceModel  # noqa: E402
 
 
-def run(batch=64, prompt=128, gen=1920, layers=0, graph=True, pdl=True, block_attn=False):
+PRESETS = {"llama3_8b": T.LlamaConfig.llama3_8b, "llama3_2_1b": T.LlamaConfig.llama3_2_1b, "qwen2_0_5b": T.Qwen2Config.qwen2_0_5b}
+
+
+def run(batch=64, prompt=128, gen=1920, layers=0, graph=True, pdl=True, block_attn=False, preset="llama3_8b"):
     class A:
         pass
     a = A()
     a.batch, a.prompt, a.gen, a.layers, a.no_graph, a.no_pdl, a.block_attn = batch, prompt, gen, layers, not graph, not pdl, block_attn
+    a.preset = preset
     return _run(a)
 
 
 def _run(a):
-    cfg = T.LlamaConfig.llama3_8b(num_hidden_layers=a.layers) if a.layers else T.LlamaConfig.llama3_8b()
+    make = PRESETS[a.preset]
+    cfg = make(num_hidden_layers=a.layers) if a.layers else make()
     m = LlamaForCausalLMInferenceModel(cfg, block_attn=a.block_attn)
     m.init_random(seed=42)
     g = torch.Generator().manual_seed(1234)
@@ -53,7 +59,7 @@ def _run(a):
     steps = a.gen - 1
     L = cfg.num_hidden_layers
     h, I, V = cfg.hidden_size, cfg.intermediate_size, cfg.vocab_size
-    kvd = cfg.num_key_value_heads * 128
+    kvd = cfg.num_key_value_heads * (h // cfg.num_attention_heads)
     w_bytes = L * (h * (h + 2 * kvd) + h * h + 3 * h * I) * 2 + V * h * 2
     kv_per_tok = 2 * L * a.batch * kvd * 2
     mean_t = a.prompt + steps / 2.0
@@ -63,7 +69,8 @@ def _run(a):
     ms_step = decode_ms / steps
     achieved = bytes_per_step / (ms_step / 1e3) / 1e9
     rec = dict(workload="Llama-3-8B generation decode, batch 64, prompt 128 -> +1920, FusedMultiTransformer KV-cache path "
-                        "(BASELINE.json configs[4])" if (a.batch, a.prompt, a.gen, a.layers) == (64, 128, 1920, 0) else "custom",
+                        "(BASELINE.json configs[4])" if (a.batch, a.prompt, a.gen, a.layers, a.preset) == (64, 128, 1920, 0, "llama3_8b")
+               else f"{a.preset} decode, batch {a.batch}, prompt {a.prompt} -> +{a.gen}",
                batch=a.batch, prompt=a.prompt, gen=a.gen, layers=L, paged_kv=bool(a.block_attn), prefill_ms=prefill_ms, decode_ms=decode_ms,
                ms_per_step=ms_step,
                decode_tokens_per_s=a.batch * steps / (decode_ms / 1e3), bytes_per_step_gb=bytes_per_step / 1e9,
@@ -81,6 +88,7 @@ def main():
     ap.add_argument("--layers", type=int, default=0)
     ap.add_argument("--no-graph", action="store_true")
     ap.add_argument("--no-pdl", action="store_true")
+    ap.add_argument("--preset", choices=sorted(PRESETS), default="llama3_8b")
     ap.add_argument("--block-attn", action="store_true", help="paged KV cache (FusedBlockMultiTransformer, 64-row blocks)")
     a = ap.parse_args()
     print(json.dumps(_run(a)), flush=True)
