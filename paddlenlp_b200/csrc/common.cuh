@@ -121,6 +121,18 @@ __device__ __forceinline__ void tma_reduce_add_4d(const CUtensorMap* tm, const v
                "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
                : "memory");
 }
+// shared -> global, 2D tile (bulk-group completion); elements outside the tensor are not written.
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* tm, uint32_t smem_src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(reinterpret_cast<uint64_t>(tm)),
+               "r"(smem_src), "r"(c0), "r"(c1)
+               : "memory");
+}
+// Pull a 2D tile of a tensor map into L2 (no shared memory, no completion to wait for).
+__device__ __forceinline__ void tma_prefetch_l2_2d(const CUtensorMap* tm, int c0, int c1) {
+  asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];" ::"l"(reinterpret_cast<uint64_t>(tm)), "r"(c0),
+               "r"(c1)
+               : "memory");
+}
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void tma_store_wait_read() {
@@ -256,6 +268,11 @@ __device__ __forceinline__ uint4 ld_nc_v4(const void* p) {
 __device__ __forceinline__ void st_na_v4(void* p, const uint4& v) {
   asm volatile("st.global.L1::no_allocate.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z),
                "r"(v.w));
+}
+// Ordered against other asm volatile statements (e.g. fence.proxy.async), but no "memory" clobber: global loads of the same
+// loop may still be scheduled ahead of it.
+__device__ __forceinline__ void st_shared_u32(uint32_t saddr, uint32_t v) {
+  asm volatile("st.shared.u32 [%0], %1;" ::"r"(saddr), "r"(v));
 }
 __device__ __forceinline__ uint4 ld_shared_v4(uint32_t saddr) {
   uint4 r;

@@ -12,7 +12,9 @@
 //   warpgroups 1,2  MMA + epilogue : each owns 64 rows of the tile: wgmma m64n256k16 x 4 per k-block, fp32 accumulators in
 //                                    128 registers per thread; a k-block's stage is released once the next block's wgmmas
 //                                    are in flight; the epilogue (+bias, +C_old | +residual, SwiGLU forms, split-K
-//                                    reduction) works on the accumulator registers and stores straight to global memory
+//                                    reduction) works on the accumulator registers; with 128-row tiles it stages bf16
+//                                    64 x 64 boxes in shared memory and stores them with TMA (C_old / residual / gate|up
+//                                    prefetched into L2 during the tile's last k-blocks), else it stores to global memory
 //   Operand majors: both K-major (contraction dim contiguous) and MN-major operands are fed straight from their
 //   row-major global layout through TMA (wgmma reads either major for 16-bit types); no transposes are materialised.
 #include "../../include/b200nlp.h"
@@ -28,6 +30,8 @@ namespace gemm {
 constexpr int BN = 256;   // tile columns (wgmma N)
 constexpr int BK = 64;    // K per pipeline stage (= one 128-byte swizzle row of bf16)
 constexpr int B_BYTES = BN * BK * 2;              // 32 KB
+constexpr int EPI_BOX = 64;                       // epilogue TMA box: 64 rows x 64 columns (one 128-byte swizzle row wide)
+constexpr int EPI_BOX_BYTES = EPI_BOX * EPI_BOX * 2;   // 8 KB
 
 // NWG consumer warpgroups of 64 rows each.  NWG = 2 (128-row tiles) for the training shapes; NWG = 1 (64-row tiles) for the
 // decode step's M <= 64 token rows, where the kernel is a weight stream: 8 KB of activations and 32 KB of weights per stage,
@@ -39,7 +43,9 @@ struct Tile {
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int STAGES = NWG == 2 ? 4 : 5;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 256 + 1024;   // ring + barriers + alignment slack (<= 227 KB)
+  // NWG = 2: two 64 x 64 bf16 output boxes per consumer warpgroup for the shared-memory epilogue
+  static constexpr int EPI_BYTES = NWG == 2 ? NWG * 2 * EPI_BOX_BYTES : 0;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BYTES + 256 + 1024;   // + barriers + alignment slack (<= 227 KB)
 };
 static int tile_wgs(int64_t M) { return M <= 64 ? 1 : 2; }
 
@@ -64,6 +70,8 @@ struct Params {
   bf16* aux;               // mode 4: gate|up output (nullable); mode 5: saved gate|up input
   int64_t ld_aux;
   float* ws;               // mode 3: fp32 [M, N] accumulation buffer
+  int smem_epi;            // NWG = 2, modes 0, 1, 2, 4, 5 with 16-byte aligned outputs: the epilogue stores through shared
+                           // memory and TMA (tmC, tmX); otherwise it stores from the registers
 };
 
 __device__ __forceinline__ void tile_coords(int t, int num_m, int num_n, int& m_blk, int& n_blk, int GM) {
@@ -91,14 +99,64 @@ __device__ __forceinline__ void store_bf16x2(bf16* base, int64_t ld, int row, in
   else if (col < N) *dst = __float2bfloat16_rn(v0);
 }
 
+// ---- shared-memory epilogue (NWG = 2) ----
+// A consumer warpgroup's 64 x 256 accumulator tile leaves as 64 x 64 bf16 boxes.  The warpgroup writes a box into one of its
+// two 8 KB buffers in the 128B-swizzled TMA layout, one thread stores it with cp.async.bulk.tensor, and the warpgroup goes on
+// to the next box, or to the next tile's wgmmas, while the store drains.  TMA drops rows >= M and columns past the tensor
+// map's width.  The global loads of a box's inputs (C_old, residual, saved gate|up) are all issued before its first use:
+// no store to global memory sits between them any more.
+//
+// Address of this thread's bf16 pair in row r, columns 8 jj + 2 (lane % 4) + {0, 1}, of a box buffer: 16-byte chunk jj of row r
+// sits at chunk jj ^ (r % 8).  A warp's 8 rows then hit 8 different chunks: the stores are free of bank conflicts.
+__device__ __forceinline__ uint32_t epi_slot(uint32_t buf, int r, int jj, int lane) {
+  return buf + r * 128 + ((jj ^ (r & 7)) << 4) + 4 * (lane & 3);
+}
+// Before a warpgroup writes box buffers: at most KEEP earlier stores (the ones reading the other buffer) may still be reading
+// shared memory.
+template <int KEEP>
+__device__ __forceinline__ void epi_begin(int cw, bool leader) {
+  if (leader) tma_store_wait_read<KEEP>();
+  named_bar_sync(1 + cw, 128);
+}
+// After: the writes are visible to the TMA unit, and the leader may store the boxes.
+__device__ __forceinline__ void epi_end(int cw) {
+  fence_proxy_async_smem();
+  named_bar_sync(1 + cw, 128);
+}
+// The bf16 pair at (row, col), col even; 0 outside the matrix (those outputs are not stored).
+__device__ __forceinline__ uint32_t ld_pair(const bf16* base, int64_t ld, int row, int col, int M, int N) {
+  if (row >= M || col >= N) return 0u;
+  const bf16* src = base + static_cast<int64_t>(row) * ld + col;
+  if (col + 1 < N) return *reinterpret_cast<const uint32_t*>(src);
+  return static_cast<uint32_t>(__bfloat16_as_ushort(*src));
+}
+// Pull the epilogue inputs of a warpgroup's 64 rows into L2 while the tile's last k-blocks run, so the loads above hit L2.
+__device__ __forceinline__ void epi_prefetch(const CUtensorMap* tmC, const CUtensorMap* tmX, const Params& p, int n_blk, int row0) {
+  for (int s = 0; s < BN / EPI_BOX; ++s) {
+    const int col0 = n_blk * BN + EPI_BOX * s;
+    if (col0 >= p.N) break;
+    if (p.epi_mode == 1) {
+      tma_prefetch_l2_2d(tmC, col0, row0);
+    } else if (p.epi_mode == 2) {
+      tma_prefetch_l2_2d(tmX, col0, row0);
+    } else {
+      tma_prefetch_l2_2d(tmX, col0, row0);
+      tma_prefetch_l2_2d(tmX, p.swiglu_inter + col0, row0);
+    }
+  }
+}
+
+// tmC / tmX: the epilogue's tensor maps when p.smem_epi is set (box {64, 64}).  tmC is the output (mode 4: m); tmX is the
+// residual (mode 2, read through L2 prefetches only), gate|up (mode 4 output, mode 5 input).
 template <int NWG, bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(Tile<NWG>::NUM_THREADS, 1)
-gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const Params p) {
+gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                 const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmX, const Params p) {
   using T = Tile<NWG>;
   constexpr int BM = T::BM, A_BYTES = T::A_BYTES, STAGE_BYTES = T::STAGE_BYTES, STAGES = T::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);   // [STAGES]
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + T::EPI_BYTES);   // [STAGES]
   uint64_t* empty_bar = full_bar + STAGES;                                           // [STAGES]
 
   const int num_items = p.num_m_tiles * p.num_n_tiles * p.split_k;
@@ -163,6 +221,10 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   // descriptor byte offsets of k-step kk (16 k) inside a stage
   constexpr uint32_t A_KSTEP = A_MN ? 2048u : 32u, B_KSTEP = B_MN ? 2048u : 32u;
   const uint32_t a_off = static_cast<uint32_t>(cw) * (64 * BK * 2);
+  const bool leader = (threadIdx.x & 127) == 0;           // issues the warpgroup's epilogue stores and prefetches
+  const bool prefetch = p.smem_epi && leader && (p.epi_mode == 1 || p.epi_mode == 2 || p.epi_mode == 5);
+  const uint32_t ebuf = smem_u32(smem + STAGES * STAGE_BYTES) + cw * 2 * EPI_BOX_BYTES;   // this warpgroup's two boxes
+  uint32_t nbox = 0;                                       // boxes stored so far (modes 0-2 alternate the two buffers)
   uint32_t it = 0;
   float acc[128];
   for (int t = blockIdx.x; t < num_items; t += gridDim.x) {
@@ -170,6 +232,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     tile_coords(t / p.split_k, p.num_m_tiles, p.num_n_tiles, m_blk, n_blk, p.gm);
     const int kb0 = (t % p.split_k) * p.kb_per_split;
     const int nkb = min(num_kb_total, kb0 + p.kb_per_split) - kb0;
+    const int prefetch_kb = nkb > 8 ? nkb - 8 : 0;
     fence_acc(acc);                                        // the previous tile's epilogue reads precede the zeroing
 #pragma unroll
     for (int i = 0; i < 128; ++i) acc[i] = 0.f;
@@ -186,6 +249,9 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         wgmma_m64n256k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, dA + ((kk * A_KSTEP) >> 4), dB + ((kk * B_KSTEP) >> 4),
                                                      (i > 0 || kk > 0) ? 1u : 0u);
       wgmma_commit();
+      if constexpr (NWG == 2) {
+        if (prefetch && i == prefetch_kb) epi_prefetch(&tmC, &tmX, p, n_blk, m_blk * BM + cw * 64);
+      }
       wgmma_wait<1>();                                     // k-block i-1 is finished: its stage can be refilled
       if (i > 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
     }
@@ -196,6 +262,128 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     // accumulator fragment: register 4j + 2i + e holds row 16 wi + lane/4 + 8i, column 8j + 2 (lane % 4) + e
     const int row_base = m_blk * BM + cw * 64 + wi * 16 + (lane >> 2);
     const int cq = 2 * (lane & 3);
+    if constexpr (NWG == 2) {
+      if (p.smem_epi) {
+        // Same fp32 operations in the same order, and the same bf16 roundings, as the register epilogue below.
+        const int row0 = m_blk * BM + cw * 64;             // first row of the warpgroup's boxes
+        const int r_lo = wi * 16 + (lane >> 2);            // this thread's rows in a box: r_lo + 8 i
+        if (p.epi_mode == 4) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {                    // 64 channels per box
+            const int ch0 = n_blk * 128 + EPI_BOX * h;
+            if (ch0 >= p.swiglu_inter) continue;
+            if (p.aux != nullptr) {                        // gate and up, as the unfused GEMM rounds them
+              epi_begin<0>(cw, leader);
+#pragma unroll
+              for (int i = 0; i < 2; ++i)
+#pragma unroll
+                for (int jj = 0; jj < 8; ++jj) {
+                  const int j = 8 * h + jj;
+                  st_shared_u32(epi_slot(ebuf, r_lo + 8 * i, jj, lane), pack_bf16x2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]));
+                  st_shared_u32(epi_slot(ebuf + EPI_BOX_BYTES, r_lo + 8 * i, jj, lane),
+                                pack_bf16x2(acc[4 * (j + 16) + 2 * i], acc[4 * (j + 16) + 2 * i + 1]));
+                }
+              epi_end(cw);
+              if (leader) {
+                tma_store_2d(&tmX, ebuf, ch0, row0);
+                tma_store_2d(&tmX, ebuf + EPI_BOX_BYTES, p.swiglu_inter + ch0, row0);
+                tma_store_commit();
+              }
+            }
+            epi_begin<0>(cw, leader);
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+#pragma unroll
+              for (int jj = 0; jj < 8; ++jj) {
+                const int j = 8 * h + jj;
+                const uint32_t gp = pack_bf16x2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
+                const uint32_t up = pack_bf16x2(acc[4 * (j + 16) + 2 * i], acc[4 * (j + 16) + 2 * i + 1]);
+                st_shared_u32(epi_slot(ebuf, r_lo + 8 * i, jj, lane), swiglu_fwd_pair(gp, up));
+              }
+            epi_end(cw);
+            if (leader) {
+              tma_store_2d(&tmC, ebuf, ch0, row0);
+              tma_store_commit();
+            }
+          }
+          continue;
+        }
+        if (p.epi_mode == 5) {                             // d(gate) box | d(up) box per 64 channels
+#pragma unroll
+          for (int s = 0; s < BN / EPI_BOX; ++s) {
+            const int ch0 = n_blk * BN + EPI_BOX * s;
+            if (ch0 >= p.N) continue;
+            epi_begin<0>(cw, leader);
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {                  // 8 input registers at a time next to the 128 accumulators
+              const int i = q >> 1, jj0 = 4 * (q & 1);
+              uint32_t g[4], u[4];
+#pragma unroll
+              for (int k = 0; k < 4; ++k) {
+                const int row = row0 + r_lo + 8 * i, ch = ch0 + 8 * (jj0 + k) + cq;
+                g[k] = ld_pair(p.aux, p.ld_aux, row, ch, p.M, p.N);
+                u[k] = ld_pair(p.aux + p.swiglu_inter, p.ld_aux, row, ch, p.M, p.N);
+              }
+#pragma unroll
+              for (int k = 0; k < 4; ++k) {
+                const int jj = jj0 + k, j = 8 * s + jj;
+                uint32_t dg2, du2;                         // d(m) with the GEMM's own bf16 output rounding
+                swiglu_bwd_pair(g[k], u[k], bf16_round(acc[4 * j + 2 * i]), bf16_round(acc[4 * j + 2 * i + 1]), dg2, du2);
+                st_shared_u32(epi_slot(ebuf, r_lo + 8 * i, jj, lane), dg2);
+                st_shared_u32(epi_slot(ebuf + EPI_BOX_BYTES, r_lo + 8 * i, jj, lane), du2);
+              }
+            }
+            epi_end(cw);
+            if (leader) {
+              tma_store_2d(&tmC, ebuf, ch0, row0);
+              tma_store_2d(&tmC, ebuf + EPI_BOX_BYTES, p.swiglu_inter + ch0, row0);
+              tma_store_commit();
+            }
+          }
+          continue;
+        }
+        // modes 0, 1, 2
+#pragma unroll
+        for (int s = 0; s < BN / EPI_BOX; ++s) {
+          const int col0 = n_blk * BN + EPI_BOX * s;
+          if (col0 >= p.N) continue;
+          const uint32_t buf = ebuf + (nbox++ & 1u) * EPI_BOX_BYTES;
+          epi_begin<1>(cw, leader);
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            uint32_t o[8];                                 // C_old (mode 1) or residual (mode 2) pairs of row r_lo + 8 i
+            if (p.epi_mode != 0) {
+              const bf16* src = p.epi_mode == 1 ? p.c : p.r;
+              const int64_t ld = p.epi_mode == 1 ? p.ldc : p.ldr;
+#pragma unroll
+              for (int jj = 0; jj < 8; ++jj) o[jj] = ld_pair(src, ld, row0 + r_lo + 8 * i, col0 + 8 * jj + cq, p.M, p.N);
+            }
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+              const int j = 8 * s + jj, col = col0 + 8 * jj + cq;
+              float f0 = acc[4 * j + 2 * i], f1 = acc[4 * j + 2 * i + 1];
+              if (p.bias != nullptr) {
+                if (col < p.N) f0 += __ldg(p.bias + col);
+                if (col + 1 < p.N) f1 += __ldg(p.bias + col + 1);
+              }
+              if (p.epi_mode != 0) {
+                if (p.epi_mode == 2) { f0 = bf16_round(f0); f1 = bf16_round(f1); }
+                const float2 of = unpack_bf16x2(o[jj]);
+                f0 += of.x;
+                f1 += of.y;
+              }
+              st_shared_u32(epi_slot(buf, r_lo + 8 * i, jj, lane), pack_bf16x2(f0, f1));
+            }
+          }
+          epi_end(cw);
+          if (leader) {
+            tma_store_2d(&tmC, buf, col0, row0);
+            tma_store_commit();
+          }
+        }
+        continue;
+      }
+    }
     if (p.epi_mode == 4) {
       // gate|up + SwiGLU (llama/modeling.py:38-45, 632-652): accumulator columns [0,128) = gate, [128,256) = up of channels
       // [128 n_blk, +128).  Rounding points of the unfused path: gate and up each rounded to bf16 (the Linear outputs, kept for
@@ -271,10 +459,14 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       }
     }
   }
+  if constexpr (NWG == 2) {
+    if (leader) tma_store_wait<0>();                       // the box buffers stay allocated until the last store is done
+  }
 }
 
 template <int NWG, bool A_MN, bool B_MN>
-static int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const Params& p, int max_ctas, cudaStream_t stream) {
+static int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const CUtensorMap& tmX, const Params& p,
+                  int max_ctas, cudaStream_t stream) {
   using T = Tile<NWG>;
   constexpr int SMEM_BYTES = T::SMEM_BYTES;
   auto kern = gemm_bf16_kernel<NWG, A_MN, B_MN>;
@@ -296,7 +488,7 @@ static int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const Params& 
   // out of L2 by every wave while the B panels stream through once per group.  16 m-tiles of 128 rows keep the group's A
   // panels within ~18 MB of the 50 MB L2 for K <= 4608; longer K takes 8.
   pp.gm = (16ll * 128 * p.K * 2 <= (18ll << 20)) ? 16 : 8;
-  cudaError_t e = launch_pdl(kern, dim3(ctas), dim3(T::NUM_THREADS), SMEM_BYTES, stream, tmA, tmB, pp);
+  cudaError_t e = launch_pdl(kern, dim3(ctas), dim3(T::NUM_THREADS), SMEM_BYTES, stream, tmA, tmB, tmC, tmX, pp);
   if (e != cudaSuccess) {
     set_last_error("gemm launch: %s", cudaGetErrorString(e));
     return static_cast<int>(e);
@@ -304,18 +496,61 @@ static int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const Params& 
   return 0;
 }
 
-static int dispatch(bool a_mn, bool b_mn, const CUtensorMap& tmA, const CUtensorMap& tmB, const Params& p, int max_ctas,
-                    cudaStream_t stream) {
-  if (tile_wgs(p.M) == 1) {
-    if (a_mn && b_mn) return launch<1, true, true>(tmA, tmB, p, max_ctas, stream);
-    if (a_mn) return launch<1, true, false>(tmA, tmB, p, max_ctas, stream);
-    if (b_mn) return launch<1, false, true>(tmA, tmB, p, max_ctas, stream);
-    return launch<1, false, false>(tmA, tmB, p, max_ctas, stream);
+// Epilogue box map: a [rows, cols] bf16 matrix with leading dimension ld, box {64 columns, 64 rows}.
+static int make_epi_map(CUtensorMap* tm, const void* base, int64_t rows, int64_t cols, int64_t ld) {
+  const uint64_t dims[2] = {static_cast<uint64_t>(cols), static_cast<uint64_t>(rows)}, strides[1] = {static_cast<uint64_t>(ld) * 2};
+  const uint32_t box[2] = {EPI_BOX, EPI_BOX};
+  return encode_tmap_bf16(tm, base, 2, dims, strides, box);
+}
+static bool aligned16(const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; }
+
+// Selects the shared-memory epilogue for 128-row tiles outside split-K and builds its tensor maps.  TMA needs 16-byte aligned
+// base addresses (the strides are multiples of 8 elements already); an operand that is not (e.g. an `out=` view starting at
+// an odd column) keeps the register epilogue.
+static int setup_smem_epilogue(Params& p, CUtensorMap* tmC, CUtensorMap* tmX) {
+  p.smem_epi = 0;
+  if (tile_wgs(p.M) != 2 || p.epi_mode == 3 || !aligned16(p.c)) return 0;
+  int rc = 0;
+  switch (p.epi_mode) {
+    case 2:
+      if (!aligned16(p.r)) return 0;
+      if ((rc = make_epi_map(tmX, p.r, p.M, p.N, p.ldr)) != 0) return rc;
+      rc = make_epi_map(tmC, p.c, p.M, p.N, p.ldc);
+      break;
+    case 4:   // p.N = 2 I: tmC is m [M, I], tmX the gate|up output [M, 2I]
+      if (p.aux != nullptr && !aligned16(p.aux)) return 0;
+      if (p.aux != nullptr && (rc = make_epi_map(tmX, p.aux, p.M, p.N, p.ld_aux)) != 0) return rc;
+      rc = make_epi_map(tmC, p.c, p.M, p.swiglu_inter, p.ldc);
+      break;
+    case 5:   // p.N = I: tmC is d(gate)|d(up) [M, 2I], tmX the saved gate|up [M, 2I]
+      if (!aligned16(p.aux)) return 0;
+      if ((rc = make_epi_map(tmX, p.aux, p.M, 2ll * p.N, p.ld_aux)) != 0) return rc;
+      rc = make_epi_map(tmC, p.c, p.M, 2ll * p.N, p.ldc);
+      break;
+    default:  // 0, 1
+      rc = make_epi_map(tmC, p.c, p.M, p.N, p.ldc);
   }
-  if (a_mn && b_mn) return launch<2, true, true>(tmA, tmB, p, max_ctas, stream);
-  if (a_mn) return launch<2, true, false>(tmA, tmB, p, max_ctas, stream);
-  if (b_mn) return launch<2, false, true>(tmA, tmB, p, max_ctas, stream);
-  return launch<2, false, false>(tmA, tmB, p, max_ctas, stream);
+  if (rc == 0) p.smem_epi = 1;
+  return rc;
+}
+
+static int dispatch(bool a_mn, bool b_mn, const CUtensorMap& tmA, const CUtensorMap& tmB, Params p, int max_ctas,
+                    cudaStream_t stream) {
+  CUtensorMap tmC, tmX;
+  memset(&tmC, 0, sizeof(tmC));
+  memset(&tmX, 0, sizeof(tmX));
+  int rc;
+  if ((rc = setup_smem_epilogue(p, &tmC, &tmX)) != 0) return rc;
+  if (tile_wgs(p.M) == 1) {
+    if (a_mn && b_mn) return launch<1, true, true>(tmA, tmB, tmC, tmX, p, max_ctas, stream);
+    if (a_mn) return launch<1, true, false>(tmA, tmB, tmC, tmX, p, max_ctas, stream);
+    if (b_mn) return launch<1, false, true>(tmA, tmB, tmC, tmX, p, max_ctas, stream);
+    return launch<1, false, false>(tmA, tmB, tmC, tmX, p, max_ctas, stream);
+  }
+  if (a_mn && b_mn) return launch<2, true, true>(tmA, tmB, tmC, tmX, p, max_ctas, stream);
+  if (a_mn) return launch<2, true, false>(tmA, tmB, tmC, tmX, p, max_ctas, stream);
+  if (b_mn) return launch<2, false, true>(tmA, tmB, tmC, tmX, p, max_ctas, stream);
+  return launch<2, false, false>(tmA, tmB, tmC, tmX, p, max_ctas, stream);
 }
 
 // A operand map.  K-major: stored [M, K], box {64 k, 128 m}.  MN-major: stored [K, M], box {64 m, 64 k}.
