@@ -39,8 +39,9 @@ int b200_device_check(void);
  * may become resident while the previous kernel of the stream is still draining; it waits (griddepcontrol.wait) before
  * touching operands or outputs.  Used for the decode-step chain. */
 int b200_set_pdl(int enable);
-/* q-tile height of b200_fa_fwd / b200_fa_fwd_flashmask (returns the previous setting; NOT an error code): 2 (default) = 128
- * rows (8 warps) per CTA, 1 = 64 rows (4 warps).  Same rounding points; kept switchable for A/B measurements. */
+/* Kernel of b200_fa_fwd / b200_fa_fwd_flashmask (returns the previous setting; NOT an error code): 2 (default) = the wgmma
+ * kernel (128-row q tiles, TMA-fed 128-row K/V tiles), 1 = the mma.sync kernel (128-row q tiles, 8 warps), kept as the
+ * cross-check and as the paged prefill of b200_append_attention.  Same rounding points. */
 int b200_set_fa_fwd_impl(int impl);
 /* Kernel of b200_fa_bwd / b200_fa_bwd_flashmask (returns the previous setting): 2 (default) = the warp-specialised wgmma
  * kernel (128-row kv tiles, TMA-fed 64-row q tiles, TMA reduce-adds), 1 = the mma.sync kernel (64-row kv and q tiles), kept as

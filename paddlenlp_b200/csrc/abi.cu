@@ -35,7 +35,7 @@ int check_launch(const char* what) {
 
 static int g_pdl = 0;
 bool pdl_enabled() { return g_pdl != 0; }
-// attention kernel tile sizes (fa_fwd.cu, fa_bwd.cu): b200_set_fa_fwd_impl / b200_set_fa_bwd_impl
+// attention kernels (fa_fwd.cu, fa_bwd.cu): b200_set_fa_fwd_impl / b200_set_fa_bwd_impl, 2 = wgmma, 1 = mma.sync
 static int g_fa_fwd_impl = 2;
 int fa_fwd_impl() { return g_fa_fwd_impl; }
 static int g_fa_bwd_impl = 2;

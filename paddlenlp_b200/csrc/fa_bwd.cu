@@ -583,14 +583,6 @@ fa_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   }
 }
 
-// [B, S, heads, D] bf16 view with token stride ld, box {64 d, 1 head, rows, 1}: one 128-byte swizzled block of `rows` rows
-static int make_bf16_map(CUtensorMap* tm, const void* base, int64_t B, int64_t S, int64_t heads, int64_t D, int64_t ld,
-                         uint32_t rows) {
-  const uint64_t dims[4] = {static_cast<uint64_t>(D), static_cast<uint64_t>(heads), static_cast<uint64_t>(S), static_cast<uint64_t>(B)};
-  const uint64_t strides[3] = {static_cast<uint64_t>(D) * 2, static_cast<uint64_t>(ld) * 2, static_cast<uint64_t>(S * ld) * 2};
-  const uint32_t box[4] = {64, 1, rows, 1};
-  return encode_tmap_bf16(tm, base, 4, dims, strides, box);
-}
 // [B, S, heads, D] fp32 accumulation buffer, box {32 d, 1 head, 64 rows, 1}
 static int make_f32_map(CUtensorMap* tm, float* base, int64_t B, int64_t S, int64_t heads, int64_t D) {
   const uint64_t dims[4] = {static_cast<uint64_t>(D), static_cast<uint64_t>(heads), static_cast<uint64_t>(S), static_cast<uint64_t>(B)};
@@ -716,10 +708,10 @@ extern "C" int b200_fa_bwd_flashmask(const void* q, const void* k, const void* v
       rc = mask_start_rows ? launch<128, 64, true>(p, stream) : launch<128, 64, false>(p, stream);
   } else {
     CUtensorMap tm[7];
-    if ((rc = wg::make_bf16_map(&tm[0], q, B, S, num_heads, head_dim, ldq, wg::BQ)) != 0) return rc;
-    if ((rc = wg::make_bf16_map(&tm[1], k, B, S, num_kv_heads, head_dim, ldk, wg::BKV)) != 0) return rc;
-    if ((rc = wg::make_bf16_map(&tm[2], v, B, S, num_kv_heads, head_dim, ldv, wg::BKV)) != 0) return rc;
-    if ((rc = wg::make_bf16_map(&tm[3], dout, B, S, num_heads, head_dim, lddo, wg::BQ)) != 0) return rc;
+    if ((rc = make_bf16_map(&tm[0], q, B, S, num_heads, head_dim, ldq, wg::BQ)) != 0) return rc;
+    if ((rc = make_bf16_map(&tm[1], k, B, S, num_kv_heads, head_dim, ldk, wg::BKV)) != 0) return rc;
+    if ((rc = make_bf16_map(&tm[2], v, B, S, num_kv_heads, head_dim, ldv, wg::BKV)) != 0) return rc;
+    if ((rc = make_bf16_map(&tm[3], dout, B, S, num_heads, head_dim, lddo, wg::BQ)) != 0) return rc;
     if ((rc = wg::make_f32_map(&tm[4], dq_acc, B, S, num_heads, head_dim)) != 0) return rc;
     if ((rc = wg::make_f32_map(&tm[5], dk_acc, B, S, num_kv_heads, head_dim)) != 0) return rc;
     if ((rc = wg::make_f32_map(&tm[6], dv_acc, B, S, num_kv_heads, head_dim)) != 0) return rc;

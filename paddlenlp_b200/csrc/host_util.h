@@ -15,7 +15,7 @@ int fail_arg(const char* fmt, ...);   // records message, returns -1
 int check_launch(const char* what);  // cudaGetLastError() -> return code
 
 int sm_count();  // multiprocessors of the current device (cached per device)
-int fa_fwd_impl();         // b200_set_fa_fwd_impl(): 2 = 128-row q tiles (8 warps), 1 = 64-row q tiles (4 warps)
+int fa_fwd_impl();         // b200_set_fa_fwd_impl(): 2 = wgmma kernel, 1 = mma.sync kernel (cross-check)
 int fa_bwd_impl();         // b200_set_fa_bwd_impl(): 2 = wgmma kernel, 1 = mma.sync kernel (cross-check)
 // fa_fwd.cu, paged instantiation: prefill half of b200_append_attention
 int launch_fa_prefill_paged(const void* qkv, const void* key_cache, const void* value_cache, void* out, const int32_t* cu_seqlens_q,
@@ -53,6 +53,15 @@ int encode_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_
 // Same for fp32 elements (box[0] * 4 must be <= 128); used for TMA reduce-add into fp32 accumulation buffers.
 int encode_tmap_f32(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides,
                     const uint32_t* box);
+// Attention operand [B, S, heads, D] bf16 with token stride ld (elements), box {64 d, 1 head, rows, 1}: one 128-byte swizzled
+// block of `rows` rows.  Rows past S read as zeros, so a box never reaches into the next batch row.
+inline int make_bf16_map(CUtensorMap* tm, const void* base, int64_t B, int64_t S, int64_t heads, int64_t D, int64_t ld,
+                         uint32_t rows) {
+  const uint64_t dims[4] = {static_cast<uint64_t>(D), static_cast<uint64_t>(heads), static_cast<uint64_t>(S), static_cast<uint64_t>(B)};
+  const uint64_t strides[3] = {static_cast<uint64_t>(D) * 2, static_cast<uint64_t>(ld) * 2, static_cast<uint64_t>(S * ld) * 2};
+  const uint32_t box[4] = {64, 1, rows, 1};
+  return encode_tmap_bf16(tm, base, 4, dims, strides, box);
+}
 
 }  // namespace b200
 

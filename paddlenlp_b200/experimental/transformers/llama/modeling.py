@@ -112,11 +112,15 @@ class LlamaForCausalLMInferenceModel(GenerationInferenceModel):
         return {"block_tables": self.block_tables} if self.block_attn else {}
 
     # ---- forward ----
-    def _head(self, hidden):
+    def _head(self, hidden, decode=True):
+        """Logits of the given rows.  decode=False (prefill, once per prompt): the training path's GEMM, whose per-row sums run
+        in the same order as the training forward's, so prefill logits carry its bits; the decode step's split-K kernel
+        (few rows, weight streaming) adds K-range partials in L2 and can round a logit one bf16 ulp differently."""
         hn, _ = ops.add_rmsnorm(hidden, None, self.norm_weight, self.config.rms_norm_eps, want_residual=False)
-        if self.tied:
-            return self.transformer_block._mm(hn, self.embed_tokens, trans_b=True)
-        return self.transformer_block._mm(hn, self.lm_head_weight)
+        w, trans_b = (self.embed_tokens, True) if self.tied else (self.lm_head_weight, False)
+        if not decode:
+            return ops.gemm(hn, w, trans_b=trans_b)
+        return self.transformer_block._mm(hn, w, trans_b=trans_b)
 
     def _prefill(self, input_ids, seq_lens_encoder, caches):
         B, S = input_ids.shape
@@ -124,7 +128,7 @@ class LlamaForCausalLMInferenceModel(GenerationInferenceModel):
         hidden = self.transformer_block(emb, caches, B=B, S=S, seq_lens_encoder=seq_lens_encoder, **self._cache_kw())
         # rebuild_padding: keep the last valid position of every sequence
         last = (torch.arange(B, device=self.device) * S + seq_lens_encoder.to(torch.int64) - 1)
-        return self._head(hidden.index_select(0, last).contiguous())
+        return self._head(hidden.index_select(0, last).contiguous(), decode=False)
 
     def _decode(self, tgt_ids, seq_lens_decoder, caches):
         B = tgt_ids.numel()
@@ -140,4 +144,4 @@ class LlamaForCausalLMInferenceModel(GenerationInferenceModel):
         caches = self.allocate_caches(B, S)
         emb = ops.embedding_fwd(input_ids.to(self.device).reshape(-1), self.embed_tokens)
         hidden = self.transformer_block(emb, caches, B=B, S=S, seq_lens_encoder=None, **self._cache_kw())
-        return self._head(hidden).view(B, S, -1)
+        return self._head(hidden, decode=False).view(B, S, -1)

@@ -1,10 +1,12 @@
-"""Time the flash-attention forward and both backward kernels (b200_set_fa_bwd_impl 2 = wgmma, 1 = mma.sync) on an H100.
+"""Time both flash-attention forward kernels (b200_set_fa_fwd_impl 2 = wgmma, 1 = mma.sync) and both backward kernels
+(b200_set_fa_bwd_impl, the same numbering) on an H100.
 
 Shapes (B, S, q heads, kv heads, head_dim): the two benchmarked models, Llama-3.2-3B (1 x 4096, 24 / 8 heads) and the
 Qwen2-1.5B SFT micro-batch (4 x 2048, 12 / 2 heads), then the Llama-3-8B and Qwen2-7B layouts, all at head_dim 128; then the
 head_dim 64 models: Llama-3.2-1B (1 x 4096, 32 / 8), a Qwen2-0.5B SFT micro-batch (4 x 2048, 14 / 2) and TinyLlama
-(1 x 2048, 32 / 4).  The forward and the two backward kernels are timed alternately in one process (REPEATS rounds each), so
-clock and neighbour drift hit all alike; each line gives the median and the spread (min, max).
+(1 x 2048, 32 / 4).  The four kernels are timed alternately in one process (REPEATS rounds each), so clock and neighbour
+drift hit all alike; each line gives the median and the spread (min, max), and the impl 1 / impl 2 time ratio of the forward
+and of the backward.
 """
 import json
 import os
@@ -50,6 +52,7 @@ def main():
     dev = "cuda:0"
     lib = _lib.load()
     print(json.dumps(dict(gpu=gpu_info())), flush=True)
+    old_fwd = lib.b200_set_fa_fwd_impl(2)
     old_impl = lib.b200_set_fa_bwd_impl(2)
     for (B, S, nh, kvh, d) in SHAPES:
         ld = (nh + 2 * kvh) * d
@@ -63,22 +66,25 @@ def main():
         dq = dqkv[:, :, : nh * d].view(B, S, nh, d)
         dk = dqkv[:, :, nh * d: (nh + kvh) * d].view(B, S, kvh, d)
         dv = dqkv[:, :, (nh + kvh) * d:].view(B, S, kvh, d)
-        t_f = []
+        t_f = {1: [], 2: []}
         t_b = {1: [], 2: []}
         for _ in range(REPEATS):
-            t_f.append(timeit(lambda: ops.flash_attn_fwd(q, k, v, out=out)))
+            for impl in (2, 1):
+                lib.b200_set_fa_fwd_impl(impl)
+                t_f[impl].append(timeit(lambda: ops.flash_attn_fwd(q, k, v, out=out)))
+            lib.b200_set_fa_fwd_impl(2)
             for impl in (2, 1):
                 lib.b200_set_fa_bwd_impl(impl)
                 t_b[impl].append(timeit(lambda: ops.flash_attn_bwd(q, k, v, out, dout, lse, dq, dk, dv)))
         lib.b200_set_fa_bwd_impl(2)
         fl_f = 4.0 * B * nh * S * S * d / 2        # causal
         fl_b = 2.5 * fl_f
-        sm = summary(t_f)
-        rec = dict(shape=[B, S, nh, kvh], head_dim=d, fwd=dict(sm, tflops=fl_f / sm["median_ms"] / 1e9))
-        for impl in (2, 1):
-            sm = summary(t_b[impl])
-            rec[f"bwd_impl{impl}"] = dict(sm, tflops=fl_b / sm["median_ms"] / 1e9)
-        rec["bwd_impl1_over_impl2"] = rec["bwd_impl1"]["median_ms"] / rec["bwd_impl2"]["median_ms"]
+        rec = dict(shape=[B, S, nh, kvh], head_dim=d)
+        for kind, ts, fl in (("fwd", t_f, fl_f), ("bwd", t_b, fl_b)):
+            for impl in (2, 1):
+                sm = summary(ts[impl])
+                rec[f"{kind}_impl{impl}"] = dict(sm, tflops=fl / sm["median_ms"] / 1e9)
+            rec[f"{kind}_impl1_over_impl2"] = rec[f"{kind}_impl1"]["median_ms"] / rec[f"{kind}_impl2"]["median_ms"]
         print(json.dumps(rec), flush=True)
     lib.b200_set_fa_bwd_impl(old_impl)
     # FlashMask (packed samples): Qwen2-7B SFT row of 2048 tokens holding documents of 700 / 900 / 448 tokens; useful flops only
@@ -99,13 +105,24 @@ def main():
     out, lse = ops.flash_attn_fwd(q, k, v, mask_start=ms)
     dout = torch.randn_like(out)
     dq, dk, dv = torch.empty_like(out), torch.empty(B, S, kvh, d, device=dev, dtype=torch.bfloat16), torch.empty(B, S, kvh, d, device=dev, dtype=torch.bfloat16)
-    t_f = timeit(lambda: ops.flash_attn_fwd(q, k, v, out=out, mask_start=ms))
+    t_f = {1: [], 2: []}
+    for _ in range(REPEATS):
+        for impl in (2, 1):
+            lib.b200_set_fa_fwd_impl(impl)
+            t_f[impl].append(timeit(lambda: ops.flash_attn_fwd(q, k, v, out=out, mask_start=ms)))
+    lib.b200_set_fa_fwd_impl(2)
     t_b = timeit(lambda: ops.flash_attn_bwd(q, k, v, out, dout, lse, dq, dk, dv, mask_start=ms))
     t_fc = timeit(lambda: ops.flash_attn_fwd(q, k, v, out=out))
     t_bc = timeit(lambda: ops.flash_attn_bwd(q, k, v, out, dout, lse, dq, dk, dv))
     fl = 4.0 * B * nh * useful * d / 2
-    print(json.dumps(dict(flashmask_docs=docs, shape=[B, S, nh, kvh], fwd_ms=t_f, bwd_ms=t_b, plain_causal_fwd_ms=t_fc,
-                          plain_causal_bwd_ms=t_bc, useful_fwd_tflops=fl / t_f / 1e9, useful_bwd_tflops=2.5 * fl / t_b / 1e9)), flush=True)
+    rec = dict(flashmask_docs=docs, shape=[B, S, nh, kvh])
+    for impl in (2, 1):
+        sm = summary(t_f[impl])
+        rec[f"fwd_impl{impl}"] = dict(sm, useful_tflops=fl / sm["median_ms"] / 1e9)
+    rec["fwd_impl1_over_impl2"] = rec["fwd_impl1"]["median_ms"] / rec["fwd_impl2"]["median_ms"]
+    rec.update(bwd_ms=t_b, plain_causal_fwd_ms=t_fc, plain_causal_bwd_ms=t_bc, useful_bwd_tflops=2.5 * fl / t_b / 1e9)
+    print(json.dumps(rec), flush=True)
+    lib.b200_set_fa_fwd_impl(old_fwd)
 
 
 if __name__ == "__main__":
