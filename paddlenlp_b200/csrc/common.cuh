@@ -74,8 +74,9 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     }
   }
 }
-// The same bounded wait without the printf.  For loops that keep wgmma accumulators live across the wait: a function call
-// there makes ptxas save the accumulators around it (local-memory spills) and serialise every wgmma of the kernel.
+// The same bounded wait without the printf.  For kernels that issue wgmma: a function call in a loop that keeps accumulators
+// live makes ptxas save them around it (local-memory spills), and a call anywhere in the kernel, the producer branch included,
+// makes it wait for each wgmma before it issues the next (ptxas info C7510).
 __device__ __forceinline__ void mbar_wait_nocall(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   long long t0 = clock64();

@@ -10,9 +10,9 @@
 //   warpgroup 0     TMA producer   : one thread streams A (128 x 64) and B (64 x 256) k-blocks into a 4-stage ring of
 //                                    128B-swizzled shared memory (48 KB per stage); its registers go to the consumers
 //   warpgroups 1,2  MMA + epilogue : each owns 64 rows of the tile: wgmma m64n256k16 x 4 per k-block, fp32 accumulators in
-//                                    128 registers per thread; a k-block's stage is released once the next block's wgmmas
-//                                    are in flight; the epilogue (+bias, +C_old | +residual, SwiGLU forms, split-K
-//                                    reduction) works on the accumulator registers; with 128-row tiles it stages bf16
+//                                    128 registers per thread, the four wgmmas of a k-block issued back to back; a
+//                                    k-block's stage is released once the next block's wgmmas are in flight; the epilogue
+//                                    (+bias, +C_old | +residual, SwiGLU forms, split-K reduction) works on the accumulator registers; with 128-row tiles it stages bf16
 //                                    64 x 64 boxes in shared memory and stores them with TMA (C_old / residual / gate|up
 //                                    prefetched into L2 during the tile's last k-blocks), else it stores to global memory
 //   Operand majors: both K-major (contraction dim contiguous) and MN-major operands are fed straight from their
@@ -187,7 +187,9 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         const int kb1 = min(num_kb_total, kb0 + p.kb_per_split);
         for (int kb = kb0; kb < kb1; ++kb, ++it) {
           const int st = static_cast<int>(it % STAGES);
-          mbar_wait(&empty_bar[st], ((it / STAGES) & 1u) ^ 1u);
+          // No wait in this kernel may contain a function call (mbar_wait's printf), not even here in the producer: ptxas then
+          // serialises every wgmma of the kernel (it reports C7510), one k-step at a time with the tensor cores idle between them.
+          mbar_wait_nocall(&empty_bar[st], ((it / STAGES) & 1u) ^ 1u);
           uint8_t* sA = smem + st * STAGE_BYTES;
           uint8_t* sB = sA + A_BYTES;
           mbar_arrive_expect_tx(&full_bar[st], STAGE_BYTES);
@@ -239,7 +241,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     fence_acc(acc);
     for (int i = 0; i < nkb; ++i, ++it) {
       const int st = static_cast<int>(it % STAGES);
-      mbar_wait(&full_bar[st], (it / STAGES) & 1u);
+      mbar_wait_nocall(&full_bar[st], (it / STAGES) & 1u);
       const uint32_t sA = ring + st * STAGE_BYTES + a_off, sB = ring + st * STAGE_BYTES + A_BYTES;
       const uint64_t dA = wgmma_desc_sw128(sA, A_MN ? 64 * BK * 2 : 16, 1024);
       const uint64_t dB = wgmma_desc_sw128(sB, B_MN ? B_BYTES / 4 : 16, 1024);
