@@ -57,8 +57,9 @@ int b200_set_fa_bwd_impl(int impl);
  *   accumulate != 0: C_new = bf16(fp32(C_old) + acc)   (gradient accumulation, cf. llm/utils/fused_layers.py:36-74)
  *   bias            : optional fp32 [N], added in fp32 before the rounding (Qwen2 q/k/v bias, qwen2/modeling.py:478-480)
  * Reference call sites: llama/modeling.py:933-935,1103 (q/k/v/o), :632-652 (gate/up/down), :1894-1921 (lm_head).
- * Requires lda, ldb, ldc multiples of 8 elements and 16-byte aligned base pointers (M, N, K themselves are free: TMA
- * zero-fills / clips partial tiles).
+ * Requires lda, ldb, ldc multiples of 8 elements and 16-byte aligned base pointers: A, B, C and residual here, X, W, GU and
+ * Mout of b200_gemm_swiglu_bf16, dY, Wdown, GU and DGU of b200_gemm_swiglu_bwd_bf16, A, B and a non-NULL C of
+ * b200_gemm_bf16_splitk; any other is an argument error (M, N, K themselves are free: TMA zero-fills / clips partial tiles).
  */
 int b200_gemm_bf16(const void* A, const void* B, void* C, const float* bias, int64_t M, int64_t N, int64_t K,
                    int64_t lda, int64_t ldb, int64_t ldc, int a_mn_major, int b_mn_major, int accumulate,

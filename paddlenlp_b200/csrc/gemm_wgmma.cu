@@ -12,9 +12,9 @@
 //   warpgroups 1,2  MMA + epilogue : each owns 64 rows of the tile: wgmma m64n256k16 x 4 per k-block, fp32 accumulators in
 //                                    128 registers per thread, the four wgmmas of a k-block issued back to back; a
 //                                    k-block's stage is released once the next block's wgmmas are in flight; the epilogue
-//                                    (+bias, +C_old | +residual, SwiGLU forms, split-K reduction) works on the accumulator registers; with 128-row tiles it stages bf16
-//                                    64 x 64 boxes in shared memory and stores them with TMA (C_old / residual / gate|up
-//                                    prefetched into L2 during the tile's last k-blocks), else it stores to global memory
+//                                    (+bias, +C_old | +residual, SwiGLU forms) stages bf16 64 x 64 boxes in shared memory and
+//                                    stores them with TMA (C_old / residual / gate|up prefetched into L2 during the tile's
+//                                    last k-blocks); split-K adds its fp32 partial sums from the registers into L2
 //   Operand majors: both K-major (contraction dim contiguous) and MN-major operands are fed straight from their
 //   row-major global layout through TMA (wgmma reads either major for 16-bit types); no transposes are materialised.
 #include "../../include/b200nlp.h"
@@ -43,8 +43,8 @@ struct Tile {
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int STAGES = NWG == 2 ? 4 : 5;
-  // NWG = 2: two 64 x 64 bf16 output boxes per consumer warpgroup for the shared-memory epilogue
-  static constexpr int EPI_BYTES = NWG == 2 ? NWG * 2 * EPI_BOX_BYTES : 0;
+  // two 64 x 64 bf16 output boxes per consumer warpgroup for the shared-memory epilogue
+  static constexpr int EPI_BYTES = NWG * 2 * EPI_BOX_BYTES;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BYTES + 256 + 1024;   // + barriers + alignment slack (<= 227 KB)
 };
 static int tile_wgs(int64_t M) { return M <= 64 ? 1 : 2; }
@@ -70,8 +70,6 @@ struct Params {
   bf16* aux;               // mode 4: gate|up output (nullable); mode 5: saved gate|up input
   int64_t ld_aux;
   float* ws;               // mode 3: fp32 [M, N] accumulation buffer
-  int smem_epi;            // NWG = 2, modes 0, 1, 2, 4, 5 with 16-byte aligned outputs: the epilogue stores through shared
-                           // memory and TMA (tmC, tmX); otherwise it stores from the registers
 };
 
 __device__ __forceinline__ void tile_coords(int t, int num_m, int num_n, int& m_blk, int& n_blk, int GM) {
@@ -93,13 +91,7 @@ __device__ __forceinline__ void fence_acc(float (&acc)[128]) {
   for (int i = 0; i < 128; ++i) asm volatile("" : "+f"(acc[i])::"memory");
 }
 
-__device__ __forceinline__ void store_bf16x2(bf16* base, int64_t ld, int row, int col, int N, float v0, float v1) {
-  bf16* dst = base + static_cast<int64_t>(row) * ld + col;
-  if (col + 1 < N) *reinterpret_cast<uint32_t*>(dst) = pack_bf16x2(v0, v1);
-  else if (col < N) *dst = __float2bfloat16_rn(v0);
-}
-
-// ---- shared-memory epilogue (NWG = 2) ----
+// ---- shared-memory epilogue (every mode but split-K) ----
 // A consumer warpgroup's 64 x 256 accumulator tile leaves as 64 x 64 bf16 boxes.  The warpgroup writes a box into one of its
 // two 8 KB buffers in the 128B-swizzled TMA layout, one thread stores it with cp.async.bulk.tensor, and the warpgroup goes on
 // to the next box, or to the next tile's wgmmas, while the store drains.  TMA drops rows >= M and columns past the tensor
@@ -146,7 +138,7 @@ __device__ __forceinline__ void epi_prefetch(const CUtensorMap* tmC, const CUten
   }
 }
 
-// tmC / tmX: the epilogue's tensor maps when p.smem_epi is set (box {64, 64}).  tmC is the output (mode 4: m); tmX is the
+// tmC / tmX: the epilogue's tensor maps outside split-K (box {64, 64}).  tmC is the output (mode 4: m); tmX is the
 // residual (mode 2, read through L2 prefetches only), gate|up (mode 4 output, mode 5 input).
 template <int NWG, bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(Tile<NWG>::NUM_THREADS, 1)
@@ -224,7 +216,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   constexpr uint32_t A_KSTEP = A_MN ? 2048u : 32u, B_KSTEP = B_MN ? 2048u : 32u;
   const uint32_t a_off = static_cast<uint32_t>(cw) * (64 * BK * 2);
   const bool leader = (threadIdx.x & 127) == 0;           // issues the warpgroup's epilogue stores and prefetches
-  const bool prefetch = p.smem_epi && leader && (p.epi_mode == 1 || p.epi_mode == 2 || p.epi_mode == 5);
+  const bool prefetch = leader && (p.epi_mode == 1 || p.epi_mode == 2 || p.epi_mode == 5);
   const uint32_t ebuf = smem_u32(smem + STAGES * STAGE_BYTES) + cw * 2 * EPI_BOX_BYTES;   // this warpgroup's two boxes
   uint32_t nbox = 0;                                       // boxes stored so far (modes 0-2 alternate the two buffers)
   uint32_t it = 0;
@@ -251,9 +243,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         wgmma_m64n256k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, dA + ((kk * A_KSTEP) >> 4), dB + ((kk * B_KSTEP) >> 4),
                                                      (i > 0 || kk > 0) ? 1u : 0u);
       wgmma_commit();
-      if constexpr (NWG == 2) {
-        if (prefetch && i == prefetch_kb) epi_prefetch(&tmC, &tmX, p, n_blk, m_blk * BM + cw * 64);
-      }
+      if (prefetch && i == prefetch_kb) epi_prefetch(&tmC, &tmX, p, n_blk, m_blk * BM + cw * 64);
       wgmma_wait<1>();                                     // k-block i-1 is finished: its stage can be refilled
       if (i > 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
     }
@@ -262,208 +252,146 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     if (nkb > 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
 
     // accumulator fragment: register 4j + 2i + e holds row 16 wi + lane/4 + 8i, column 8j + 2 (lane % 4) + e
-    const int row_base = m_blk * BM + cw * 64 + wi * 16 + (lane >> 2);
+    const int row0 = m_blk * BM + cw * 64;                 // first row of the warpgroup's rows and boxes
+    const int r_lo = wi * 16 + (lane >> 2);                // this thread's rows: row0 + r_lo + 8 i
     const int cq = 2 * (lane & 3);
-    if constexpr (NWG == 2) {
-      if (p.smem_epi) {
-        // Same fp32 operations in the same order, and the same bf16 roundings, as the register epilogue below.
-        const int row0 = m_blk * BM + cw * 64;             // first row of the warpgroup's boxes
-        const int r_lo = wi * 16 + (lane >> 2);            // this thread's rows in a box: r_lo + 8 i
-        if (p.epi_mode == 4) {
+    if (p.epi_mode == 3) {
+      // split-K: fp32 partial sums reduced in L2 (N % 8 == 0: a pair is 8-byte aligned); the bias is added where the sums are
+      // rounded to bf16
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {                    // 64 channels per box
-            const int ch0 = n_blk * 128 + EPI_BOX * h;
-            if (ch0 >= p.swiglu_inter) continue;
-            if (p.aux != nullptr) {                        // gate and up, as the unfused GEMM rounds them
-              epi_begin<0>(cw, leader);
+      for (int i = 0; i < 2; ++i) {
+        const int row = row0 + r_lo + 8 * i;
+        if (row >= p.M) continue;
 #pragma unroll
-              for (int i = 0; i < 2; ++i)
-#pragma unroll
-                for (int jj = 0; jj < 8; ++jj) {
-                  const int j = 8 * h + jj;
-                  st_shared_u32(epi_slot(ebuf, r_lo + 8 * i, jj, lane), pack_bf16x2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]));
-                  st_shared_u32(epi_slot(ebuf + EPI_BOX_BYTES, r_lo + 8 * i, jj, lane),
-                                pack_bf16x2(acc[4 * (j + 16) + 2 * i], acc[4 * (j + 16) + 2 * i + 1]));
-                }
-              epi_end(cw);
-              if (leader) {
-                tma_store_2d(&tmX, ebuf, ch0, row0);
-                tma_store_2d(&tmX, ebuf + EPI_BOX_BYTES, p.swiglu_inter + ch0, row0);
-                tma_store_commit();
-              }
-            }
-            epi_begin<0>(cw, leader);
-#pragma unroll
-            for (int i = 0; i < 2; ++i)
-#pragma unroll
-              for (int jj = 0; jj < 8; ++jj) {
-                const int j = 8 * h + jj;
-                const uint32_t gp = pack_bf16x2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
-                const uint32_t up = pack_bf16x2(acc[4 * (j + 16) + 2 * i], acc[4 * (j + 16) + 2 * i + 1]);
-                st_shared_u32(epi_slot(ebuf, r_lo + 8 * i, jj, lane), swiglu_fwd_pair(gp, up));
-              }
-            epi_end(cw);
-            if (leader) {
-              tma_store_2d(&tmC, ebuf, ch0, row0);
-              tma_store_commit();
-            }
-          }
-          continue;
+        for (int j = 0; j < 32; ++j) {
+          const int col = n_blk * BN + 8 * j + cq;
+          if (col >= p.N) continue;
+          float* w = p.ws + static_cast<int64_t>(row) * p.N + col;
+          asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(w), "f"(acc[4 * j + 2 * i]), "f"(acc[4 * j + 2 * i + 1])
+                       : "memory");
         }
-        if (p.epi_mode == 5) {                             // d(gate) box | d(up) box per 64 channels
-#pragma unroll
-          for (int s = 0; s < BN / EPI_BOX; ++s) {
-            const int ch0 = n_blk * BN + EPI_BOX * s;
-            if (ch0 >= p.N) continue;
-            epi_begin<0>(cw, leader);
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {                  // 8 input registers at a time next to the 128 accumulators
-              const int i = q >> 1, jj0 = 4 * (q & 1);
-              uint32_t g[4], u[4];
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                const int row = row0 + r_lo + 8 * i, ch = ch0 + 8 * (jj0 + k) + cq;
-                g[k] = ld_pair(p.aux, p.ld_aux, row, ch, p.M, p.N);
-                u[k] = ld_pair(p.aux + p.swiglu_inter, p.ld_aux, row, ch, p.M, p.N);
-              }
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                const int jj = jj0 + k, j = 8 * s + jj;
-                uint32_t dg2, du2;                         // d(m) with the GEMM's own bf16 output rounding
-                swiglu_bwd_pair(g[k], u[k], bf16_round(acc[4 * j + 2 * i]), bf16_round(acc[4 * j + 2 * i + 1]), dg2, du2);
-                st_shared_u32(epi_slot(ebuf, r_lo + 8 * i, jj, lane), dg2);
-                st_shared_u32(epi_slot(ebuf + EPI_BOX_BYTES, r_lo + 8 * i, jj, lane), du2);
-              }
-            }
-            epi_end(cw);
-            if (leader) {
-              tma_store_2d(&tmC, ebuf, ch0, row0);
-              tma_store_2d(&tmC, ebuf + EPI_BOX_BYTES, p.swiglu_inter + ch0, row0);
-              tma_store_commit();
-            }
-          }
-          continue;
-        }
-        // modes 0, 1, 2
-#pragma unroll
-        for (int s = 0; s < BN / EPI_BOX; ++s) {
-          const int col0 = n_blk * BN + EPI_BOX * s;
-          if (col0 >= p.N) continue;
-          const uint32_t buf = ebuf + (nbox++ & 1u) * EPI_BOX_BYTES;
-          epi_begin<1>(cw, leader);
-#pragma unroll
-          for (int i = 0; i < 2; ++i) {
-            uint32_t o[8];                                 // C_old (mode 1) or residual (mode 2) pairs of row r_lo + 8 i
-            if (p.epi_mode != 0) {
-              const bf16* src = p.epi_mode == 1 ? p.c : p.r;
-              const int64_t ld = p.epi_mode == 1 ? p.ldc : p.ldr;
-#pragma unroll
-              for (int jj = 0; jj < 8; ++jj) o[jj] = ld_pair(src, ld, row0 + r_lo + 8 * i, col0 + 8 * jj + cq, p.M, p.N);
-            }
-#pragma unroll
-            for (int jj = 0; jj < 8; ++jj) {
-              const int j = 8 * s + jj, col = col0 + 8 * jj + cq;
-              float f0 = acc[4 * j + 2 * i], f1 = acc[4 * j + 2 * i + 1];
-              if (p.bias != nullptr) {
-                if (col < p.N) f0 += __ldg(p.bias + col);
-                if (col + 1 < p.N) f1 += __ldg(p.bias + col + 1);
-              }
-              if (p.epi_mode != 0) {
-                if (p.epi_mode == 2) { f0 = bf16_round(f0); f1 = bf16_round(f1); }
-                const float2 of = unpack_bf16x2(o[jj]);
-                f0 += of.x;
-                f1 += of.y;
-              }
-              st_shared_u32(epi_slot(buf, r_lo + 8 * i, jj, lane), pack_bf16x2(f0, f1));
-            }
-          }
-          epi_end(cw);
-          if (leader) {
-            tma_store_2d(&tmC, buf, col0, row0);
-            tma_store_commit();
-          }
-        }
-        continue;
       }
+      continue;
     }
     if (p.epi_mode == 4) {
       // gate|up + SwiGLU (llama/modeling.py:38-45, 632-652): accumulator columns [0,128) = gate, [128,256) = up of channels
       // [128 n_blk, +128).  Rounding points of the unfused path: gate and up each rounded to bf16 (the Linear outputs, kept for
       // the backward), then silu(g) * u in fp32 and one rounding.
 #pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        const int row = row_base + 8 * i;
-        if (row >= p.M) continue;
+      for (int h = 0; h < 2; ++h) {                        // 64 channels per box
+        const int ch0 = n_blk * 128 + EPI_BOX * h;
+        if (ch0 >= p.swiglu_inter) continue;
+        if (p.aux != nullptr) {                            // gate and up, as the unfused GEMM rounds them
+          epi_begin<0>(cw, leader);
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const int ch = n_blk * 128 + 8 * j + cq;
-          if (ch >= p.swiglu_inter) continue;
-          const uint32_t gp = pack_bf16x2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
-          const uint32_t up = pack_bf16x2(acc[4 * (j + 16) + 2 * i], acc[4 * (j + 16) + 2 * i + 1]);
-          if (p.aux != nullptr) {
-            bf16* g = p.aux + static_cast<int64_t>(row) * p.ld_aux + ch;
-            *reinterpret_cast<uint32_t*>(g) = gp;
-            *reinterpret_cast<uint32_t*>(g + p.swiglu_inter) = up;
+          for (int i = 0; i < 2; ++i)
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+              const int j = 8 * h + jj;
+              st_shared_u32(epi_slot(ebuf, r_lo + 8 * i, jj, lane), pack_bf16x2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]));
+              st_shared_u32(epi_slot(ebuf + EPI_BOX_BYTES, r_lo + 8 * i, jj, lane),
+                            pack_bf16x2(acc[4 * (j + 16) + 2 * i], acc[4 * (j + 16) + 2 * i + 1]));
+            }
+          epi_end(cw);
+          if (leader) {
+            tma_store_2d(&tmX, ebuf, ch0, row0);
+            tma_store_2d(&tmX, ebuf + EPI_BOX_BYTES, p.swiglu_inter + ch0, row0);
+            tma_store_commit();
           }
-          *reinterpret_cast<uint32_t*>(p.c + static_cast<int64_t>(row) * p.ldc + ch) = swiglu_fwd_pair(gp, up);
+        }
+        epi_begin<0>(cw, leader);
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const int j = 8 * h + jj;
+            const uint32_t gp = pack_bf16x2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
+            const uint32_t up = pack_bf16x2(acc[4 * (j + 16) + 2 * i], acc[4 * (j + 16) + 2 * i + 1]);
+            st_shared_u32(epi_slot(ebuf, r_lo + 8 * i, jj, lane), swiglu_fwd_pair(gp, up));
+          }
+        epi_end(cw);
+        if (leader) {
+          tma_store_2d(&tmC, ebuf, ch0, row0);
+          tma_store_commit();
         }
       }
       continue;
     }
-    if (p.epi_mode == 5) {
-      // d(m) with the GEMM's own bf16 output rounding, then the SwiGLU backward of the saved gate|up (bit-identical to
-      // b200_gemm_bf16 followed by b200_swiglu_bwd)
+    if (p.epi_mode == 5) {                                 // d(gate) box | d(up) box per 64 channels
+#pragma unroll
+      for (int s = 0; s < BN / EPI_BOX; ++s) {
+        const int ch0 = n_blk * BN + EPI_BOX * s;
+        if (ch0 >= p.N) continue;
+        epi_begin<0>(cw, leader);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {                      // 8 input registers at a time next to the 128 accumulators
+          const int i = q >> 1, jj0 = 4 * (q & 1);
+          uint32_t g[4], u[4];
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const int row = row0 + r_lo + 8 * i, ch = ch0 + 8 * (jj0 + k) + cq;
+            g[k] = ld_pair(p.aux, p.ld_aux, row, ch, p.M, p.N);
+            u[k] = ld_pair(p.aux + p.swiglu_inter, p.ld_aux, row, ch, p.M, p.N);
+          }
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const int jj = jj0 + k, j = 8 * s + jj;
+            uint32_t dg2, du2;                             // d(m) with the GEMM's own bf16 output rounding
+            swiglu_bwd_pair(g[k], u[k], bf16_round(acc[4 * j + 2 * i]), bf16_round(acc[4 * j + 2 * i + 1]), dg2, du2);
+            st_shared_u32(epi_slot(ebuf, r_lo + 8 * i, jj, lane), dg2);
+            st_shared_u32(epi_slot(ebuf + EPI_BOX_BYTES, r_lo + 8 * i, jj, lane), du2);
+          }
+        }
+        epi_end(cw);
+        if (leader) {
+          tma_store_2d(&tmC, ebuf, ch0, row0);
+          tma_store_2d(&tmC, ebuf + EPI_BOX_BYTES, p.swiglu_inter + ch0, row0);
+          tma_store_commit();
+        }
+      }
+      continue;
+    }
+    // modes 0, 1, 2
+#pragma unroll
+    for (int s = 0; s < BN / EPI_BOX; ++s) {
+      const int col0 = n_blk * BN + EPI_BOX * s;
+      if (col0 >= p.N) continue;
+      const uint32_t buf = ebuf + (nbox++ & 1u) * EPI_BOX_BYTES;
+      epi_begin<1>(cw, leader);
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
-        const int row = row_base + 8 * i;
-        if (row >= p.M) continue;
-        const bf16* gu = p.aux + static_cast<int64_t>(row) * p.ld_aux;
-        bf16* dgu = p.c + static_cast<int64_t>(row) * p.ldc;
+        uint32_t o[8];                                     // C_old (mode 1) or residual (mode 2) pairs of row r_lo + 8 i
+        if (p.epi_mode != 0) {
+          const bf16* src = p.epi_mode == 1 ? p.c : p.r;
+          const int64_t ld = p.epi_mode == 1 ? p.ldc : p.ldr;
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const int ch = n_blk * BN + 8 * j + cq;
-          if (ch >= p.N) continue;
-          const float2 dr = unpack_bf16x2(pack_bf16x2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]));
-          uint32_t dg2, du2;
-          swiglu_bwd_pair(*reinterpret_cast<const uint32_t*>(gu + ch), *reinterpret_cast<const uint32_t*>(gu + p.swiglu_inter + ch),
-                          dr.x, dr.y, dg2, du2);
-          *reinterpret_cast<uint32_t*>(dgu + ch) = dg2;
-          *reinterpret_cast<uint32_t*>(dgu + p.swiglu_inter + ch) = du2;
+          for (int jj = 0; jj < 8; ++jj) o[jj] = ld_pair(src, ld, row0 + r_lo + 8 * i, col0 + 8 * jj + cq, p.M, p.N);
+        }
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          const int j = 8 * s + jj, col = col0 + 8 * jj + cq;
+          float f0 = acc[4 * j + 2 * i], f1 = acc[4 * j + 2 * i + 1];
+          if (p.bias != nullptr) {
+            if (col < p.N) f0 += __ldg(p.bias + col);
+            if (col + 1 < p.N) f1 += __ldg(p.bias + col + 1);
+          }
+          if (p.epi_mode != 0) {
+            if (p.epi_mode == 2) { f0 = bf16_round(f0); f1 = bf16_round(f1); }
+            const float2 of = unpack_bf16x2(o[jj]);
+            f0 += of.x;
+            f1 += of.y;
+          }
+          st_shared_u32(epi_slot(buf, r_lo + 8 * i, jj, lane), pack_bf16x2(f0, f1));
         }
       }
-      continue;
-    }
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      const int row = row_base + 8 * i;
-      if (row >= p.M) continue;
-#pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        const int col = n_blk * BN + 8 * j + cq;
-        if (col >= p.N) continue;
-        float f0 = acc[4 * j + 2 * i], f1 = acc[4 * j + 2 * i + 1];
-        if (p.epi_mode == 3) {          // split-K: fp32 partial sums reduced in L2 (N % 8 == 0: a pair is 8-byte aligned)
-          float* w = p.ws + static_cast<int64_t>(row) * p.N + col;
-          asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(w), "f"(f0), "f"(f1) : "memory");
-          continue;
-        }
-        if (p.bias != nullptr) {
-          f0 += __ldg(p.bias + col);
-          if (col + 1 < p.N) f1 += __ldg(p.bias + col + 1);
-        }
-        if (p.epi_mode == 1 || p.epi_mode == 2) {
-          const bf16* o = p.epi_mode == 1 ? p.c + static_cast<int64_t>(row) * p.ldc + col : p.r + static_cast<int64_t>(row) * p.ldr + col;
-          if (p.epi_mode == 2) { f0 = bf16_round(f0); f1 = bf16_round(f1); }
-          f0 += __bfloat162float(o[0]);
-          if (col + 1 < p.N) f1 += __bfloat162float(o[1]);
-        }
-        store_bf16x2(p.c, p.ldc, row, col, p.N, f0, f1);
+      epi_end(cw);
+      if (leader) {
+        tma_store_2d(&tmC, buf, col0, row0);
+        tma_store_commit();
       }
     }
   }
-  if constexpr (NWG == 2) {
-    if (leader) tma_store_wait<0>();                       // the box buffers stay allocated until the last store is done
-  }
+  if (leader) tma_store_wait<0>();                         // the box buffers stay allocated until the last store is done
 }
 
 template <int NWG, bool A_MN, bool B_MN>
@@ -506,34 +434,25 @@ static int make_epi_map(CUtensorMap* tm, const void* base, int64_t rows, int64_t
 }
 static bool aligned16(const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; }
 
-// Selects the shared-memory epilogue for 128-row tiles outside split-K and builds its tensor maps.  TMA needs 16-byte aligned
-// base addresses (the strides are multiples of 8 elements already); an operand that is not (e.g. an `out=` view starting at
-// an odd column) keeps the register epilogue.
-static int setup_smem_epilogue(Params& p, CUtensorMap* tmC, CUtensorMap* tmX) {
-  p.smem_epi = 0;
-  if (tile_wgs(p.M) != 2 || p.epi_mode == 3 || !aligned16(p.c)) return 0;
-  int rc = 0;
+// Tensor maps of the shared-memory epilogue (every mode but split-K).  TMA needs 16-byte aligned base addresses (the strides
+// are multiples of 8 elements already): the entry points reject outputs and epilogue inputs that are not.
+static int setup_smem_epilogue(const Params& p, CUtensorMap* tmC, CUtensorMap* tmX) {
+  int rc;
   switch (p.epi_mode) {
     case 2:
-      if (!aligned16(p.r)) return 0;
       if ((rc = make_epi_map(tmX, p.r, p.M, p.N, p.ldr)) != 0) return rc;
-      rc = make_epi_map(tmC, p.c, p.M, p.N, p.ldc);
-      break;
+      return make_epi_map(tmC, p.c, p.M, p.N, p.ldc);
+    case 3:
+      return 0;
     case 4:   // p.N = 2 I: tmC is m [M, I], tmX the gate|up output [M, 2I]
-      if (p.aux != nullptr && !aligned16(p.aux)) return 0;
       if (p.aux != nullptr && (rc = make_epi_map(tmX, p.aux, p.M, p.N, p.ld_aux)) != 0) return rc;
-      rc = make_epi_map(tmC, p.c, p.M, p.swiglu_inter, p.ldc);
-      break;
+      return make_epi_map(tmC, p.c, p.M, p.swiglu_inter, p.ldc);
     case 5:   // p.N = I: tmC is d(gate)|d(up) [M, 2I], tmX the saved gate|up [M, 2I]
-      if (!aligned16(p.aux)) return 0;
       if ((rc = make_epi_map(tmX, p.aux, p.M, 2ll * p.N, p.ld_aux)) != 0) return rc;
-      rc = make_epi_map(tmC, p.c, p.M, 2ll * p.N, p.ldc);
-      break;
+      return make_epi_map(tmC, p.c, p.M, 2ll * p.N, p.ldc);
     default:  // 0, 1
-      rc = make_epi_map(tmC, p.c, p.M, p.N, p.ldc);
+      return make_epi_map(tmC, p.c, p.M, p.N, p.ldc);
   }
-  if (rc == 0) p.smem_epi = 1;
-  return rc;
 }
 
 static int dispatch(bool a_mn, bool b_mn, const CUtensorMap& tmA, const CUtensorMap& tmB, Params p, int max_ctas,
@@ -600,6 +519,8 @@ extern "C" int b200_gemm_bf16_ex(const void* A, const void* B, void* C, const fl
   B200_CHECK_ARG(!(residual && accumulate), "gemm: residual and accumulate are mutually exclusive");
   B200_CHECK_ARG(!residual || ldr % 8 == 0, "gemm: ldr must be a multiple of 8");
   B200_CHECK_ARG(M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31), "gemm: dimension too large");
+  B200_CHECK_ARG(aligned16(C), "gemm: C must be 16-byte aligned");
+  B200_CHECK_ARG(!residual || aligned16(residual), "gemm: residual must be 16-byte aligned");
   CUtensorMap tmA, tmB;
   int rc;
   if ((rc = make_a_map(&tmA, A, M, K, lda, a_mn_major)) != 0) return rc;
@@ -628,6 +549,8 @@ extern "C" int b200_gemm_swiglu_bf16(const void* X, const void* W, void* GU, voi
                  (long long)inter);
   B200_CHECK_ARG(ldx % 8 == 0 && ldw % 8 == 0 && ldgu % 8 == 0 && ldm % 8 == 0, "gemm_swiglu: leading dimensions must be multiples of 8");
   B200_CHECK_ARG(M < (1ll << 31) && inter < (1ll << 30) && K < (1ll << 31), "gemm_swiglu: dimension too large");
+  B200_CHECK_ARG(aligned16(Mout), "gemm_swiglu: Mout must be 16-byte aligned");
+  B200_CHECK_ARG(!GU || aligned16(GU), "gemm_swiglu: GU must be 16-byte aligned");
   CUtensorMap tmA, tmB;
   int rc;
   if ((rc = make_a_map(&tmA, X, M, K, ldx, false)) != 0) return rc;
@@ -655,6 +578,8 @@ extern "C" int b200_gemm_swiglu_bwd_bf16(const void* dY, const void* Wdown, cons
                  (long long)inter);
   B200_CHECK_ARG(lddy % 8 == 0 && ldw % 8 == 0 && ldgu % 8 == 0 && lddgu % 8 == 0, "gemm_swiglu_bwd: leading dimensions must be multiples of 8");
   B200_CHECK_ARG(M < (1ll << 31) && inter < (1ll << 30) && K < (1ll << 31), "gemm_swiglu_bwd: dimension too large");
+  B200_CHECK_ARG(aligned16(GU), "gemm_swiglu_bwd: GU must be 16-byte aligned");
+  B200_CHECK_ARG(aligned16(DGU), "gemm_swiglu_bwd: DGU must be 16-byte aligned");
   CUtensorMap tmA, tmB;
   int rc;
   if ((rc = make_a_map(&tmA, dY, M, K, lddy, false)) != 0) return rc;
@@ -710,6 +635,7 @@ extern "C" int b200_gemm_bf16_splitk(const void* A, const void* B, void* C, cons
   B200_CHECK_ARG(A && B && workspace, "gemm_splitk: null pointer");
   B200_CHECK_ARG(M > 0 && N > 0 && K > 0 && N % 8 == 0, "gemm_splitk: bad dimensions (N must be a multiple of 8)");
   B200_CHECK_ARG(lda % 8 == 0 && ldb % 8 == 0 && ldc % 8 == 0, "gemm_splitk: leading dimensions must be multiples of 8");
+  B200_CHECK_ARG(!C || aligned16(C), "gemm_splitk: C must be 16-byte aligned");
   CUtensorMap tmA, tmB;
   int rc;
   if ((rc = make_a_map(&tmA, A, M, K, lda, a_mn_major)) != 0) return rc;

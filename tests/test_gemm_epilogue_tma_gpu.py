@@ -1,4 +1,4 @@
-"""Bit-exact checks of the wgmma GEMM's shared-memory / TMA-store epilogue (128-row tiles).
+"""Bit-exact checks of the wgmma GEMM's shared-memory / TMA-store epilogue (64- and 128-row tiles).
 
 Reference: the kernel's own fp32 accumulators, from b200_gemm_bf16_splitk with split_k = 1 and C = NULL (the same tiles in the
 same k order; its reduce-add into a zeroed workspace is exact).  The epilogue is then applied in torch with the kernel's
@@ -106,16 +106,20 @@ def test_step_gemm_bit_exact(case):
 
 @pytest.mark.parametrize("mode", [0, 1, 2])
 @pytest.mark.parametrize("trans", [(False, False), (True, False), (False, True), (True, True)])
-def test_ragged_edges(mode, trans):
-    """M and N not multiples of the tile: TMA clips the last boxes (5112 = 19 x 256 + 248, 4095 = 31 x 128 + 127)."""
-    _check(4095, 5112, 1000, trans[0], trans[1], mode, bias=mode != 1, seed=11)
+@pytest.mark.parametrize("M", [4095, 5, 33, 48, 64])
+def test_ragged_edges(M, mode, trans):
+    """M and N not multiples of the tile: TMA clips the last boxes (5112 = 19 x 256 + 248, 4095 = 31 x 128 + 127).
+    M <= 64 runs 64-row tiles (the decode step's and small prefills' GEMMs)."""
+    _check(M, 5112, 1000, trans[0], trans[1], mode, bias=mode != 1, seed=11)
 
 
 @pytest.mark.parametrize("max_ctas", [1, 7, 0])
 @pytest.mark.parametrize("mode", [0, 1, 2])
-def test_max_ctas_buffer_recycling(max_ctas, mode):
-    """One CTA walking every tile, 7 CTAs (a partial last raster group), and all SMs."""
-    _check(1100, 1400, 192, False, False, mode, bias=True, max_ctas=max_ctas, seed=21)
+@pytest.mark.parametrize("M,N", [(1100, 1400), (48, 3000)])
+def test_max_ctas_buffer_recycling(M, N, max_ctas, mode):
+    """One CTA walking every tile, 7 CTAs (a partial last raster group; 5 of them run two of the 12 64-row tiles), and all
+    SMs."""
+    _check(M, N, 192, False, False, mode, bias=True, max_ctas=max_ctas, seed=21)
 
 
 @pytest.mark.parametrize("mode", [0, 1, 2])
@@ -123,30 +127,26 @@ def test_strided_views(mode):
     _check(700, 520, 256, False, True, mode, out_pad=72, seed=31)
 
 
+@pytest.mark.parametrize("offset", [4, 8])
 @pytest.mark.parametrize("mode", [0, 1, 2])
-def test_misaligned_output_register_fallback(mode):
-    """An output view starting 8 bytes past a 16-byte boundary cannot be a TMA base: the register epilogue stores it."""
+def test_misaligned_output_rejected(mode, offset):
+    """A view starting 4 or 8 bytes past a 16-byte boundary cannot be a TMA base: an output (modes 0, 1) or residual (mode 2)
+    view like that is an argument error, and nothing is written."""
+    from paddlenlp_b200._lib import B200Error
+
     ops = _ops()
     M, N, K = 600, 512, 256
     a, b = _operands(M, N, K, False, False, 41)
-    acc = _acc(a, b, False, False)
+    e = offset // 2
     buf = torch.full((M, N + 8), float("nan"), dtype=BF16, device=DEV)
-    out = buf[:, 4:N + 4]
-    residual = None
-    if mode == 0:
-        want = acc.to(BF16)
-    elif mode == 1:
-        out.copy_(_rand(M, N, seed=42))
-        want = (acc + out.float()).to(BF16)
-    else:
-        rbuf = torch.empty(M, N + 8, dtype=BF16, device=DEV)
-        residual = rbuf[:, 4:N + 4]
-        residual.copy_(_rand(M, N, seed=43))
-        want = (acc.to(BF16).float() + residual.float()).to(BF16)
-    ops.gemm(a, b, out, accumulate=mode == 1, residual=residual)
+    out, residual = buf[:, e:N + e], None
+    if mode == 2:
+        out = buf[:, :N]
+        residual = _rand(M, N + 8, seed=43)[:, e:N + e]
+    with pytest.raises(B200Error, match="residual must be 16-byte aligned" if mode == 2 else "C must be 16-byte aligned"):
+        ops.gemm(a, b, out, accumulate=mode == 1, residual=residual)
     torch.cuda.synchronize()
-    assert torch.equal(out, want)
-    assert torch.isnan(buf[:, :4].float()).all() and torch.isnan(buf[:, N + 4:].float()).all()
+    assert torch.isnan(buf.float()).all()
 
 
 def test_in_place_accumulate_into_live_gradient_buffer():
@@ -166,9 +166,11 @@ def test_in_place_accumulate_into_live_gradient_buffer():
     assert torch.equal(flat[: h * N], before[: h * N]) and torch.equal(flat[2 * h * N:], before[2 * h * N:])
 
 
-@pytest.mark.parametrize("M,h,inter", [(4096, 3072, 8192), (8192, 1536, 8960), (4095, 1000, 4160)])
+@pytest.mark.parametrize("M,h,inter", [(4096, 3072, 8192), (8192, 1536, 8960), (4095, 1000, 4160), (5, 4096, 14336),
+                                       (64, 1000, 4160)])
 def test_swiglu_fwd_fused_equals_unfused(M, h, inter):
-    """Mode 4: gate|up and m equal the plain GEMM followed by swiglu_fwd (4160 channels: the last n-tile has 64)."""
+    """Mode 4: gate|up and m equal the plain GEMM followed by swiglu_fwd (4160 channels: the last n-tile has 64; M <= 64: 64-row
+    tiles, as the decode step's ffn1, which stores m only)."""
     ops = _ops()
     x, w = _rand(M, h, seed=61), _rand(h, 2 * inter, scale=0.05, seed=62)
     gu = torch.full((M, 2 * inter), float("nan"), dtype=BF16, device=DEV)
@@ -183,7 +185,8 @@ def test_swiglu_fwd_fused_equals_unfused(M, h, inter):
     assert torch.equal(m_only, m_ref)
 
 
-@pytest.mark.parametrize("M,h,inter", [(4096, 3072, 8192), (8192, 1536, 8960), (4095, 1000, 4160)])
+@pytest.mark.parametrize("M,h,inter", [(4096, 3072, 8192), (8192, 1536, 8960), (4095, 1000, 4160), (5, 3072, 8192),
+                                       (64, 1000, 4160)])
 def test_swiglu_bwd_fused_equals_unfused(M, h, inter):
     """Mode 5: d(gate)|d(up) equals the plain dX GEMM followed by swiglu_bwd."""
     ops = _ops()
