@@ -176,6 +176,13 @@ int b200_ce_fwd(const void* logits, const int64_t* labels, float* loss_tok, floa
 int b200_ce_bwd(void* logits_inout, const int64_t* labels, const float* loss_tok, const float* lse,
                 const float* loss_out, float grad_scale, const float* grad_scale_dev, int64_t tokens, int64_t vocab,
                 int64_t ld, cudaStream_t stream);
+/* Evaluation row pass over rows [row0, row0 + rows): `logits` points at row row0 (row stride ld); labels, loss_tok and pred
+ * are indexed by absolute row.  One read of each row gives loss_tok (bit-identical to b200_ce_fwd's) and, when pred is not
+ * null, pred (bit-identical to b200_argmax_bf16's).  No lse, no reduction: b200_ce_reduce then gives b200_ce_fwd's
+ * loss_out over all rows, so the logits can be produced and consumed a chunk of rows at a time. */
+int b200_ce_rows_fwd(const void* logits, const int64_t* labels, float* loss_tok, int64_t* pred, int64_t row0, int64_t rows,
+                     int64_t vocab, int64_t ld, int64_t ignore_index, cudaStream_t stream);
+int b200_ce_reduce(const float* loss_tok, float* loss_out, int64_t tokens, cudaStream_t stream);
 /* Greedy token choice: first maximal index of each bf16 row (generation_utils.py:291-363 with top_p = 0). */
 int b200_argmax_bf16(const void* logits, int64_t* out, int64_t rows, int64_t vocab, int64_t ld, cudaStream_t stream);
 

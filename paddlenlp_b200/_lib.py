@@ -50,6 +50,8 @@ _SIGNATURES = {
     "b200_fa_bwd": [P, P, P, P, P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I64, I64, I64, I64, I64, I64, F, P],
     "b200_ce_fwd": [P, P, P, P, P, I64, I64, I64, I64, P],
     "b200_ce_bwd": [P, P, P, P, P, F, P, I64, I64, I64, P],
+    "b200_ce_rows_fwd": [P, P, P, P, I64, I64, I64, I64, I64, P],
+    "b200_ce_reduce": [P, P, I64, P],
     "b200_argmax_bf16": [P, P, I64, I64, I64, P],
     "b200_grad_sqnorm_workspace_bytes": [],
     "b200_grad_sqnorm": [P, P, P, I64, F, P],
@@ -127,7 +129,7 @@ class B200Error(RuntimeError):
 KERNELS_PER_CALL = {
     "b200_gemm_bf16": 1, "b200_gemm_bf16_ex": 1, "b200_gemm_bf16_splitk": 2, "b200_rmsnorm_fwd": 1, "b200_rmsnorm_bwd": 2, "b200_colsum_bf16": 2,
     "b200_rope_inplace": 1, "b200_swiglu_fwd": 1, "b200_swiglu_bwd": 1, "b200_embedding_fwd": 1, "b200_embedding_bwd": 1,
-    "b200_fa_fwd": 1, "b200_fa_bwd": 5, "b200_fa_fwd_flashmask": 1, "b200_fa_bwd_flashmask": 5, "b200_ce_fwd": 2, "b200_ce_bwd": 1, "b200_argmax_bf16": 1, "b200_grad_sqnorm": 2,
+    "b200_fa_fwd": 1, "b200_fa_bwd": 5, "b200_fa_fwd_flashmask": 1, "b200_fa_bwd_flashmask": 5, "b200_ce_fwd": 2, "b200_ce_bwd": 1, "b200_ce_rows_fwd": 1, "b200_ce_reduce": 1, "b200_argmax_bf16": 1, "b200_grad_sqnorm": 2,
     "b200_adamw_step": 1, "b200_bf16_to_f32": 1, "b200_token_penalty_multi_scores": 2, "b200_generate_step_update": 2, "b200_decode_attention": 2, "b200_decode_attention_tc": 2, "b200_decode_attention_paged": 2, "b200_append_attention": 5,
 }
 launch_count = 0       # kernels launched through this module since import

@@ -18,21 +18,36 @@ __device__ __forceinline__ void online_merge(float& m, float& s, float m2, float
   m = nm;
 }
 
-// One CTA per token row.  Single pass online logsumexp over the bf16 row.
+// arg-max step with argmax_kernel's order: larger value wins, the lower index wins a tie, NaN never wins.
+__device__ __forceinline__ void argmax_take(float& best, int& bi, float v, int i) {
+  if (v > best || (v == best && i < bi)) { best = v; bi = i; }
+}
+
+// One CTA per token row.  Single pass online logsumexp over the bf16 row.  ARGMAX: the same pass also keeps the row's
+// first maximal index (pred[row], equal to argmax_kernel's).  LSE: write lse_out (only the backward needs it).
+template <bool ARGMAX, bool LSE>
 __global__ void __launch_bounds__(256) ce_fwd_kernel(const bf16* __restrict__ logits, const int64_t* __restrict__ labels,
                                                      float* __restrict__ loss_tok, float* __restrict__ lse_out,
-                                                     int vocab, int64_t ld, int ignore_index) {
+                                                     int64_t* __restrict__ pred, int vocab, int64_t ld, int ignore_index) {
   __shared__ float sm[8], ss[8];
+  __shared__ float sbest[8];
+  __shared__ int sbi[8];
   const int row = blockIdx.x;
   const bf16* lr = logits + static_cast<size_t>(row) * ld;
   const int nchunk = vocab >> 3;
   float m = -INFINITY, s = 0.f;
+  float best = -INFINITY;
+  int bi = 0x7fffffff;
   for (int c = threadIdx.x; c < nchunk; c += blockDim.x) {
     const uint4 v = ld_nc_v4(reinterpret_cast<const uint4*>(lr) + c);
     const uint32_t* vi = reinterpret_cast<const uint32_t*>(&v);
     float f[8];
 #pragma unroll
     for (int j = 0; j < 4; ++j) { const float2 t = unpack_bf16x2(vi[j]); f[2 * j] = t.x; f[2 * j + 1] = t.y; }
+    if (ARGMAX) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) argmax_take(best, bi, f[j], c * 8 + j);
+    }
     float cm = f[0];
 #pragma unroll
     for (int j = 1; j < 8; ++j) cm = fmaxf(cm, f[j]);
@@ -45,6 +60,7 @@ __global__ void __launch_bounds__(256) ce_fwd_kernel(const bf16* __restrict__ lo
   }
   for (int i = (nchunk << 3) + threadIdx.x; i < vocab; i += blockDim.x) {  // tail (vocab % 8)
     const float f = __bfloat162float(lr[i]);
+    if (ARGMAX) argmax_take(best, bi, f, i);
     const float nm = fmaxf(m, f);
     s = s * __expf(m - nm) + __expf(f - nm);
     m = nm;
@@ -53,9 +69,17 @@ __global__ void __launch_bounds__(256) ce_fwd_kernel(const bf16* __restrict__ lo
   for (int o = 16; o > 0; o >>= 1) {
     const float m2 = __shfl_xor_sync(0xffffffffu, m, o), s2 = __shfl_xor_sync(0xffffffffu, s, o);
     online_merge(m, s, m2, s2);
+    if (ARGMAX) {
+      const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+      argmax_take(best, bi, ob, oi);
+    }
   }
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (lane == 0) { sm[warp] = m; ss[warp] = s; }
+  if (lane == 0) {
+    sm[warp] = m; ss[warp] = s;
+    if (ARGMAX) { sbest[warp] = best; sbi[warp] = bi; }
+  }
   __syncthreads();
   if (warp == 0) {
     m = lane < (blockDim.x >> 5) ? sm[lane] : -INFINITY;
@@ -65,9 +89,13 @@ __global__ void __launch_bounds__(256) ce_fwd_kernel(const bf16* __restrict__ lo
       const float m2 = __shfl_xor_sync(0xffffffffu, m, o), s2 = __shfl_xor_sync(0xffffffffu, s, o);
       online_merge(m, s, m2, s2);
     }
+    if (ARGMAX && lane == 0) {
+      for (int w = 1; w < (blockDim.x >> 5); ++w) argmax_take(best, bi, sbest[w], sbi[w]);
+      pred[row] = bi;
+    }
     if (lane == 0) {
       const float lse = m + logf(s);
-      lse_out[row] = lse;
+      if (LSE) lse_out[row] = lse;
       const int64_t lab = labels[row];
       float l = 0.f;
       if (lab != ignore_index && lab >= 0 && lab < vocab) l = lse - __bfloat162float(lr[lab]);
@@ -289,12 +317,33 @@ extern "C" int b200_ce_fwd(const void* logits, const int64_t* labels, float* los
                            int64_t tokens, int64_t vocab, int64_t ld, int64_t ignore_index, cudaStream_t stream) {
   B200_CHECK_ARG(logits && labels && loss_tok && lse && loss_out, "ce_fwd: null pointer");
   B200_CHECK_ARG(tokens > 0 && vocab > 0 && ld % 8 == 0, "ce_fwd: ld must be a multiple of 8");
-  ce_fwd_kernel<<<static_cast<unsigned>(tokens), 256, 0, stream>>>(static_cast<const bf16*>(logits), labels, loss_tok, lse,
-                                                                  (int)vocab, ld, (int)ignore_index);
+  ce_fwd_kernel<false, true><<<static_cast<unsigned>(tokens), 256, 0, stream>>>(
+      static_cast<const bf16*>(logits), labels, loss_tok, lse, nullptr, (int)vocab, ld, (int)ignore_index);
   int rc = check_launch("ce_fwd");
   if (rc) return rc;
   ce_reduce_kernel<<<1, 1024, 0, stream>>>(loss_tok, loss_out, tokens);
   return check_launch("ce_fwd(reduce)");
+}
+
+extern "C" int b200_ce_rows_fwd(const void* logits, const int64_t* labels, float* loss_tok, int64_t* pred, int64_t row0,
+                                int64_t rows, int64_t vocab, int64_t ld, int64_t ignore_index, cudaStream_t stream) {
+  B200_CHECK_ARG(logits && labels && loss_tok, "ce_rows_fwd: null pointer");
+  B200_CHECK_ARG(row0 >= 0 && rows > 0 && vocab > 0 && ld % 8 == 0 && (reinterpret_cast<uintptr_t>(logits) & 15) == 0,
+                 "ce_rows_fwd: ld must be a multiple of 8 and logits 16-byte aligned");
+  const bf16* lg = static_cast<const bf16*>(logits);
+  if (pred != nullptr)
+    ce_fwd_kernel<true, false><<<static_cast<unsigned>(rows), 256, 0, stream>>>(
+        lg, labels + row0, loss_tok + row0, nullptr, pred + row0, (int)vocab, ld, (int)ignore_index);
+  else
+    ce_fwd_kernel<false, false><<<static_cast<unsigned>(rows), 256, 0, stream>>>(
+        lg, labels + row0, loss_tok + row0, nullptr, nullptr, (int)vocab, ld, (int)ignore_index);
+  return check_launch("ce_rows_fwd");
+}
+
+extern "C" int b200_ce_reduce(const float* loss_tok, float* loss_out, int64_t tokens, cudaStream_t stream) {
+  B200_CHECK_ARG(loss_tok && loss_out && tokens > 0, "ce_reduce: bad arguments");
+  ce_reduce_kernel<<<1, 1024, 0, stream>>>(loss_tok, loss_out, tokens);
+  return check_launch("ce_reduce");
 }
 
 extern "C" int b200_ce_bwd(void* logits_inout, const int64_t* labels, const float* loss_tok, const float* lse,

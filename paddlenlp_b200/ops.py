@@ -407,6 +407,32 @@ def ce_fwd(logits: torch.Tensor, labels: torch.Tensor, ignore_index: int = -100)
     return loss_out, loss_tok, lse
 
 
+def ce_rows_fwd(logits: torch.Tensor, labels: torch.Tensor, loss_tok: torch.Tensor, pred: Optional[torch.Tensor] = None,
+                row0: int = 0, ignore_index: int = -100):
+    """Evaluation row pass: `logits` [rows, V] holds rows [row0, row0 + rows) of a [T, V] logits matrix; fills
+    loss_tok[row0:row0 + rows] (fp32 [T], as ce_fwd's loss_tok) and, if given, pred[row0:row0 + rows] (int64 [T], as
+    argmax) from one read of those rows."""
+    _chk(logits, "logits"); _chk(labels, "labels", torch.int64); _chk(loss_tok, "loss_tok", torch.float32)
+    rows, V = logits.shape
+    T = labels.numel()
+    assert logits.stride(1) == 1 and labels.is_contiguous() and loss_tok.is_contiguous() and loss_tok.numel() == T
+    assert 0 <= row0 and row0 + rows <= T
+    if pred is not None:
+        _chk(pred, "pred", torch.int64)
+        assert pred.is_contiguous() and pred.numel() == T
+    call("b200_ce_rows_fwd", ptr(logits), ptr(labels), ptr(loss_tok), ptr(pred), row0, rows, V, logits.stride(0),
+         ignore_index, stream_ptr())
+
+
+def ce_reduce(loss_tok: torch.Tensor) -> torch.Tensor:
+    """loss_out [2] = (masked mean of loss_tok over l > 0, count): ce_fwd's reduction."""
+    _chk(loss_tok, "loss_tok", torch.float32)
+    assert loss_tok.dim() == 1 and loss_tok.is_contiguous()
+    loss_out = torch.empty(2, dtype=torch.float32, device=loss_tok.device)
+    call("b200_ce_reduce", ptr(loss_tok), ptr(loss_out), loss_tok.numel(), stream_ptr())
+    return loss_out
+
+
 def ce_bwd_(logits: torch.Tensor, labels: torch.Tensor, loss_tok, lse, loss_out, grad_scale: float = 1.0,
             grad_scale_dev: Optional[torch.Tensor] = None):
     """Overwrites logits with dlogits.  grad_scale_dev: optional fp32 device scalar multiplied into grad_scale."""

@@ -6,7 +6,9 @@ Call pattern reproduced (SURVEY.md §3.1):
        training_step                :2211  (H2D of the batch, bf16 O2 forward, loss / grad_accum, loss.backward())
        gradient exchange            :1934-1954 / :1079-1110  -> ONE all-reduce of the flat gradient buffer
        optimizer.step / lr_scheduler.step / optimizer.clear_grad     :1171-1185
-       _maybe_log_save_evaluate     :1388-1455 (all-gathered mean loss, speed_metrics keys of trainer_utils.py:351-380)
+       _maybe_log_save_evaluate     :1388-1455 (all-gathered mean loss, speed_metrics keys of trainer_utils.py:351-380;
+                                    evaluate() every eval_steps or at epoch end, then the checkpoint keeps the best metric)
+    .evaluate() / .predict()        :2846-3286 (evaluation_loop, prediction_step)
 Differences by design: the whole model's gradients live in one buffer, so there are no reducer buckets; gradient
 averaging (1/world) is folded into the optimizer kernel; the step is host-sync free except at logging steps.
 """
@@ -23,10 +25,13 @@ import time
 from dataclasses import dataclass
 from typing import Any, Callable, Dict, List, Optional
 
+import numpy as np
 import torch
 
 from .. import distributed as dist_env
 from ..optimizer import AdamW, ClipGradByGlobalNorm, get_scheduler
+from ..utils.batch_sampler import DistributedBatchSampler
+from .trainer_utils import EvalLoopOutput, EvalPrediction, IntervalStrategy, PredictionOutput
 from .training_args import TrainingArguments
 
 
@@ -42,6 +47,7 @@ class TrainerCallback:
     def on_step_begin(self, args, state, control, **kw): ...
     def on_step_end(self, args, state, control, **kw): ...
     def on_log(self, args, state, control, logs=None, **kw): ...
+    def on_evaluate(self, args, state, control, metrics=None, **kw): ...
     def on_train_end(self, args, state, control, **kw): ...
 
 
@@ -189,6 +195,28 @@ def speed_metrics(split, start_time, num_samples=None, num_steps=None, seq_lengt
     return result
 
 
+def _pad_concat(a: Optional[np.ndarray], b: np.ndarray, padding_index: int = -100) -> np.ndarray:
+    """trainer_utils nested_concat: concatenate along the batch axis, right-padding axis 1 with padding_index when the
+    sequence lengths differ."""
+    if a is None:
+        return b
+    if a.ndim == 1 or a.shape[1] == b.shape[1]:
+        return np.concatenate((a, b), axis=0)
+    shape = (a.shape[0] + b.shape[0], max(a.shape[1], b.shape[1])) + a.shape[2:]
+    out = np.full(shape, padding_index, dtype=a.dtype)
+    out[:a.shape[0], :a.shape[1]] = a
+    out[a.shape[0]:, :b.shape[1]] = b
+    return out
+
+
+def _batch_size(inputs) -> Optional[int]:
+    """trainer_utils find_batch_size: leading dimension of the first tensor of a batch."""
+    for v in (inputs.values() if isinstance(inputs, dict) else inputs):
+        if isinstance(v, torch.Tensor) and v.dim() > 0:
+            return v.shape[0]
+    return None
+
+
 def default_data_collator(features: List[Dict[str, Any]]) -> Dict[str, torch.Tensor]:
     out = {}
     for k in features[0]:
@@ -209,6 +237,7 @@ class Trainer:
         self.train_dataset = train_dataset
         self.eval_dataset = eval_dataset
         self.tokenizer = tokenizer
+        self.compute_metrics = compute_metrics
         self.optimizer, self.lr_scheduler = optimizers
         self.callbacks = list(callbacks or []) + [PrinterCallback()]
         self.state = TrainerState(log_history=[])
@@ -352,6 +381,8 @@ class Trainer:
         if resume_from_checkpoint:
             self._load_from_checkpoint(resume_from_checkpoint)
         dl = self.get_train_dataloader()
+        if a.evaluation_strategy != IntervalStrategy.NO and self.eval_dataset is None:
+            raise ValueError(f"evaluation_strategy={a.evaluation_strategy}: training with evaluation requires an eval_dataset")
         accum = max(1, a.gradient_accumulation_steps)
         try:
             steps_per_epoch = max(len(dl) // accum, 1)
@@ -474,14 +505,24 @@ class Trainer:
                     logged_step = gs
                     t_log = time.time()
                     self.log(logs)
-                if a.save_strategy == "steps" and a.save_steps > 0 and gs % a.save_steps == 0:
-                    self._save_checkpoint(model)
+                metrics = None
+                if a.evaluation_strategy == IntervalStrategy.STEPS and gs % a.eval_steps == 0:
+                    metrics = self.evaluate()
+                if a.save_strategy == IntervalStrategy.STEPS and a.save_steps > 0 and gs % a.save_steps == 0:
+                    self._save_checkpoint(model, metrics=metrics)
                 if gs >= max_steps:
                     done = True
                     break
+            metrics = None                                       # trainer_callback.py:463-474: epoch-end events
+            if a.evaluation_strategy == IntervalStrategy.EPOCH:
+                metrics = self.evaluate()
+            if a.save_strategy == IntervalStrategy.EPOCH:
+                self._save_checkpoint(model, metrics=metrics)
             if done:
                 break
         torch.cuda.synchronize(dev)
+        if a.load_best_model_at_end and self.state.best_model_checkpoint is not None:    # trainer.py:1231-1260
+            self._load_from_checkpoint(self.state.best_model_checkpoint)
         if self.state.global_step > logged_step:
             loss_t = tr_loss.clone()
             if world > 1:
@@ -496,6 +537,201 @@ class Trainer:
         for cb in self.callbacks:
             cb.on_train_end(a, self.state, self.control)
         return TrainOutput(self.state.global_step, logged_loss_total / gs, metrics)
+
+    # ------------------------------------------------------------------------------------------------
+    # evaluation  (trainer.py:1555-1660 eval / test dataloaders, :2846-3286 evaluate, predict, evaluation_loop,
+    # prediction_step)
+    # ------------------------------------------------------------------------------------------------
+    def _get_eval_sampler(self, eval_dataset):
+        """Every sample once, in order: sequential batches for one process; across ranks, DistributedBatchSampler without
+        shuffling, whose last global batch wraps around to the first samples (evaluation_loop truncates them away)."""
+        a = self.args
+        if a.dataset_world_size <= 1:
+            return torch.utils.data.BatchSampler(torch.utils.data.SequentialSampler(eval_dataset),
+                                                 batch_size=a.per_device_eval_batch_size, drop_last=False)
+        return DistributedBatchSampler(eval_dataset, batch_size=a.per_device_eval_batch_size, num_replicas=a.dataset_world_size,
+                                       rank=a.dataset_rank, shuffle=False, drop_last=False)
+
+    def _eval_dataloader(self, ds):
+        a = self.args
+        if isinstance(ds, torch.utils.data.IterableDataset):
+            if a.dataset_world_size > 1:
+                ds = IterableDatasetShard(ds, batch_size=a.per_device_eval_batch_size, drop_last=a.dataloader_drop_last,
+                                          num_processes=a.dataset_world_size, process_index=a.dataset_rank)
+            return torch.utils.data.DataLoader(ds, batch_size=a.per_device_eval_batch_size, collate_fn=self.data_collator)
+        return torch.utils.data.DataLoader(ds, batch_sampler=self._get_eval_sampler(ds), collate_fn=self.data_collator,
+                                           num_workers=a.dataloader_num_workers)
+
+    def get_eval_dataloader(self, eval_dataset=None):
+        if eval_dataset is None and self.eval_dataset is None:
+            raise ValueError("Trainer: evaluation requires an eval_dataset.")
+        return self._eval_dataloader(eval_dataset if eval_dataset is not None else self.eval_dataset)
+
+    def get_test_dataloader(self, test_dataset):
+        if test_dataset is None:
+            raise ValueError("Trainer: prediction requires a test_dataset.")
+        return self._eval_dataloader(test_dataset)
+
+    def evaluate(self, eval_dataset=None, ignore_keys: Optional[List[str]] = None, metric_key_prefix: str = "eval"):
+        """Loss (and `compute_metrics` of the predictions, when given) over the evaluation set; logged and returned."""
+        dl = self.get_eval_dataloader(eval_dataset)
+        start = time.time()
+        output = self.evaluation_loop(dl, description="Evaluation",
+                                      prediction_loss_only=True if self.compute_metrics is None else None,
+                                      ignore_keys=ignore_keys, metric_key_prefix=metric_key_prefix,
+                                      max_eval_iters=self.args.max_evaluate_steps)
+        total_batch = self.args.eval_batch_size * self.args.dataset_world_size
+        output.metrics.update(speed_metrics(metric_key_prefix, start, num_samples=output.num_samples,
+                                            num_steps=math.ceil(output.num_samples / total_batch)))
+        self.log(output.metrics)
+        self.state.log_history[-1].setdefault("global_step", self.state.global_step)
+        for cb in self.callbacks:
+            cb.on_evaluate(self.args, self.state, self.control, metrics=output.metrics)
+        return output.metrics
+
+    def predict(self, test_dataset, ignore_keys: Optional[List[str]] = None, metric_key_prefix: str = "test"):
+        dl = self.get_test_dataloader(test_dataset)
+        start = time.time()
+        output = self.evaluation_loop(dl, description="Prediction", ignore_keys=ignore_keys,
+                                      prediction_loss_only=True if self.compute_metrics is None else None,
+                                      metric_key_prefix=metric_key_prefix, max_eval_iters=self.args.max_evaluate_steps)
+        total_batch = self.args.per_device_eval_batch_size * self.args.dataset_world_size
+        output.metrics.update(speed_metrics(metric_key_prefix, start, num_samples=output.num_samples,
+                                            num_steps=math.ceil(output.num_samples / total_batch)))
+        return PredictionOutput(predictions=output.predictions, label_ids=output.label_ids, metrics=output.metrics)
+
+    def _nested_gather(self, t: torch.Tensor) -> torch.Tensor:
+        """Concatenation over ranks (rank order) along axis 0; every rank passes the same shape."""
+        world = self.args.world_size
+        if world <= 1:
+            return t
+        parts = [torch.empty_like(t) for _ in range(world)]
+        torch.distributed.all_gather(parts, t.contiguous())
+        return torch.cat(parts, dim=0)
+
+    def _pad_across_processes(self, t: torch.Tensor, padding_index: int = -100) -> torch.Tensor:
+        """Right-pad axis 1 to the longest sequence of any rank, so that _nested_gather can stack the batches."""
+        if self.args.world_size <= 1 or t.dim() < 2:
+            return t
+        n = torch.tensor([t.shape[1]], device=t.device)
+        torch.distributed.all_reduce(n, op=torch.distributed.ReduceOp.MAX)
+        n = int(n.item())
+        if n == t.shape[1]:
+            return t
+        out = t.new_full((t.shape[0], n) + tuple(t.shape[2:]), padding_index)
+        out[:, :t.shape[1]] = t
+        return out
+
+    def evaluation_loop(self, dataloader, description: str, prediction_loss_only: Optional[bool] = None,
+                        ignore_keys: Optional[List[str]] = None, metric_key_prefix: str = "eval",
+                        max_eval_iters: Optional[int] = -1) -> EvalLoopOutput:
+        """trainer.py:3016-3104.  Each batch's loss, repeated batch-size times, is gathered over the ranks; predictions and
+        labels are gathered, padded with -100 and concatenated in sample order.  All three are truncated to num_samples
+        (len(dataset), or batch * world * max_eval_iters when the iterations are capped), so the samples the sampler
+        repeats to even out the ranks are dropped, and eval_loss is the mean of what remains.  The losses stay on the
+        device until that mean: a loss-only evaluation synchronises once."""
+        a = self.args
+        prediction_loss_only = prediction_loss_only if prediction_loss_only is not None else a.prediction_loss_only
+        max_eval_iters = max_eval_iters if max_eval_iters is not None else -1
+        model = self.model
+        batch_size = getattr(dataloader.batch_sampler, "batch_size", None) or dataloader.batch_size
+        world = a.dataset_world_size
+        num_samples = batch_size * world * max_eval_iters if max_eval_iters > 0 else None
+        losses: List[torch.Tensor] = []
+        all_preds = all_labels = None
+        observed = 0
+        model.eval()
+        # evaluation draws nothing from the host RNG that training may use (the DataLoader seeds itself from it)
+        with torch.random.fork_rng(devices=[]):
+            for step, inputs in enumerate(dataloader):
+                bs = _batch_size(inputs)
+                if bs is not None:
+                    observed += bs
+                    batch_size = bs
+                loss, logits, labels = self.prediction_step(model, inputs, prediction_loss_only, ignore_keys=ignore_keys)
+                if loss is not None:
+                    losses.append(self._nested_gather(loss.detach().float().reshape(1).repeat(batch_size)))
+                if labels is not None:
+                    labels = self._nested_gather(self._pad_across_processes(labels.detach()))
+                    all_labels = _pad_concat(all_labels, labels.cpu().numpy())
+                if logits is not None:
+                    logits = self._nested_gather(self._pad_across_processes(logits.detach()))
+                    all_preds = _pad_concat(all_preds, logits.float().cpu().numpy() if logits.is_floating_point()
+                                            else logits.cpu().numpy())
+                if max_eval_iters > 0 and step >= max_eval_iters - 1:
+                    break
+        model.train()
+        if num_samples is None:
+            try:
+                num_samples = len(dataloader.dataset)
+            except TypeError:                                    # an iterable dataset: what the ranks saw
+                num_samples = observed * world
+        if all_preds is not None:
+            all_preds = all_preds[:num_samples]
+        if all_labels is not None:
+            all_labels = all_labels[:num_samples]
+        metrics = {}
+        if self.compute_metrics is not None and all_preds is not None and all_labels is not None:
+            metrics = dict(self.compute_metrics(EvalPrediction(predictions=all_preds, label_ids=all_labels)))
+        if losses:
+            metrics[f"{metric_key_prefix}_loss"] = torch.cat(losses)[:num_samples].double().mean().item()
+        for key in list(metrics):
+            if not key.startswith(f"{metric_key_prefix}_"):
+                metrics[f"{metric_key_prefix}_{key}"] = metrics.pop(key)
+        return EvalLoopOutput(predictions=all_preds, label_ids=all_labels, metrics=metrics, num_samples=num_samples)
+
+    def _fused_eval_ignore_index(self) -> Optional[int]:
+        """ignore_index of the built-in pre-training criterion when it computes the loss (no criterion, or a
+        LlamaPretrainingCriterion / Qwen2PretrainingCriterion), else None: a custom criterion needs the logits."""
+        from ..transformers.llama.modeling import LlamaPretrainingCriterion
+
+        inner = getattr(self.model, "_layers", self.model)
+        if self._engine() is None or not isinstance(getattr(inner, "criterion", None), LlamaPretrainingCriterion):
+            return None
+        if self.criterion is None:
+            return inner.criterion.ignore_index
+        return self.criterion.ignore_index if isinstance(self.criterion, LlamaPretrainingCriterion) else None
+
+    def _forward_eval(self, inputs, ignore_index: int, predictions: bool):
+        """engine.forward_eval on a prepared batch: (loss_out [2], preds [B, S] or None), on the device."""
+        from ..transformers.llama.modeling import _resolve_mask
+
+        ms = _resolve_mask(inputs.get("attention_mask"), inputs.get("attn_mask_startend_row_indices"))
+        return self._engine().forward_eval(inputs["input_ids"], inputs["labels"], inputs.get("position_ids"), ignore_index,
+                                           attn_mask_startend_row_indices=ms, predictions=predictions)
+
+    def prediction_step(self, model, inputs, prediction_loss_only: bool, ignore_keys: Optional[List[str]] = None):
+        """(loss, logits, labels) of one batch, each optional.  With the built-in criterion a loss-only step runs the
+        engine's chunked evaluation forward (no [T, V] logits); otherwise the model forward (or compute_loss with a
+        custom criterion) under no_grad."""
+        has_labels = inputs.get("labels") is not None
+        inputs = self._prepare_inputs(inputs)
+        labels = inputs["labels"] if has_labels else None
+        ignore_keys = list(ignore_keys or [])
+        with torch.no_grad():
+            if has_labels and prediction_loss_only:
+                ign = self._fused_eval_ignore_index()
+                if ign is not None:
+                    loss_out, _ = self._forward_eval(inputs, ign, predictions=False)
+                    return loss_out[0], None, None
+            if has_labels:
+                loss, outputs = self.compute_loss(model, inputs, return_outputs=True)
+                loss = loss.mean().detach()
+                if isinstance(outputs, dict):
+                    logits = tuple(v for k, v in outputs.items() if k not in ignore_keys + ["loss"] and v is not None)
+                else:
+                    logits = tuple(outputs[1:])
+            else:
+                loss = None
+                outputs = model(**inputs)
+                if isinstance(outputs, dict):
+                    logits = tuple(v for k, v in outputs.items() if k not in ignore_keys and v is not None)
+                else:
+                    logits = tuple(outputs) if isinstance(outputs, (tuple, list)) else (outputs,)
+        if prediction_loss_only:
+            return loss, None, None
+        logits = logits[0] if len(logits) == 1 else logits
+        return loss, logits, labels
 
     def log_metrics(self, split: str, metrics: Dict[str, float]):
         """trainer_utils.py log_metrics: formatted dump of a metrics dict (rank 0)."""
@@ -547,6 +783,13 @@ class Trainer:
         a = self.args
         out = os.path.join(a.output_dir, f"{PREFIX_CHECKPOINT_DIR}-{self.state.global_step}")
         world = a.world_size
+        if metrics is not None and a.metric_for_best_model is not None:          # trainer.py:2463-2477
+            key = a.metric_for_best_model if a.metric_for_best_model.startswith("eval_") else f"eval_{a.metric_for_best_model}"
+            value = metrics[key]
+            better = np.greater if a.greater_is_better else np.less
+            if self.state.best_metric is None or self.state.best_model_checkpoint is None or better(value, self.state.best_metric):
+                self.state.best_metric = value
+                self.state.best_model_checkpoint = out
         rng = self._rng_states()
         if world > 1:                                            # trainer.py:2495-2500: one list entry per rank
             rng_list = [None] * world
@@ -580,7 +823,8 @@ class Trainer:
         return out
 
     def _rotate_checkpoints(self):
-        """trainer.py:2549-2576: keep the newest `save_total_limit` checkpoint-N directories."""
+        """trainer.py:2549-2585: keep the newest `save_total_limit` checkpoint-N directories, and never the best one: it
+        is moved to second-newest, and with a limit of 1 the newest is kept too (so that training can resume)."""
         limit = self.args.save_total_limit
         if not limit or limit <= 0:
             return
@@ -588,9 +832,16 @@ class Trainer:
         for name in os.listdir(self.args.output_dir):
             m = re.fullmatch(PREFIX_CHECKPOINT_DIR + r"-(\d+)", name)
             if m:
-                found.append((int(m.group(1)), name))
-        for _, name in sorted(found)[:-limit]:
-            shutil.rmtree(os.path.join(self.args.output_dir, name), ignore_errors=True)
+                found.append((int(m.group(1)), os.path.join(self.args.output_dir, name)))
+        paths = [p for _, p in sorted(found)]
+        best = self.state.best_model_checkpoint
+        if best is not None and best in paths:
+            i = paths.index(best)
+            paths.insert(max(i, len(paths) - 2), paths.pop(i))
+            if limit == 1 and paths[-1] != best:
+                limit = 2
+        for path in paths[:max(0, len(paths) - limit)]:
+            shutil.rmtree(path, ignore_errors=True)
 
     def _load_from_checkpoint(self, checkpoint: str):
         from ..transformers import conversion_utils as cu

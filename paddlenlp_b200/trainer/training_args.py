@@ -12,6 +12,7 @@ from dataclasses import asdict, dataclass, field
 from typing import Optional
 
 from .. import distributed as dist_env
+from .trainer_utils import IntervalStrategy
 
 
 class _SchedulerName(str):
@@ -46,7 +47,17 @@ class TrainingArguments:
     logging_steps: int = 500
     logging_first_step: bool = False
     save_steps: int = 0
-    save_strategy: str = "steps"
+    save_strategy: str = "steps"                  # "no" / "steps" (every save_steps) / "epoch"
+    # evaluation (training_args.py:396-420, 739-779): defaults and __post_init__ rules of the reference
+    evaluation_strategy: str = "no"               # "no" / "steps" (every eval_steps) / "epoch"
+    eval_steps: Optional[int] = None              # falls back to logging_steps
+    per_device_eval_batch_size: int = 8
+    eval_accumulation_steps: Optional[int] = None  # accepted; predictions are moved to the host after every batch
+    prediction_loss_only: bool = False
+    max_evaluate_steps: int = -1                  # > 0: evaluate on that many batches per process only
+    load_best_model_at_end: bool = False
+    metric_for_best_model: Optional[str] = None
+    greater_is_better: Optional[bool] = None
     save_total_limit: Optional[int] = None
     resume_from_checkpoint: Optional[str] = None
     save_only_model: bool = False
@@ -67,7 +78,7 @@ class TrainingArguments:
     max_seq_length: Optional[int] = None
     # fields the reference's training scripts read (llm/run_pretrain.py:358-575); inert on the pure data-parallel path
     overwrite_output_dir: bool = False
-    do_eval: bool = False
+    do_eval: bool = False                         # True with evaluation_strategy "no" means "steps"
     do_predict: bool = False
     autotuner_benchmark: bool = False
     sequence_parallel: bool = False
@@ -104,6 +115,30 @@ class TrainingArguments:
         if self.sequence_parallel or self.enable_linear_fused_grad_add:
             raise NotImplementedError("sequence_parallel / enable_linear_fused_grad_add belong to the tensor-parallel path")
         self.lr_scheduler_type = _SchedulerName(getattr(self.lr_scheduler_type, "value", self.lr_scheduler_type))
+        # training_args.py:926-970
+        self.evaluation_strategy = IntervalStrategy(self.evaluation_strategy)
+        self.save_strategy = IntervalStrategy(self.save_strategy)
+        if self.do_eval is False and self.evaluation_strategy != IntervalStrategy.NO:
+            self.do_eval = True
+        if self.do_eval and self.evaluation_strategy == IntervalStrategy.NO:
+            self.evaluation_strategy = IntervalStrategy.STEPS
+        if self.evaluation_strategy == IntervalStrategy.STEPS and not self.eval_steps:
+            if self.logging_steps > 0:
+                self.eval_steps = self.logging_steps
+            else:
+                raise ValueError(f"evaluation strategy {self.evaluation_strategy} requires either non-zero --eval_steps or "
+                                 "--logging_steps")
+        if self.load_best_model_at_end:
+            if self.evaluation_strategy != self.save_strategy:
+                raise ValueError("--load_best_model_at_end requires the save and eval strategy to match, but found\n- "
+                                 f"Evaluation strategy: {self.evaluation_strategy}\n- Save strategy: {self.save_strategy}")
+            if self.evaluation_strategy == IntervalStrategy.STEPS and self.save_steps % self.eval_steps != 0:
+                raise ValueError("--load_best_model_at_end requires the saving steps to be a round multiple of the evaluation "
+                                 f"steps, but found {self.save_steps}, which is not a round multiple of {self.eval_steps}.")
+        if self.load_best_model_at_end and self.metric_for_best_model is None:
+            self.metric_for_best_model = "loss"
+        if self.greater_is_better is None and self.metric_for_best_model is not None:
+            self.greater_is_better = self.metric_for_best_model not in ["loss", "eval_loss"]
         dist_env.init_parallel_env()
 
     def print_config(self, args=None, key=""):
@@ -149,12 +184,17 @@ class TrainingArguments:
         return self.per_device_train_batch_size
 
     @property
+    def eval_batch_size(self) -> int:
+        return self.per_device_eval_batch_size
+
+    @property
     def should_log(self) -> bool:
         return self.process_index == 0
 
     def to_dict(self):
         d = asdict(self)
-        d["lr_scheduler_type"] = str(self.lr_scheduler_type)
+        for k in ("lr_scheduler_type", "evaluation_strategy", "save_strategy"):
+            d[k] = str(d[k])
         return d
 
     def to_json_string(self):

@@ -31,6 +31,9 @@ import torch
 from .. import ops
 
 BF16 = torch.bfloat16
+# forward_eval() produces the logits at most this many bytes at a time (whole multiples of 128 rows), so evaluation never
+# holds the [T, V] logits: 4.98 GB at 8 x 2048 tokens of a 151 936-token vocabulary.
+EVAL_LOGITS_CHUNK_BYTES = 512 << 20
 
 
 def _align8(n: int) -> int:
@@ -328,11 +331,23 @@ class DecoderEngine:
         hf, rstd_f = ops.rmsnorm_fwd(x, self.p["norm"], self.eps)
         return B, S, ids, pos, x, hf, rstd_f
 
-    def _logits(self, hf: torch.Tensor) -> torch.Tensor:
+    def _logits(self, hf: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """[T, V] = hf @ head, or hf @ E^T when tied (E [V, h] is the GEMM's K-major B operand)."""
         if self.tied:
-            return ops.gemm(hf, self.p["embed"], trans_b=True)
-        return ops.gemm(hf, self.p["head"])
+            return ops.gemm(hf, self.p["embed"], out=out, trans_b=True)
+        return ops.gemm(hf, self.p["head"], out=out)
+
+    def _eval_chunks(self, T: int) -> List[Tuple[int, int]]:
+        """Row ranges [lo, hi) covering T rows, each at most EVAL_LOGITS_CHUNK_BYTES of logits and a multiple of 128 rows.
+        A tail of 64 rows or fewer joins the chunk before it: the GEMM picks 64-row tiles for M <= 64 and 128-row tiles
+        otherwise, so every chunk then runs the tiles of the unchunked GEMM, which never splits K, and each logit keeps
+        its bits."""
+        rows = max(128, EVAL_LOGITS_CHUNK_BYTES // (2 * self.V) // 128 * 128)
+        chunks = [(lo, min(T, lo + rows)) for lo in range(0, T, rows)]
+        if len(chunks) > 1 and chunks[-1][1] - chunks[-1][0] <= 64:
+            chunks.pop()
+            chunks[-1] = (chunks[-1][0], T)
+        return chunks
 
     @torch.no_grad()
     def forward_logits(self, input_ids, position_ids=None, attn_mask_startend_row_indices=None) -> torch.Tensor:
@@ -358,6 +373,32 @@ class DecoderEngine:
             self._saved = dict(B=B, S=S, ids=ids, pos=pos, mask=self._mask, layers=save, x_last=x, hf=hf, rstd_f=rstd_f, logits=logits,
                                labels=lab, loss_tok=loss_tok, lse=lse, loss_out=loss_out)
         return loss_out, logits.view(B, S, self.V)
+
+    @torch.no_grad()
+    def forward_eval(self, input_ids, labels, position_ids=None, ignore_index: int = -100,
+                     attn_mask_startend_row_indices=None, predictions: bool = True):
+        """Evaluation forward: (loss_out [2] = forward_loss's masked-mean loss and token count, preds [B, S] int64 = the
+        arg-max token of every position, or None when predictions=False), both on the device, without a host
+        synchronisation.  The head GEMM runs over chunks of rows into one reused logits buffer and one pass over each
+        row gives its loss and arg-max (reference llm_utils.py CausalLMTrainer.prediction_step takes the arg-max to avoid
+        gathering the logits), so the [T, V] logits never exist.  Loss and predictions are bit-identical to
+        forward_loss() + ops.argmax()."""
+        B, S, ids, pos, x, hf, _ = self.hidden_states(input_ids, position_ids, save=None,
+                                                      attn_mask_startend_row_indices=attn_mask_startend_row_indices)
+        del x
+        T = B * S
+        lab = labels.to(device=self.device, dtype=torch.int64, non_blocking=True).contiguous().view(-1)
+        if lab.numel() != T:
+            raise ValueError(f"labels have {lab.numel()} elements for {T} tokens")
+        loss_tok = torch.empty(T, dtype=torch.float32, device=self.device)
+        preds = torch.empty(T, dtype=torch.int64, device=self.device) if predictions else None
+        chunks = self._eval_chunks(T)
+        buf = torch.empty(max(hi - lo for lo, hi in chunks), self.V, dtype=BF16, device=self.device)
+        for lo, hi in chunks:
+            logits = self._logits(hf[lo:hi], out=buf[:hi - lo])
+            ops.ce_rows_fwd(logits, lab, loss_tok, preds, lo, ignore_index)
+        loss_out = ops.ce_reduce(loss_tok)
+        return loss_out, (preds.view(B, S) if predictions else None)
 
     @torch.no_grad()
     def forward_logits_train(self, input_ids, position_ids=None, attn_mask_startend_row_indices=None) -> torch.Tensor:
