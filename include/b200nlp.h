@@ -72,6 +72,13 @@ int b200_gemm_bf16(const void* A, const void* B, void* C, const float* bias, int
 int b200_gemm_bf16_ex(const void* A, const void* B, void* C, const float* bias, const void* residual, int64_t M,
                       int64_t N, int64_t K, int64_t lda, int64_t ldb, int64_t ldc, int64_t ldr, int a_mn_major,
                       int b_mn_major, int accumulate, int max_ctas, cudaStream_t stream);
+/* Same operands, fp32 output C [M, ldc] (fp32 master gradients, amp_master_grad; cf. fused_linear_param_grad_add(...,
+ * multi_precision=True), llm/utils/fused_layers.py:44-50):
+ *   accumulate == 0: C = acc ;  accumulate != 0: C += acc, one fp32 add per element (TMA reduce-add in L2; a subnormal sum
+ *   is flushed to zero).  No rounding to bf16 anywhere.
+ * Requires lda, ldb multiples of 8, ldc a multiple of 4 and >= N, A, B and C 16-byte aligned; any other is an argument error. */
+int b200_gemm_bf16_f32(const void* A, const void* B, float* C, int64_t M, int64_t N, int64_t K, int64_t lda, int64_t ldb,
+                       int64_t ldc, int a_mn_major, int b_mn_major, int accumulate, cudaStream_t stream);
 
 /* Weight-streaming GEMM for the decode step (M <= ~128 tokens): same math as b200_gemm_bf16 (C = op(A) op(B) + bias, one
  * rounding), but K is split over CTAs (split_k, 0 = auto) so that every SM streams part of the weight matrix; fp32 partial
@@ -111,12 +118,18 @@ int b200_rmsnorm_fwd(const void* x, const void* w, void* y, float* rstd, int64_t
 int64_t b200_rmsnorm_bwd_workspace_bytes(int64_t rows, int64_t h);
 int b200_rmsnorm_bwd(const void* dy, const void* x, const void* w, const float* rstd, const void* dres, void* dx,
                      void* dw, int accumulate_dw, void* workspace, int64_t rows, int64_t h, cudaStream_t stream);
+/* Same, dw an fp32 gradient (16-byte aligned): dw (+)= the fp32 column sums, never rounded to bf16. */
+int b200_rmsnorm_bwd_f32(const void* dy, const void* x, const void* w, const float* rstd, const void* dres, void* dx,
+                         float* dw, int accumulate_dw, void* workspace, int64_t rows, int64_t h, cudaStream_t stream);
 
 /* Column sums of a bf16 [rows, n] matrix (leading dimension ld) into a bf16 vector: bias gradients of Qwen2 q/k/v
  * (qwen2/modeling.py:478-480).  workspace: b200_colsum_workspace_bytes(rows, n). */
 int64_t b200_colsum_workspace_bytes(int64_t rows, int64_t n);
 int b200_colsum_bf16(const void* a, void* out, int accumulate, void* workspace, int64_t rows, int64_t n, int64_t ld,
                      cudaStream_t stream);
+/* Same into an fp32 vector (16-byte aligned). */
+int b200_colsum_f32(const void* a, float* out, int accumulate, void* workspace, int64_t rows, int64_t n, int64_t ld,
+                    cudaStream_t stream);
 
 /* ---- RoPE (rotate-half), in place on `num_heads` consecutive heads starting at x: replaces Paddle-core
  * fused_rotary_position_embedding(use_neox_rotary_style=False) (fusion_ops.py:57-116; llama/modeling.py:557-577).
@@ -139,6 +152,9 @@ int b200_embedding_fwd(const int64_t* ids, const void* table, void* out, int64_t
                        cudaStream_t stream);
 int b200_embedding_bwd(const int64_t* ids, const void* dout, void* dtable, int64_t tokens, int64_t h, int64_t vocab,
                        cudaStream_t stream);
+/* Same scatter-add into an fp32 table (16-byte aligned; dout 8-byte aligned): fp32 vector atomics, 4 columns each. */
+int b200_embedding_bwd_f32(const int64_t* ids, const void* dout, float* dtable, int64_t tokens, int64_t h, int64_t vocab,
+                           cudaStream_t stream);
 
 /* ---- Flash attention, causal, GQA, head_dim 64 or 128 (anything else: argument error): replaces F.scaled_dot_product_attention(is_causal=True)
  * (fusion_ops.py:147-267; Paddle-vendored FlashAttention-2) and its gradient (csrc/gpu/flash_attn_bwd.cc:22-92).
@@ -194,6 +210,12 @@ int b200_grad_sqnorm(const void* grads, float* out, void* workspace, int64_t n, 
 int b200_adamw_step(void* params_bf16, const void* grads_bf16, float* master, float* exp_avg, float* exp_avg_sq,
                     const float* grad_sqnorm, int64_t n, int64_t decay_end, float lr, float beta1, float beta2, float eps,
                     float weight_decay, int64_t step, float grad_scale, float max_grad_norm, cudaStream_t stream);
+/* The same two ops on an fp32 gradient buffer (fp32 master gradients; 16-byte aligned).  The arithmetic is the bf16 forms':
+ * those convert each gradient to fp32 first, so a buffer of bf16-representable values gives the same bits. */
+int b200_grad_sqnorm_f32(const float* grads, float* out, void* workspace, int64_t n, float scale, cudaStream_t stream);
+int b200_adamw_step_f32(void* params_bf16, const float* grads, float* master, float* exp_avg, float* exp_avg_sq,
+                        const float* grad_sqnorm, int64_t n, int64_t decay_end, float lr, float beta1, float beta2, float eps,
+                        float weight_decay, int64_t step, float grad_scale, float max_grad_norm, cudaStream_t stream);
 int b200_bf16_to_f32(const void* src, float* dst, int64_t n, cudaStream_t stream);
 
 /* ======================================================================================================================

@@ -28,6 +28,7 @@ _SIGNATURES = {
     "b200_set_fa_bwd_impl": [I],
     "b200_gemm_bf16": [P, P, P, P, I64, I64, I64, I64, I64, I64, I, I, I, P],
     "b200_gemm_bf16_ex": [P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I, I, I, I, P],
+    "b200_gemm_bf16_f32": [P, P, P, I64, I64, I64, I64, I64, I64, I, I, I, P],
     "b200_gemm_swiglu_bf16": [P, P, P, P, I64, I64, I64, I64, I64, I64, I64, P],
     "b200_gemm_swiglu_bwd_bf16": [P, P, P, P, I64, I64, I64, I64, I64, I64, I64, P],
     "b200_gemm_splitk_workspace_bytes": [I64, I64],
@@ -35,14 +36,17 @@ _SIGNATURES = {
     "b200_rmsnorm_fwd": [P, P, P, P, I64, I64, F, P],
     "b200_rmsnorm_bwd_workspace_bytes": [I64, I64],
     "b200_rmsnorm_bwd": [P, P, P, P, P, P, P, I, P, I64, I64, P],
+    "b200_rmsnorm_bwd_f32": [P, P, P, P, P, P, P, I, P, I64, I64, P],
     "b200_colsum_workspace_bytes": [I64, I64],
     "b200_colsum_bf16": [P, P, I, P, I64, I64, I64, P],
+    "b200_colsum_f32": [P, P, I, P, I64, I64, I64, P],
     "b200_rope_inplace": [P, P, P, P, I64, I64, I64, I64, I64, I, P],
     "b200_swiglu_fwd": [P, P, I64, I64, P],
     "b200_swiglu_fwd_f32": [P, P, I64, I64, P],
     "b200_swiglu_bwd": [P, P, P, I64, I64, P],
     "b200_embedding_fwd": [P, P, P, I64, I64, I64, P],
     "b200_embedding_bwd": [P, P, P, I64, I64, I64, P],
+    "b200_embedding_bwd_f32": [P, P, P, I64, I64, I64, P],
     "b200_fa_fwd": [P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I64, I64, F, P],
     "b200_fa_fwd_flashmask": [P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I64, I64, F, P],
     "b200_fa_bwd_flashmask": [P, P, P, P, P, P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I64, I64, I64, I64, I64, I64, F, P],
@@ -56,6 +60,8 @@ _SIGNATURES = {
     "b200_grad_sqnorm_workspace_bytes": [],
     "b200_grad_sqnorm": [P, P, P, I64, F, P],
     "b200_adamw_step": [P, P, P, P, P, P, I64, I64, F, F, F, F, F, I64, F, F, P],
+    "b200_grad_sqnorm_f32": [P, P, P, I64, F, P],
+    "b200_adamw_step_f32": [P, P, P, P, P, P, I64, I64, F, F, F, F, F, I64, F, F, P],
     "b200_bf16_to_f32": [P, P, I64, P],
     "b200_add_rmsnorm": [P, P, P, P, P, I64, I64, F, P],
     "b200_add_rmsnorm_f32": [P, P, P, P, P, I64, I64, F, P],
@@ -127,9 +133,9 @@ class B200Error(RuntimeError):
 
 # CUDA kernels each entry point launches (used by bench.py to report `gpu_launches`; memsets are not counted).
 KERNELS_PER_CALL = {
-    "b200_gemm_bf16": 1, "b200_gemm_bf16_ex": 1, "b200_gemm_bf16_splitk": 2, "b200_rmsnorm_fwd": 1, "b200_rmsnorm_bwd": 2, "b200_colsum_bf16": 2,
+    "b200_gemm_bf16": 1, "b200_gemm_bf16_ex": 1, "b200_gemm_bf16_splitk": 2, "b200_rmsnorm_fwd": 1, "b200_rmsnorm_bwd": 2, "b200_rmsnorm_bwd_f32": 2, "b200_colsum_bf16": 2, "b200_colsum_f32": 2,
     "b200_rope_inplace": 1, "b200_swiglu_fwd": 1, "b200_swiglu_bwd": 1, "b200_embedding_fwd": 1, "b200_embedding_bwd": 1,
-    "b200_fa_fwd": 1, "b200_fa_bwd": 5, "b200_fa_fwd_flashmask": 1, "b200_fa_bwd_flashmask": 5, "b200_ce_fwd": 2, "b200_ce_bwd": 1, "b200_ce_rows_fwd": 1, "b200_ce_reduce": 1, "b200_argmax_bf16": 1, "b200_grad_sqnorm": 2,
+    "b200_fa_fwd": 1, "b200_fa_bwd": 5, "b200_fa_fwd_flashmask": 1, "b200_fa_bwd_flashmask": 5, "b200_ce_fwd": 2, "b200_ce_bwd": 1, "b200_ce_rows_fwd": 1, "b200_ce_reduce": 1, "b200_argmax_bf16": 1, "b200_grad_sqnorm": 2, "b200_grad_sqnorm_f32": 2,
     "b200_adamw_step": 1, "b200_bf16_to_f32": 1, "b200_token_penalty_multi_scores": 2, "b200_generate_step_update": 2, "b200_decode_attention": 2, "b200_decode_attention_tc": 2, "b200_decode_attention_paged": 2, "b200_append_attention": 5,
 }
 launch_count = 0       # kernels launched through this module since import

@@ -122,6 +122,14 @@ __device__ __forceinline__ void tma_reduce_add_4d(const CUtensorMap* tm, const v
                "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
                : "memory");
 }
+// shared -> global element-wise ADD (fp32 tensor map), 2D tile (bulk-group completion); elements outside the tensor are not
+// touched.  The reduction runs in L2 and flushes subnormal results to zero.
+__device__ __forceinline__ void tma_reduce_add_2d(const CUtensorMap* tm, uint32_t smem_src, int c0, int c1) {
+  asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
+                   reinterpret_cast<uint64_t>(tm)),
+               "r"(smem_src), "r"(c0), "r"(c1)
+               : "memory");
+}
 // shared -> global, 2D tile (bulk-group completion); elements outside the tensor are not written.
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* tm, uint32_t smem_src, int c0, int c1) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(reinterpret_cast<uint64_t>(tm)),
@@ -284,6 +292,9 @@ __device__ __forceinline__ void st_na_v4(void* p, const uint4& v) {
 // loop may still be scheduled ahead of it.
 __device__ __forceinline__ void st_shared_u32(uint32_t saddr, uint32_t v) {
   asm volatile("st.shared.u32 [%0], %1;" ::"r"(saddr), "r"(v));
+}
+__device__ __forceinline__ void st_shared_f32x2(uint32_t saddr, float a, float b) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(saddr), "f"(a), "f"(b));
 }
 __device__ __forceinline__ uint4 ld_shared_v4(uint32_t saddr) {
   uint4 r;

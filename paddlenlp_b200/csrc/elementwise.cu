@@ -2,6 +2,7 @@
 // scatter-add, bias-gradient column sums.  All are 128-bit vectorised, fp32 math, ONE rounding to bf16 per output
 // (rounding points listed in SURVEY.md §8a).  Roofline for each: algorithmic bytes / measured HBM bandwidth.
 #include "../../include/b200nlp.h"
+#include <type_traits>
 #include "common.cuh"
 #include "host_util.h"
 
@@ -218,9 +219,10 @@ __global__ void __launch_bounds__(1024) rmsnorm_bwd_kernel(const bf16* __restric
   }
 }
 
-// dw[c] (+)= sum_p partial[p, c]   (bf16 gradient, fp32 sum).
+// dw[c] (+)= sum_p partial[p, c]   (fp32 sum; the gradient OutT is bf16, or fp32 for fp32 master gradients).
 // Block = 32 column-quads (128 columns, float4 loads) x 8 partial-row lanes; the 8 lanes are folded through smem.
-__global__ void __launch_bounds__(256) colsum_reduce_kernel(const float* __restrict__ partial, bf16* __restrict__ dw,
+template <typename OutT>
+__global__ void __launch_bounds__(256) colsum_reduce_kernel(const float* __restrict__ partial, OutT* __restrict__ dw,
                                                             int nparts, int h, int accumulate) {
   __shared__ float4 red[8][32];
   const int cq = threadIdx.x & 31, pl = threadIdx.x >> 5;
@@ -240,13 +242,22 @@ __global__ void __launch_bounds__(256) colsum_reduce_kernel(const float* __restr
       const float4 v = red[k][cq];
       acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
     }
-    __nv_bfloat162* d2 = reinterpret_cast<__nv_bfloat162*>(dw + col);
-    if (accumulate) {
-      const float2 o0 = __bfloat1622float2(d2[0]), o1 = __bfloat1622float2(d2[1]);
-      acc.x += o0.x; acc.y += o0.y; acc.z += o1.x; acc.w += o1.y;
+    if constexpr (std::is_same<OutT, float>::value) {
+      float4* d4 = reinterpret_cast<float4*>(dw + col);
+      if (accumulate) {
+        const float4 o = *d4;
+        acc.x += o.x; acc.y += o.y; acc.z += o.z; acc.w += o.w;
+      }
+      *d4 = acc;
+    } else {
+      __nv_bfloat162* d2 = reinterpret_cast<__nv_bfloat162*>(dw + col);
+      if (accumulate) {
+        const float2 o0 = __bfloat1622float2(d2[0]), o1 = __bfloat1622float2(d2[1]);
+        acc.x += o0.x; acc.y += o0.y; acc.z += o1.x; acc.w += o1.y;
+      }
+      d2[0] = __floats2bfloat162_rn(acc.x, acc.y);
+      d2[1] = __floats2bfloat162_rn(acc.z, acc.w);
     }
-    d2[0] = __floats2bfloat162_rn(acc.x, acc.y);
-    d2[1] = __floats2bfloat162_rn(acc.z, acc.w);
   }
 }
 
@@ -404,14 +415,27 @@ __global__ void embedding_fwd_kernel(const int64_t* __restrict__ ids, const bf16
   for (int c = threadIdx.x; c < (h >> 3); c += blockDim.x) dst[c] = __ldg(src + c);
 }
 
+// dtable[ids[t]] += dout[t]: bf16 pair atomics into a bf16 table, or fp32 vector atomics (4 columns per red) into an fp32 one.
+template <typename T>
 __global__ void embedding_bwd_kernel(const int64_t* __restrict__ ids, const bf16* __restrict__ dout,
-                                     bf16* __restrict__ dtable, int tokens, int h, int vocab) {
+                                     T* __restrict__ dtable, int tokens, int h, int vocab) {
   const int tok = blockIdx.x;
   const int64_t id = ids[tok];
   if (id < 0 || id >= vocab) return;
-  const __nv_bfloat162* src = reinterpret_cast<const __nv_bfloat162*>(dout + static_cast<size_t>(tok) * h);
-  __nv_bfloat162* dst = reinterpret_cast<__nv_bfloat162*>(dtable + id * h);
-  for (int c = threadIdx.x; c < (h >> 1); c += blockDim.x) atomicAdd(dst + c, src[c]);
+  if constexpr (std::is_same<T, float>::value) {
+    const uint2* src = reinterpret_cast<const uint2*>(dout + static_cast<size_t>(tok) * h);
+    float* dst = dtable + id * h;
+    for (int c = threadIdx.x; c < (h >> 2); c += blockDim.x) {
+      const uint2 v = src[c];
+      const float2 a = unpack_bf16x2(v.x), b = unpack_bf16x2(v.y);
+      asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + 4 * c), "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y)
+                   : "memory");
+    }
+  } else {
+    const __nv_bfloat162* src = reinterpret_cast<const __nv_bfloat162*>(dout + static_cast<size_t>(tok) * h);
+    __nv_bfloat162* dst = reinterpret_cast<__nv_bfloat162*>(dtable + id * h);
+    for (int c = threadIdx.x; c < (h >> 1); c += blockDim.x) atomicAdd(dst + c, src[c]);
+  }
 }
 
 }  // namespace ew
@@ -451,9 +475,9 @@ extern "C" int64_t b200_rmsnorm_bwd_workspace_bytes(int64_t rows, int64_t h) {
   return parts * h * 4;
 }
 
-extern "C" int b200_rmsnorm_bwd(const void* dy, const void* x, const void* w, const float* rstd, const void* dres,
-                                void* dx, void* dw, int accumulate_dw, void* workspace, int64_t rows, int64_t h,
-                                cudaStream_t stream) {
+template <typename OutT>
+static int rmsnorm_bwd(const void* dy, const void* x, const void* w, const float* rstd, const void* dres, void* dx, OutT* dw,
+                       int accumulate_dw, void* workspace, int64_t rows, int64_t h, cudaStream_t stream) {
   B200_CHECK_ARG(dy && x && w && rstd && dx && dw && workspace, "rmsnorm_bwd: null pointer");
   B200_CHECK_ARG(rows > 0 && h > 0 && h % 8 == 0 && h <= 8192, "rmsnorm_bwd: need 0 < h <= 8192, h %% 8 == 0 (h=%lld)",
                  (long long)h);
@@ -467,8 +491,21 @@ extern "C" int b200_rmsnorm_bwd(const void* dy, const void* x, const void* w, co
   int rc = check_launch("rmsnorm_bwd");
   if (rc) return rc;
   colsum_reduce_kernel<<<static_cast<unsigned>((h + 127) / 128), 256, 0, stream>>>(
-      static_cast<const float*>(workspace), static_cast<bf16*>(dw), parts, (int)h, accumulate_dw);
+      static_cast<const float*>(workspace), dw, parts, (int)h, accumulate_dw);
   return check_launch("rmsnorm_bwd(dw reduce)");
+}
+
+extern "C" int b200_rmsnorm_bwd(const void* dy, const void* x, const void* w, const float* rstd, const void* dres,
+                                void* dx, void* dw, int accumulate_dw, void* workspace, int64_t rows, int64_t h,
+                                cudaStream_t stream) {
+  return rmsnorm_bwd(dy, x, w, rstd, dres, dx, static_cast<bf16*>(dw), accumulate_dw, workspace, rows, h, stream);
+}
+
+extern "C" int b200_rmsnorm_bwd_f32(const void* dy, const void* x, const void* w, const float* rstd, const void* dres,
+                                    void* dx, float* dw, int accumulate_dw, void* workspace, int64_t rows, int64_t h,
+                                    cudaStream_t stream) {
+  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(dw) & 15) == 0, "rmsnorm_bwd_f32: dw must be 16-byte aligned");
+  return rmsnorm_bwd(dy, x, w, rstd, dres, dx, dw, accumulate_dw, workspace, rows, h, stream);
 }
 
 extern "C" int64_t b200_colsum_workspace_bytes(int64_t rows, int64_t n) {
@@ -476,8 +513,9 @@ extern "C" int64_t b200_colsum_workspace_bytes(int64_t rows, int64_t n) {
   return parts * n * 4;
 }
 
-extern "C" int b200_colsum_bf16(const void* a, void* out, int accumulate, void* workspace, int64_t rows, int64_t n,
-                                int64_t ld, cudaStream_t stream) {
+template <typename OutT>
+static int colsum(const void* a, OutT* out, int accumulate, void* workspace, int64_t rows, int64_t n, int64_t ld,
+                  cudaStream_t stream) {
   B200_CHECK_ARG(a && out && workspace, "colsum: null pointer");
   B200_CHECK_ARG(rows > 0 && n > 0 && n % 8 == 0 && ld % 8 == 0, "colsum: n and ld must be multiples of 8");
   const int parts = static_cast<int>(rows < 64 ? rows : 64);
@@ -487,8 +525,19 @@ extern "C" int b200_colsum_bf16(const void* a, void* out, int accumulate, void* 
   int rc = check_launch("colsum(partial)");
   if (rc) return rc;
   colsum_reduce_kernel<<<static_cast<unsigned>((n + 127) / 128), 256, 0, stream>>>(
-      static_cast<const float*>(workspace), static_cast<bf16*>(out), parts, (int)n, accumulate);
+      static_cast<const float*>(workspace), out, parts, (int)n, accumulate);
   return check_launch("colsum(reduce)");
+}
+
+extern "C" int b200_colsum_bf16(const void* a, void* out, int accumulate, void* workspace, int64_t rows, int64_t n,
+                                int64_t ld, cudaStream_t stream) {
+  return colsum(a, static_cast<bf16*>(out), accumulate, workspace, rows, n, ld, stream);
+}
+
+extern "C" int b200_colsum_f32(const void* a, float* out, int accumulate, void* workspace, int64_t rows, int64_t n, int64_t ld,
+                               cudaStream_t stream) {
+  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(out) & 15) == 0, "colsum_f32: out must be 16-byte aligned");
+  return colsum(a, out, accumulate, workspace, rows, n, ld, stream);
 }
 
 extern "C" int b200_rope_inplace(void* x, const float* cos_table, const float* sin_table, const int32_t* position_ids,
@@ -554,12 +603,24 @@ extern "C" int b200_embedding_fwd(const int64_t* ids, const void* table, void* o
   return check_launch("embedding_fwd");
 }
 
-extern "C" int b200_embedding_bwd(const int64_t* ids, const void* dout, void* dtable, int64_t tokens, int64_t h,
-                                  int64_t vocab, cudaStream_t stream) {
+template <typename T>
+static int embedding_bwd(const int64_t* ids, const void* dout, T* dtable, int64_t tokens, int64_t h, int64_t vocab,
+                         cudaStream_t stream) {
   B200_CHECK_ARG(ids && dout && dtable, "embedding_bwd: null pointer");
   B200_CHECK_ARG(tokens > 0 && h % 8 == 0, "embedding_bwd: hidden size must be a multiple of 8");
-  embedding_bwd_kernel<<<static_cast<unsigned>(tokens), 128, 0, stream>>>(ids, static_cast<const bf16*>(dout),
-                                                                         static_cast<bf16*>(dtable), (int)tokens, (int)h,
-                                                                         (int)vocab);
+  embedding_bwd_kernel<<<static_cast<unsigned>(tokens), 128, 0, stream>>>(ids, static_cast<const bf16*>(dout), dtable,
+                                                                         (int)tokens, (int)h, (int)vocab);
   return check_launch("embedding_bwd");
+}
+
+extern "C" int b200_embedding_bwd(const int64_t* ids, const void* dout, void* dtable, int64_t tokens, int64_t h,
+                                  int64_t vocab, cudaStream_t stream) {
+  return embedding_bwd(ids, dout, static_cast<bf16*>(dtable), tokens, h, vocab, stream);
+}
+
+extern "C" int b200_embedding_bwd_f32(const int64_t* ids, const void* dout, float* dtable, int64_t tokens, int64_t h,
+                                      int64_t vocab, cudaStream_t stream) {
+  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(dtable) & 15) == 0 && (reinterpret_cast<uintptr_t>(dout) & 7) == 0,
+                 "embedding_bwd_f32: dtable must be 16-byte and dout 8-byte aligned");
+  return embedding_bwd(ids, dout, dtable, tokens, h, vocab, stream);
 }

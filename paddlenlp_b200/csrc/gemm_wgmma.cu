@@ -1,6 +1,7 @@
 // bf16 GEMM on Hopper tensor cores (wgmma.mma_async, accumulators in registers, operands staged by TMA).
 //
-//   C[M,N] (+)= op(A)[M,K] * op(B)[K,N] (+ bias[N])      bf16 in, fp32 accumulate, one rounding to bf16.
+//   C[M,N] (+)= op(A)[M,K] * op(B)[K,N] (+ bias[N])      bf16 in, fp32 accumulate, one rounding to bf16
+//   C_f32[M,N] (+)= op(A)[M,K] * op(B)[K,N]              the same, fp32 out, no rounding (fp32 weight gradients).
 //
 // Replaces the cuBLAS(Lt) calls under paddle `nn.Linear` on the Llama/Qwen2 hot path
 // (reference: paddlenlp/transformers/llama/modeling.py:771-799 q/k/v/o, :627-630 gate/up/down, :1894-1921 lm_head;
@@ -14,7 +15,9 @@
 //                                    k-block's stage is released once the next block's wgmmas are in flight; the epilogue
 //                                    (+bias, +C_old | +residual, SwiGLU forms) stages bf16 64 x 64 boxes in shared memory and
 //                                    stores them with TMA (C_old / residual / gate|up prefetched into L2 during the tile's
-//                                    last k-blocks); split-K adds its fp32 partial sums from the registers into L2
+//                                    last k-blocks); fp32 outputs leave as 64 x 32 fp32 boxes through the same buffers,
+//                                    stored or reduce-added by TMA; split-K adds its fp32 partial sums from the registers
+//                                    into L2
 //   Operand majors: both K-major (contraction dim contiguous) and MN-major operands are fed straight from their
 //   row-major global layout through TMA (wgmma reads either major for 16-bit types); no transposes are materialised.
 #include "../../include/b200nlp.h"
@@ -32,6 +35,7 @@ constexpr int BK = 64;    // K per pipeline stage (= one 128-byte swizzle row of
 constexpr int B_BYTES = BN * BK * 2;              // 32 KB
 constexpr int EPI_BOX = 64;                       // epilogue TMA box: 64 rows x 64 columns (one 128-byte swizzle row wide)
 constexpr int EPI_BOX_BYTES = EPI_BOX * EPI_BOX * 2;   // 8 KB
+constexpr int EPI_BOX_F32 = 32;                   // fp32 epilogue box: 64 rows x 32 columns, also 8 KB
 
 // NWG consumer warpgroups of 64 rows each.  NWG = 2 (128-row tiles) for the training shapes; NWG = 1 (64-row tiles) for the
 // decode step's M <= 64 token rows, where the kernel is a weight stream: 8 KB of activations and 32 KB of weights per stage,
@@ -58,6 +62,7 @@ struct Params {
                            //    m = bf16(silu(gate) * up) [M, I]
                            // 5: down-proj dX GEMM + SwiGLU backward: acc = d(m) tile; aux = saved gate|up [M, 2I];
                            //    C = [d(gate) | d(up)] [M, 2I]
+                           // 6: C_f32 = acc ; 7: C_f32 += acc (fp32 output through tmC, no bias: weight gradients)
   int swiglu_inter;        // modes 4, 5: I (the up half starts at column I)
   int gm;                  // m-tiles per raster group (tile_coords)
   int split_k;             // work items per output tile (K is cut into split_k ranges of kb_per_split k-blocks)
@@ -69,7 +74,7 @@ struct Params {
   int64_t ldr;
   bf16* aux;               // mode 4: gate|up output (nullable); mode 5: saved gate|up input
   int64_t ld_aux;
-  float* ws;               // mode 3: fp32 [M, N] accumulation buffer
+  float* ws;               // mode 3: fp32 [M, N] accumulation buffer; modes 6, 7: the fp32 output (leading dimension ldc)
 };
 
 __device__ __forceinline__ void tile_coords(int t, int num_m, int num_n, int& m_blk, int& n_blk, int GM) {
@@ -351,11 +356,41 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       }
       continue;
     }
-    // modes 0, 1, 2
+    // modes 0, 1, 2, 6, 7
 #pragma unroll
     for (int s = 0; s < BN / EPI_BOX; ++s) {
       const int col0 = n_blk * BN + EPI_BOX * s;
       if (col0 >= p.N) continue;
+      if (p.epi_mode >= 6) {
+        // fp32 output: the 64 columns leave as two 64 x 32 fp32 boxes (128 bytes per row, like a bf16 box), one in each
+        // buffer.  Mode 7 adds them onto C in L2 (TMA reduce-add): one fp32 add per element, C_old never enters the
+        // registers.  Row r's byte b sits at b ^ (16 (r % 8)); this thread's pair of box column 8 jj + 2 (lane % 4) is row
+        // byte 32 jj + 8 (lane % 4), and r % 8 = lane / 4 for both of its rows: a warp's 8 rows fill every chunk twice.
+        const uint32_t sw = (lane >> 2) << 4;
+        const uint32_t row_off = r_lo * 128 + ((8 * (lane & 3)) ^ (sw & 16));
+        epi_begin<0>(cw, leader);
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj) {
+            const int j = 8 * s + 4 * h + jj;
+            const uint32_t slot = ebuf + h * EPI_BOX_BYTES + row_off + ((32 * jj) ^ (sw & 96));
+            st_shared_f32x2(slot, acc[4 * j], acc[4 * j + 1]);
+            st_shared_f32x2(slot + 8 * 128, acc[4 * j + 2], acc[4 * j + 3]);
+          }
+        epi_end(cw);
+        if (leader) {
+          if (p.epi_mode == 7) {
+            tma_reduce_add_2d(&tmC, ebuf, col0, row0);
+            tma_reduce_add_2d(&tmC, ebuf + EPI_BOX_BYTES, col0 + EPI_BOX_F32, row0);
+          } else {
+            tma_store_2d(&tmC, ebuf, col0, row0);
+            tma_store_2d(&tmC, ebuf + EPI_BOX_BYTES, col0 + EPI_BOX_F32, row0);
+          }
+          tma_store_commit();
+        }
+        continue;
+      }
       const uint32_t buf = ebuf + (nbox++ & 1u) * EPI_BOX_BYTES;
       epi_begin<1>(cw, leader);
 #pragma unroll
@@ -432,6 +467,12 @@ static int make_epi_map(CUtensorMap* tm, const void* base, int64_t rows, int64_t
   const uint32_t box[2] = {EPI_BOX, EPI_BOX};
   return encode_tmap_bf16(tm, base, 2, dims, strides, box);
 }
+// fp32 output map (modes 6, 7): [rows, cols] fp32, box {32 columns, 64 rows}.
+static int make_epi_map_f32(CUtensorMap* tm, const void* base, int64_t rows, int64_t cols, int64_t ld) {
+  const uint64_t dims[2] = {static_cast<uint64_t>(cols), static_cast<uint64_t>(rows)}, strides[1] = {static_cast<uint64_t>(ld) * 4};
+  const uint32_t box[2] = {EPI_BOX_F32, EPI_BOX};
+  return encode_tmap_f32(tm, base, 2, dims, strides, box);
+}
 static bool aligned16(const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; }
 
 // Tensor maps of the shared-memory epilogue (every mode but split-K).  TMA needs 16-byte aligned base addresses (the strides
@@ -444,6 +485,9 @@ static int setup_smem_epilogue(const Params& p, CUtensorMap* tmC, CUtensorMap* t
       return make_epi_map(tmC, p.c, p.M, p.N, p.ldc);
     case 3:
       return 0;
+    case 6:
+    case 7:
+      return make_epi_map_f32(tmC, p.ws, p.M, p.N, p.ldc);
     case 4:   // p.N = 2 I: tmC is m [M, I], tmX the gate|up output [M, 2I]
       if (p.aux != nullptr && (rc = make_epi_map(tmX, p.aux, p.M, p.N, p.ld_aux)) != 0) return rc;
       return make_epi_map(tmC, p.c, p.M, p.swiglu_inter, p.ldc);
@@ -533,6 +577,31 @@ extern "C" int b200_gemm_bf16_ex(const void* A, const void* B, void* C, const fl
   p.r = static_cast<const bf16*>(residual);
   p.ldr = ldr;
   return dispatch(a_mn_major, b_mn_major, tmA, tmB, p, max_ctas, stream);
+}
+
+// fp32-output form for weight gradients kept in fp32 (fused_linear_param_grad_add(..., multi_precision=True),
+// llm/utils/fused_layers.py:44-50): C_f32 = acc, or C_f32 += acc with one fp32 add per element by TMA reduce-add.
+extern "C" int b200_gemm_bf16_f32(const void* A, const void* B, float* C, int64_t M, int64_t N, int64_t K, int64_t lda,
+                                  int64_t ldb, int64_t ldc, int a_mn_major, int b_mn_major, int accumulate, cudaStream_t stream) {
+  using namespace b200;
+  using namespace b200::gemm;
+  B200_CHECK_ARG(A && B && C, "gemm_f32: null pointer");
+  B200_CHECK_ARG(M > 0 && N > 0 && K > 0, "gemm_f32: non-positive dimension M=%lld N=%lld K=%lld", (long long)M,
+                 (long long)N, (long long)K);
+  B200_CHECK_ARG(lda % 8 == 0 && ldb % 8 == 0, "gemm_f32: lda and ldb must be multiples of 8");
+  B200_CHECK_ARG(ldc % 4 == 0 && ldc >= N, "gemm_f32: ldc must be a multiple of 4 and >= N (ldc=%lld N=%lld)", (long long)ldc,
+                 (long long)N);
+  B200_CHECK_ARG(M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31), "gemm_f32: dimension too large");
+  B200_CHECK_ARG(aligned16(C), "gemm_f32: C must be 16-byte aligned");
+  CUtensorMap tmA, tmB;
+  int rc;
+  if ((rc = make_a_map(&tmA, A, M, K, lda, a_mn_major)) != 0) return rc;
+  if ((rc = make_b_map(&tmB, B, N, K, ldb, b_mn_major)) != 0) return rc;
+  Params p = base_params(M, N, K);
+  p.epi_mode = accumulate ? 7 : 6;
+  p.ws = C;
+  p.ldc = ldc;
+  return dispatch(a_mn_major, b_mn_major, tmA, tmB, p, 0, stream);
 }
 
 // gate|up projection + SwiGLU in one kernel (training forward of LlamaMLP, llama/modeling.py:632-652 with fuse_attention_ffn):

@@ -206,21 +206,37 @@ __global__ void __launch_bounds__(1024) argmax_kernel(const bf16* __restrict__ l
 // ------------------------------------------------------------------------------------------------
 // Optimizer
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) sqnorm_partial_kernel(const bf16* __restrict__ g, float* __restrict__ partial,
-                                                             int64_t n) {
+// Gradients are bf16, or fp32 (fp32 master gradients): chunk c of 8 elements as fp32, read once (not cached in L1).
+__device__ __forceinline__ void load8_f32(const bf16* g, int64_t c, float (&f)[8]) {
+  const uint4 v = ld_nc_v4(reinterpret_cast<const uint4*>(g) + c);
+  const uint32_t* vi = reinterpret_cast<const uint32_t*>(&v);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) { const float2 t = unpack_bf16x2(vi[j]); f[2 * j] = t.x; f[2 * j + 1] = t.y; }
+}
+__device__ __forceinline__ void load8_f32(const float* g, int64_t c, float (&f)[8]) {
+  const uint4 a = ld_nc_v4(reinterpret_cast<const uint4*>(g) + 2 * c), b = ld_nc_v4(reinterpret_cast<const uint4*>(g) + 2 * c + 1);
+  const uint32_t u[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+#pragma unroll
+  for (int j = 0; j < 8; ++j) f[j] = __uint_as_float(u[j]);
+}
+__device__ __forceinline__ float to_f32(bf16 x) { return __bfloat162float(x); }
+__device__ __forceinline__ float to_f32(float x) { return x; }
+
+template <typename G>
+__global__ void __launch_bounds__(256) sqnorm_partial_kernel(const G* __restrict__ g, float* __restrict__ partial, int64_t n) {
   __shared__ float red[8];
   float acc = 0.f;
   const int64_t nchunk = n >> 3;
   for (int64_t c = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; c < nchunk;
        c += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-    const uint4 v = ld_nc_v4(reinterpret_cast<const uint4*>(g) + c);
-    const uint32_t* vi = reinterpret_cast<const uint32_t*>(&v);
+    float f[8];
+    load8_f32(g, c, f);
 #pragma unroll
-    for (int j = 0; j < 4; ++j) { const float2 t = unpack_bf16x2(vi[j]); acc += t.x * t.x + t.y * t.y; }
+    for (int j = 0; j < 4; ++j) acc += f[2 * j] * f[2 * j] + f[2 * j + 1] * f[2 * j + 1];
   }
   if (blockIdx.x == 0)
     for (int64_t i = (nchunk << 3) + threadIdx.x; i < n; i += blockDim.x) {
-      const float t = __bfloat162float(g[i]);
+      const float t = to_f32(g[i]);
       acc += t * t;
     }
   acc = warp_sum(acc);
@@ -256,7 +272,8 @@ struct AdamArgs {
 };
 
 // Paddle adamw kernel semantics: p *= (1 - lr*wd); m,v update; p -= lr/(1-b1^t) * m / (sqrt(v)/sqrt(1-b2^t) + eps).
-__global__ void __launch_bounds__(256) adamw_kernel(bf16* __restrict__ p16, const bf16* __restrict__ g16,
+template <typename G>
+__global__ void __launch_bounds__(256) adamw_kernel(bf16* __restrict__ p16, const G* __restrict__ grads,
                                                     float* __restrict__ master, float* __restrict__ m,
                                                     float* __restrict__ v, const float* __restrict__ sqnorm,
                                                     AdamArgs a) {
@@ -270,11 +287,10 @@ __global__ void __launch_bounds__(256) adamw_kernel(bf16* __restrict__ p16, cons
   const int64_t nchunk = a.n >> 3;
   for (int64_t c = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; c < nchunk;
        c += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-    const uint4 gv = ld_nc_v4(reinterpret_cast<const uint4*>(g16) + c);
-    const uint32_t* gi = reinterpret_cast<const uint32_t*>(&gv);
     float g[8];
+    load8_f32(grads, c, g);
 #pragma unroll
-    for (int j = 0; j < 4; ++j) { const float2 t = unpack_bf16x2(gi[j]); g[2 * j] = t.x * gs; g[2 * j + 1] = t.y * gs; }
+    for (int j = 0; j < 8; ++j) g[j] *= gs;
     float4* mp = reinterpret_cast<float4*>(m) + 2 * c;
     float4* vp = reinterpret_cast<float4*>(v) + 2 * c;
     float4* pp = reinterpret_cast<float4*>(master) + 2 * c;
@@ -365,22 +381,33 @@ extern "C" int b200_argmax_bf16(const void* logits, int64_t* out, int64_t rows, 
 
 extern "C" int64_t b200_grad_sqnorm_workspace_bytes(void) { return static_cast<int64_t>(sm_count()) * 8 * 4; }
 
-extern "C" int b200_grad_sqnorm(const void* grads, float* out, void* workspace, int64_t n, float scale,
-                                cudaStream_t stream) {
+template <typename G>
+static int grad_sqnorm(const G* grads, float* out, void* workspace, int64_t n, float scale, cudaStream_t stream) {
   B200_CHECK_ARG(grads && out && workspace && n > 0, "grad_sqnorm: bad arguments");
   const int blocks = sm_count() * 8;
-  sqnorm_partial_kernel<<<blocks, 256, 0, stream>>>(static_cast<const bf16*>(grads), static_cast<float*>(workspace), n);
+  sqnorm_partial_kernel<<<blocks, 256, 0, stream>>>(grads, static_cast<float*>(workspace), n);
   int rc = check_launch("grad_sqnorm(partial)");
   if (rc) return rc;
   sqnorm_final_kernel<<<1, 1024, 0, stream>>>(static_cast<const float*>(workspace), out, blocks, scale);
   return check_launch("grad_sqnorm(final)");
 }
 
-extern "C" int b200_adamw_step(void* params_bf16, const void* grads_bf16, float* master, float* exp_avg, float* exp_avg_sq,
-                               const float* grad_sqnorm, int64_t n, int64_t decay_end, float lr, float beta1, float beta2,
-                               float eps, float weight_decay, int64_t step, float grad_scale, float max_grad_norm,
-                               cudaStream_t stream) {
-  B200_CHECK_ARG(params_bf16 && grads_bf16 && master && exp_avg && exp_avg_sq, "adamw: null pointer");
+extern "C" int b200_grad_sqnorm(const void* grads, float* out, void* workspace, int64_t n, float scale,
+                                cudaStream_t stream) {
+  return grad_sqnorm(static_cast<const bf16*>(grads), out, workspace, n, scale, stream);
+}
+
+extern "C" int b200_grad_sqnorm_f32(const float* grads, float* out, void* workspace, int64_t n, float scale,
+                                    cudaStream_t stream) {
+  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(grads) & 15) == 0, "grad_sqnorm_f32: grads must be 16-byte aligned");
+  return grad_sqnorm(grads, out, workspace, n, scale, stream);
+}
+
+template <typename G>
+static int adamw_step(void* params_bf16, const G* grads, float* master, float* exp_avg, float* exp_avg_sq,
+                      const float* grad_sqnorm, int64_t n, int64_t decay_end, float lr, float beta1, float beta2, float eps,
+                      float weight_decay, int64_t step, float grad_scale, float max_grad_norm, cudaStream_t stream) {
+  B200_CHECK_ARG(params_bf16 && grads && master && exp_avg && exp_avg_sq, "adamw: null pointer");
   B200_CHECK_ARG(n > 0 && n % 8 == 0 && decay_end % 8 == 0 && decay_end <= n && step >= 1,
                  "adamw: n and decay_end must be multiples of 8, step >= 1");
   AdamArgs a;
@@ -389,9 +416,25 @@ extern "C" int b200_adamw_step(void* params_bf16, const void* grads_bf16, float*
   a.bias_corr2 = 1.f - powf(beta2, static_cast<float>(step));
   a.grad_scale = grad_scale; a.max_grad_norm = max_grad_norm; a.n = n; a.decay_end = decay_end;
   const int blocks = sm_count() * 8;
-  adamw_kernel<<<blocks, 256, 0, stream>>>(static_cast<bf16*>(params_bf16), static_cast<const bf16*>(grads_bf16), master,
-                                           exp_avg, exp_avg_sq, grad_sqnorm, a);
+  adamw_kernel<<<blocks, 256, 0, stream>>>(static_cast<bf16*>(params_bf16), grads, master, exp_avg, exp_avg_sq, grad_sqnorm, a);
   return check_launch("adamw");
+}
+
+extern "C" int b200_adamw_step(void* params_bf16, const void* grads_bf16, float* master, float* exp_avg, float* exp_avg_sq,
+                               const float* grad_sqnorm, int64_t n, int64_t decay_end, float lr, float beta1, float beta2,
+                               float eps, float weight_decay, int64_t step, float grad_scale, float max_grad_norm,
+                               cudaStream_t stream) {
+  return adamw_step(params_bf16, static_cast<const bf16*>(grads_bf16), master, exp_avg, exp_avg_sq, grad_sqnorm, n, decay_end,
+                    lr, beta1, beta2, eps, weight_decay, step, grad_scale, max_grad_norm, stream);
+}
+
+extern "C" int b200_adamw_step_f32(void* params_bf16, const float* grads, float* master, float* exp_avg, float* exp_avg_sq,
+                                   const float* grad_sqnorm, int64_t n, int64_t decay_end, float lr, float beta1, float beta2,
+                                   float eps, float weight_decay, int64_t step, float grad_scale, float max_grad_norm,
+                                   cudaStream_t stream) {
+  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(grads) & 15) == 0, "adamw_f32: grads must be 16-byte aligned");
+  return adamw_step(params_bf16, grads, master, exp_avg, exp_avg_sq, grad_sqnorm, n, decay_end, lr, beta1, beta2, eps,
+                    weight_decay, step, grad_scale, max_grad_norm, stream);
 }
 
 extern "C" int b200_bf16_to_f32(const void* src, float* dst, int64_t n, cudaStream_t stream) {

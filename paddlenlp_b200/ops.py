@@ -36,6 +36,12 @@ def _chk(t: torch.Tensor, name: str, dtype=BF16):
         raise TypeError(f"{name} must be {dtype}, got {t.dtype}")
 
 
+def _is_f32_grad(t: torch.Tensor, name: str) -> bool:
+    """A gradient operand is bf16, or fp32 (fp32 master gradients, amp_master_grad): True for fp32."""
+    _chk(t, name, torch.float32 if t.dtype == torch.float32 else BF16)
+    return t.dtype == torch.float32
+
+
 _workspaces = {}
 
 
@@ -67,7 +73,9 @@ def gemm(a: torch.Tensor, b: torch.Tensor, out: Optional[torch.Tensor] = None, *
          residual: Optional[torch.Tensor] = None, max_ctas: int = 0) -> torch.Tensor:
     """out (+)= op(a) @ op(b) (+ bias)   or   out = bf16(bf16(op(a) @ op(b) + bias) + residual).
     a, b 2-D bf16 with unit inner stride.
-    trans_a: a is stored [K, M];  trans_b: b is stored [N, K].  Default b layout [K, N] is Paddle's nn.Linear weight."""
+    trans_a: a is stored [K, M];  trans_b: b is stored [N, K].  Default b layout [K, N] is Paddle's nn.Linear weight.
+    An fp32 `out` (fp32 weight gradients) takes the fp32-output form: out = op(a) @ op(b), or out += op(a) @ op(b) with one
+    fp32 add per element and no bf16 rounding; it has no bias, residual or max_ctas."""
     _chk(a, "a"); _chk(b, "b")
     assert a.dim() == 2 and b.dim() == 2 and a.stride(1) == 1 and b.stride(1) == 1
     if trans_a:
@@ -84,7 +92,13 @@ def gemm(a: torch.Tensor, b: torch.Tensor, out: Optional[torch.Tensor] = None, *
         if accumulate:
             raise ValueError("gemm: accumulate=True needs an output tensor")
         out = torch.empty(M, N, dtype=BF16, device=a.device)
-    _chk(out, "out")
+    if _is_f32_grad(out, "out"):
+        if bias is not None or residual is not None or max_ctas:
+            raise ValueError("gemm: an fp32 output takes no bias, residual or max_ctas")
+        assert out.shape == (M, N) and out.stride(1) == 1
+        call("b200_gemm_bf16_f32", ptr(a), ptr(b), ptr(out), M, N, K, a.stride(0), b.stride(0), out.stride(0),
+             1 if trans_a else 0, 0 if trans_b else 1, 1 if accumulate else 0, stream_ptr())
+        return out
     assert out.shape == (M, N) and out.stride(1) == 1
     if bias is not None:
         _chk(bias, "bias", torch.float32)
@@ -185,25 +199,28 @@ def rmsnorm_fwd(x: torch.Tensor, w: torch.Tensor, eps: float, out: Optional[torc
 
 def rmsnorm_bwd(dy: torch.Tensor, x: torch.Tensor, w: torch.Tensor, rstd: torch.Tensor, dw: torch.Tensor,
                 dres: Optional[torch.Tensor] = None, accumulate_dw: bool = True, dx: Optional[torch.Tensor] = None):
-    _chk(dy, "dy"); _chk(x, "x"); _chk(w, "w"); _chk(dw, "dw"); _chk(rstd, "rstd", torch.float32)
+    """dx = RMSNorm backward (+ dres); dw (+)= its weight gradient, bf16 or fp32 (dw's dtype)."""
+    _chk(dy, "dy"); _chk(x, "x"); _chk(w, "w"); _chk(rstd, "rstd", torch.float32)
+    name = "b200_rmsnorm_bwd_f32" if _is_f32_grad(dw, "dw") else "b200_rmsnorm_bwd"
     h = x.shape[-1]
     rows = x.numel() // h
     assert dy.is_contiguous() and x.is_contiguous() and dw.numel() == h
     if dx is None:
         dx = torch.empty_like(x)
     ws = _workspace(_lib.load().b200_rmsnorm_bwd_workspace_bytes(rows, h), x.device, "rmsnorm_bwd")
-    call("b200_rmsnorm_bwd", ptr(dy), ptr(x), ptr(w), ptr(rstd), ptr(dres), ptr(dx), ptr(dw), 1 if accumulate_dw else 0,
+    call(name, ptr(dy), ptr(x), ptr(w), ptr(rstd), ptr(dres), ptr(dx), ptr(dw), 1 if accumulate_dw else 0,
          ptr(ws), rows, h, stream_ptr())
     return dx
 
 
 def colsum(a: torch.Tensor, out: torch.Tensor, accumulate: bool = True):
-    """out[n] (+)= sum over rows of a[rows, n] (a may be a column slice: unit inner stride, any row stride)."""
-    _chk(a, "a"); _chk(out, "out")
+    """out[n] (+)= sum over rows of a[rows, n] (a may be a column slice: unit inner stride, any row stride); out bf16 or fp32."""
+    _chk(a, "a")
+    name = "b200_colsum_f32" if _is_f32_grad(out, "out") else "b200_colsum_bf16"
     rows, n = a.shape
     assert a.stride(1) == 1 and out.numel() == n
     ws = _workspace(_lib.load().b200_colsum_workspace_bytes(rows, n), a.device, "colsum")
-    call("b200_colsum_bf16", ptr(a), ptr(out), 1 if accumulate else 0, ptr(ws), rows, n, a.stride(0), stream_ptr())
+    call(name, ptr(a), ptr(out), 1 if accumulate else 0, ptr(ws), rows, n, a.stride(0), stream_ptr())
     return out
 
 
@@ -328,10 +345,12 @@ def embedding_fwd(ids: torch.Tensor, table: torch.Tensor, out: Optional[torch.Te
 
 
 def embedding_bwd(ids: torch.Tensor, dout: torch.Tensor, dtable: torch.Tensor):
-    _chk(ids, "ids", torch.int64); _chk(dout, "dout"); _chk(dtable, "dtable")
+    """dtable[ids[t]] += dout[t]; dtable bf16 or fp32."""
+    _chk(ids, "ids", torch.int64); _chk(dout, "dout")
+    name = "b200_embedding_bwd_f32" if _is_f32_grad(dtable, "dtable") else "b200_embedding_bwd"
     vocab, h = dtable.shape
     assert dout.is_contiguous() and dtable.is_contiguous()
-    call("b200_embedding_bwd", ptr(ids), ptr(dout), ptr(dtable), ids.numel(), h, vocab, stream_ptr())
+    call(name, ptr(ids), ptr(dout), ptr(dtable), ids.numel(), h, vocab, stream_ptr())
     return dtable
 
 
@@ -456,23 +475,26 @@ def argmax(logits: torch.Tensor) -> torch.Tensor:
 # Optimizer
 # ----------------------------------------------------------------------------------------------------------
 def grad_sqnorm(grads: torch.Tensor, scale: float = 1.0, out: Optional[torch.Tensor] = None):
-    _chk(grads, "grads")
+    """out[0] = ||scale * grads||^2 of a bf16 or fp32 gradient buffer."""
+    name = "b200_grad_sqnorm_f32" if _is_f32_grad(grads, "grads") else "b200_grad_sqnorm"
     assert grads.is_contiguous()
     if out is None:
         out = torch.empty(1, dtype=torch.float32, device=grads.device)
     ws = _workspace(_lib.load().b200_grad_sqnorm_workspace_bytes(), grads.device, "sqnorm")
-    call("b200_grad_sqnorm", ptr(grads), ptr(out), ptr(ws), grads.numel(), float(scale), stream_ptr())
+    call(name, ptr(grads), ptr(out), ptr(ws), grads.numel(), float(scale), stream_ptr())
     return out
 
 
 def adamw_step(params, grads, master, exp_avg, exp_avg_sq, sqnorm, *, decay_end: int, lr: float, beta1: float,
                beta2: float, eps: float, weight_decay: float, step: int, grad_scale: float = 1.0,
                max_grad_norm: float = 1.0):
-    _chk(params, "params"); _chk(grads, "grads")
+    """Clip + AdamW over the flat buffers; grads bf16 or fp32."""
+    _chk(params, "params")
+    name = "b200_adamw_step_f32" if _is_f32_grad(grads, "grads") else "b200_adamw_step"
     for n_, t in (("master", master), ("exp_avg", exp_avg), ("exp_avg_sq", exp_avg_sq)):
         _chk(t, n_, torch.float32)
     n = params.numel()
-    call("b200_adamw_step", ptr(params), ptr(grads), ptr(master), ptr(exp_avg), ptr(exp_avg_sq), ptr(sqnorm), n,
+    call(name, ptr(params), ptr(grads), ptr(master), ptr(exp_avg), ptr(exp_avg_sq), ptr(sqnorm), n,
          decay_end, float(lr), float(beta1), float(beta2), float(eps), float(weight_decay), int(step), float(grad_scale),
          float(max_grad_norm), stream_ptr())
 

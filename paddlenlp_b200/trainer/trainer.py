@@ -397,6 +397,9 @@ class Trainer:
             max_steps = math.ceil(a.num_train_epochs * steps_per_epoch)
             epochs = math.ceil(a.num_train_epochs)
         self.state.max_steps = max_steps
+        if a.amp_master_grad:
+            # trainer.py:1921-1960: fp32 main_grad for every parameter, before the optimizer and the data-parallel wrapper
+            getattr(self.model, "_layers", self.model).set_master_grad(True)
         self.create_optimizer_and_scheduler(max_steps)
         model = self._wrap_model(self.model)
         self.model_wrapped = model

@@ -65,7 +65,7 @@ class TrainingArguments:
     bf16: bool = True
     fp16: bool = False
     fp16_opt_level: str = "O2"
-    amp_master_grad: bool = False
+    amp_master_grad: bool = False                 # fp32 gradients: accumulation, DP exchange, clipping and AdamW in fp32
     recompute: bool = False
     dataloader_num_workers: int = 0
     dataloader_drop_last: bool = True

@@ -13,8 +13,9 @@ and their autograd backward with an explicit saved-tensor plan.  Per layer, forw
 i.e. 4 wgmma GEMMs, 1 mma.sync attention and 4 HBM-bound fusions; the residual adds live in GEMM epilogues.
 
 Data layout in HBM
-  * ONE flat bf16 parameter buffer and ONE flat bf16 gradient buffer (the buffer the data-parallel all-reduce and
-    the AdamW kernel operate on).  Matrices first (weight-decayed), then norm weights and biases (not decayed).
+  * ONE flat bf16 parameter buffer and ONE flat gradient buffer (the buffer the data-parallel all-reduce and the AdamW
+    kernel operate on): bf16, or fp32 after set_master_grad(True) (amp_master_grad).  Matrices first (weight-decayed), then
+    norm weights and biases (not decayed).
   * config.tie_word_embeddings: the layout has no `head` entry; the logits are hf @ E^T with E = embed [V, h]
     (llama/modeling.py:1924-1938, LlamaLMHead(transpose_y=True)) and both gradient terms land in the one embed gradient.
   * q/k/v weights are stored fused as [hidden, (nh + 2*kvh) * d] (= concat of the reference's three [in,out]
@@ -240,6 +241,28 @@ class DecoderEngine:
         """Call after the optimizer updated the flat buffer (fp32 bias copies are stale)."""
         self._bias_f32.clear()
 
+    @property
+    def master_grad(self) -> bool:
+        """True when the gradients are kept in fp32 (set_master_grad)."""
+        return self.flat_grads.dtype == torch.float32
+
+    def set_master_grad(self, enable: bool = True):
+        """amp_master_grad (reference trainer.py:1921-1960): keep the gradients in fp32 from the first write to the optimizer
+        step.  The gradient buffer is reallocated (fp32, zero) in place of the bf16 one, and backward() then writes every
+        gradient in fp32: the weight-gradient GEMMs add their fp32 results straight into it (fused_linear_param_grad_add(...,
+        multi_precision=True), llm/utils/fused_layers.py:44-50), and the embedding scatter, the norm weight and bias sums
+        likewise.  Gradient accumulation, the data-parallel exchange, clipping and AdamW then see fp32 gradients.  Layout and
+        grad_ready_hook ranges (element offsets) are unchanged.  Not allowed while a forward waits for its backward or a
+        backward's gradients wait for an optimizer step (clear_grad() first)."""
+        if self.master_grad == bool(enable):
+            return
+        if self._saved is not None or not self.grads_fresh:
+            raise RuntimeError("set_master_grad: gradients are pending (a forward without its backward, or gradients no "
+                               "optimizer step has consumed); call clear_grad() after the step first")
+        self.flat_grads = None                                       # free the old buffer before allocating the new one
+        self.flat_grads = torch.zeros(self.numel, dtype=torch.float32 if enable else BF16, device=self.device)
+        self.g = {n: self.flat_grads[o:o + math.prod(s)].view(s) for n, (o, s) in self._offsets.items()}
+
     def _rope_tables(self, need_pos: int):
         if self._rope is None or self._rope[0].shape[0] < need_pos:
             mpe = int(getattr(self.cfg, "max_position_embeddings", 0) or 0)
@@ -420,7 +443,8 @@ class DecoderEngine:
                  dlogits: Optional[torch.Tensor] = None):
         """Backward of the last forward_loss() (or forward_logits_train() + caller-supplied `dlogits` [T, V] bf16): gradients
         are accumulated into flat_grads (or overwrite it if grads_fresh).  The logits buffer is consumed (overwritten by
-        dlogits)."""
+        dlogits).  With fp32 gradients (set_master_grad) the ops below take their fp32-output forms by the dtype of the
+        gradient views; the dX GEMMs, attention and the recompute path are the same either way."""
         st = self._saved
         if st is None:
             raise RuntimeError("backward() without a preceding forward_loss()")

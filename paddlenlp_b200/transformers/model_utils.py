@@ -1,6 +1,7 @@
 """PretrainedModel base: the slice of paddlenlp/transformers/model_utils.py (:921 class, :1101 from_config-style
 construction, :1140 recompute_enable) that the decoder hot path exercises.  Parameters are torch Parameters that
-alias the engine's flat bf16 buffer; `.grad` aliases the flat gradient buffer."""
+alias the engine's flat bf16 buffer; `.grad` aliases the flat gradient buffer, or, with fp32 gradients (set_master_grad),
+`.main_grad` does and `.grad` is None."""
 from __future__ import annotations
 
 import json
@@ -163,6 +164,21 @@ class PretrainedModel(nn.Module):
 
     def num_parameters(self) -> int:
         return self.engine.num_parameters()
+
+    def set_master_grad(self, enable: bool = True):
+        """amp_master_grad: fp32 gradients (DecoderEngine.set_master_grad).  Each parameter then exposes its fp32 gradient
+        view as `main_grad` and keeps `.grad = None`, the reference's convention (trainer.py:1139-1142); torch would refuse
+        an fp32 `.grad` on a bf16 parameter anyway."""
+        self.engine.set_master_grad(enable)
+        grads = self.engine.named_views(grads=True)
+        for name, prm in self._named.items():
+            if enable:
+                prm.grad = None
+                prm.main_grad = grads[name]
+            else:
+                prm.grad = grads[name]
+                if hasattr(prm, "main_grad"):
+                    del prm.main_grad
 
     def recompute_enable(self):
         """model_utils.py:1140: activation recomputation — every decoder layer keeps only its input and is re-run in
