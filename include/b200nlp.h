@@ -270,7 +270,9 @@ int b200_decode_attention_tc(const void* qkv, const void* cache, const int32_t* 
  * csrc/gpu/append_attention.cu:428-851): key_cache / value_cache [num_blocks, kvh, block_size, head_dim] bf16,
  * block_tables [B, max_blocks_per_seq] int32 (logical block -> physical block).  Same math as the dense entry points above:
  * prefill cache fill, decode RoPE + append (acc_f32_ws / bias optional as in b200_decode_rope_append_f32), decode attention
- * (the streaming kernel reads each cache row through the block table; block_size 32, 64 or 128). */
+ * (the streaming kernel reads each cache row through the block table).  Every paged entry point, b200_append_attention
+ * included, requires block_size 32, 64 or 128 and max_blocks_per_seq > 0 and returns an argument error otherwise, so a cache
+ * that one of them fills can be read by all of them. */
 int b200_write_cache_kv_paged(const void* qkv, void* key_cache, void* value_cache, const int32_t* block_tables,
                               const int32_t* seq_lens, int64_t B, int64_t S, int64_t num_heads, int64_t num_kv_heads,
                               int64_t head_dim, int64_t block_size, int64_t max_blocks_per_seq, int64_t ld, cudaStream_t stream);

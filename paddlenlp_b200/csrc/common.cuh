@@ -359,13 +359,42 @@ __device__ __forceinline__ void swiglu_bwd_pair(uint32_t g2, uint32_t u2, float 
   du2 = pack_bf16x2(duv.x, duv.y);
 }
 
+// RoPE (rotate-half, fp32 math, one rounding) of one 8-column chunk pair of a head at position pos: a holds columns j8 .. j8 + 7
+// of the first half, b the same columns of the second half; cos / sin tables are fp32 [positions, half].
+//   first half: x1 cos - x2 sin ; second half: x2 cos + x1 sin.  sign = -1 is the backward (sin -> -sin).
+// The round-to-nearest intrinsics pin which product is fused into each FMA.  The training RoPE (rope_kernel) fuses x1 sin into
+// the second half and the decode kernels fuse x2 cos; the two forms round differently, and FUSE_SIN keeps each caller's
+// results bit for bit.
+template <bool FUSE_SIN = false>
+__device__ __forceinline__ void rope_rotate_chunk(uint4& a, uint4& b, const float* cos_t, const float* sin_t, int pos, int half,
+                                                  int j8, float sign = 1.f) {
+  const float4* c4 = reinterpret_cast<const float4*>(cos_t + static_cast<size_t>(pos) * half + j8);
+  const float4* s4 = reinterpret_cast<const float4*>(sin_t + static_cast<size_t>(pos) * half + j8);
+  const float4 c0 = __ldg(c4), c1 = __ldg(c4 + 1), s0 = __ldg(s4), s1 = __ldg(s4 + 1);
+  const float cs[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
+  const float sn[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
+  uint32_t* ai = reinterpret_cast<uint32_t*>(&a);
+  uint32_t* bi = reinterpret_cast<uint32_t*>(&b);
+  auto first = [](float x1, float x2, float c, float s) { return __fmaf_rn(x1, c, -__fmul_rn(x2, s)); };
+  auto second = [](float x1, float x2, float c, float s) {
+    return FUSE_SIN ? __fmaf_rn(x1, s, __fmul_rn(x2, c)) : __fmaf_rn(x2, c, __fmul_rn(x1, s));
+  };
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const float2 x1 = unpack_bf16x2(ai[j]), x2 = unpack_bf16x2(bi[j]);
+    const float s_lo = sign * sn[2 * j], s_hi = sign * sn[2 * j + 1];
+    ai[j] = pack_bf16x2(first(x1.x, x2.x, cs[2 * j], s_lo), first(x1.y, x2.y, cs[2 * j + 1], s_hi));
+    bi[j] = pack_bf16x2(second(x1.x, x2.x, cs[2 * j], s_lo), second(x1.y, x2.y, cs[2 * j + 1], s_hi));
+  }
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
 
-// Split-KV partials of the decode-attention kernels (decode_attn_tc.cu, generation.cu), merged by
+// Split-KV partials of the decode-attention kernels (decode_attn_tc.cu), merged by
 // decode_attention_merge_kernel: one row of DECODE_PART_ROW floats per (sequence, head, split) at every head_dim
 // (b200_decode_attention_workspace_bytes takes no head_dim), the unnormalised o in the first d columns, the running max
 // (log2 units) at column DECODE_PART_M and the sum at DECODE_PART_M + 1.  The 132-float stride keeps the merge kernel's

@@ -303,22 +303,7 @@ __global__ void rope_kernel(bf16* __restrict__ x, const float* __restrict__ cos_
   bf16* base = x + static_cast<size_t>(tok) * ld + head * head_dim;
   uint4 a = *reinterpret_cast<const uint4*>(base + j8);
   uint4 b = *reinterpret_cast<const uint4*>(base + half + j8);
-  const float4* c4 = reinterpret_cast<const float4*>(cos_t + static_cast<size_t>(pos) * half + j8);
-  const float4* s4 = reinterpret_cast<const float4*>(sin_t + static_cast<size_t>(pos) * half + j8);
-  const float4 c0 = __ldg(c4), c1 = __ldg(c4 + 1), s0 = __ldg(s4), s1 = __ldg(s4 + 1);
-  const float cs[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
-  const float sn[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
-  uint32_t* ai = reinterpret_cast<uint32_t*>(&a);
-  uint32_t* bi = reinterpret_cast<uint32_t*>(&b);
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const float2 x1 = unpack_bf16x2(ai[j]);
-    const float2 x2 = unpack_bf16x2(bi[j]);
-    const float s_lo = sign * sn[2 * j], s_hi = sign * sn[2 * j + 1];
-    // first half:  x1*cos - x2*sin ; second half: x2*cos + x1*sin
-    ai[j] = pack_bf16x2(x1.x * cs[2 * j] - x2.x * s_lo, x1.y * cs[2 * j + 1] - x2.y * s_hi);
-    bi[j] = pack_bf16x2(x2.x * cs[2 * j] + x1.x * s_lo, x2.y * cs[2 * j + 1] + x1.y * s_hi);
-  }
+  rope_rotate_chunk<true>(a, b, cos_t, sin_t, pos, half, j8, sign);
   *reinterpret_cast<uint4*>(base + j8) = a;
   *reinterpret_cast<uint4*>(base + half + j8) = b;
 }

@@ -29,6 +29,7 @@
 #include "../../include/b200nlp.h"
 #include "common.cuh"
 #include "host_util.h"
+#include "kv_cache.cuh"
 
 namespace b200 {
 namespace fa {
@@ -57,13 +58,12 @@ struct Params {
   const int* mask_start;
   // PAGED (prefill half of append_attention, csrc/gpu/append_attention.cu:428-851): sequence b contributes seq_this[b] new query
   // rows (token rows cu_q[b] .. of the packed projection) at absolute positions seq_dec[b] + i and attends to cache positions
-  // [0, seq_dec[b] + i] of its pages; key/value caches [num_blocks, kvh, block_size, D]
+  // [0, seq_dec[b] + i] of the paged cache `kv` (k and v above are not used)
   const int* cu_q;
   const int* seq_dec;
   const int* seq_this;
   const int* seq_enc;
-  const int* block_tables;
-  int max_blocks, block_size;
+  KvCache kv;
 };
 
 // With a document mask the leading kv tiles whose every column belongs to a document that ended at or before the q tile's
@@ -108,20 +108,18 @@ __global__ void __launch_bounds__(NW * 32, 1) fa_fwd_kernel(const Params p) {
   int j_lo = 0;
   if constexpr (MODE == MASK) j_lo = first_visible_kv_tile(p.mask_start + static_cast<size_t>(batch) * p.S, p.S, q0, n_kv, BKV);
 
+  const bf16* kbase = MODE == PAGED ? p.kv.k : p.k;
+  const bf16* vbase = MODE == PAGED ? p.kv.v : p.v;
   auto kv_row = [&](const bf16* base, int64_t ld, int c) -> const bf16* {
-    if constexpr (MODE == PAGED) {
-      const int page = __ldg(p.block_tables + static_cast<size_t>(batch) * p.max_blocks + c / p.block_size);
-      return base + ((static_cast<size_t>(page) * p.kvh + kv_head) * p.block_size + c % p.block_size) * D;
-    } else {
-      return base + static_cast<size_t>(tok0 + c) * ld + kv_head * D;
-    }
+    if constexpr (MODE == PAGED) return base + p.kv.offset<true, D>(batch, kv_head, c);
+    else return base + static_cast<size_t>(tok0 + c) * ld + kv_head * D;
   };
   auto load_kv = [&](int j, int buf) {
     for (int i = threadIdx.x; i < BKV * CH; i += NW * 32) {
       const int r = i >> CH_LOG2, ch = i & (CH - 1), c = j * BKV + r;
       const bool ok = c < kv_total;
-      cp_async_16(sK + buf * KV_TILE_BYTES + swz<D>(r, ch), ok ? kv_row(p.k, p.ldk, c) + ch * 8 : p.k, ok ? 16u : 0u);
-      cp_async_16(sV + buf * KV_TILE_BYTES + swz<D>(r, ch), ok ? kv_row(p.v, p.ldv, c) + ch * 8 : p.v, ok ? 16u : 0u);
+      cp_async_16(sK + buf * KV_TILE_BYTES + swz<D>(r, ch), ok ? kv_row(kbase, p.ldk, c) + ch * 8 : kbase, ok ? 16u : 0u);
+      cp_async_16(sV + buf * KV_TILE_BYTES + swz<D>(r, ch), ok ? kv_row(vbase, p.ldv, c) + ch * 8 : vbase, ok ? 16u : 0u);
     }
   };
   for (int i = threadIdx.x; i < BQ * CH; i += NW * 32) {
@@ -531,29 +529,23 @@ static int launch(const CUtensorMap (&tm)[3], const Params& p, cudaStream_t stre
 }  // namespace fa
 
 // Prefill half of append_attention: causal attention of the NEW token rows of every prompt / prompt-chunk sequence over its paged
-// cache (cached prefix + the rows themselves, already appended).  qkv: packed projection [token_num, ldq] (q heads first, rotated);
-// key / value caches [num_blocks, kvh, block_size, head_dim]; out [token_num, ldo].  max_q_len bounds seq_lens_this_time (grid
-// size).  head_dim is 64 or 128 (checked by the caller).
-int launch_fa_prefill_paged(const void* qkv, const void* key_cache, const void* value_cache, void* out, const int32_t* cu_seqlens_q,
+// cache `kv` (cached prefix + the rows themselves, already appended).  qkv: packed projection [token_num, ldq] (q heads first,
+// rotated); out [token_num, ldo].  max_q_len bounds seq_lens_this_time (grid size).  kv.d is 64 or 128 (checked by the caller).
+int launch_fa_prefill_paged(const KvCache& kv, const void* qkv, void* out, const int32_t* cu_seqlens_q,
                             const int32_t* seq_lens_encoder, const int32_t* seq_lens_decoder, const int32_t* seq_lens_this_time,
-                            const int32_t* block_tables, int64_t B, int64_t token_num, int64_t max_q_len, int64_t num_heads,
-                            int64_t num_kv_heads, int64_t head_dim, int64_t num_blocks, int64_t block_size, int64_t max_blocks_per_seq, int64_t ldq,
-                            int64_t ldo, float softmax_scale, cudaStream_t stream) {
+                            int64_t B, int64_t max_q_len, int64_t num_heads, int64_t ldq, int64_t ldo, float softmax_scale,
+                            cudaStream_t stream) {
   using namespace fa;
-  (void)token_num; (void)num_blocks;
   Params p = {};
   p.q = static_cast<const bf16*>(qkv);
-  p.k = static_cast<const bf16*>(key_cache);
-  p.v = static_cast<const bf16*>(value_cache);
   p.o = static_cast<bf16*>(out);
   p.ldq = ldq; p.ldo = ldo;
   p.S = static_cast<int>(max_q_len); p.B = static_cast<int>(B); p.nh = static_cast<int>(num_heads);
-  p.kvh = static_cast<int>(num_kv_heads);
+  p.kvh = kv.kvh;
   p.scale_log2 = softmax_scale * 1.4426950408889634f;
   p.cu_q = cu_seqlens_q; p.seq_dec = seq_lens_decoder; p.seq_this = seq_lens_this_time; p.seq_enc = seq_lens_encoder;
-  p.block_tables = block_tables;
-  p.max_blocks = static_cast<int>(max_blocks_per_seq); p.block_size = static_cast<int>(block_size);
-  if (head_dim == 64) return launch<64, PAGED>(p, static_cast<int>(max_q_len), stream);
+  p.kv = kv;
+  if (kv.d == 64) return launch<64, PAGED>(p, static_cast<int>(max_q_len), stream);
   return launch<128, PAGED>(p, static_cast<int>(max_q_len), stream);
 }
 

@@ -17,12 +17,17 @@ int check_launch(const char* what);  // cudaGetLastError() -> return code
 int sm_count();  // multiprocessors of the current device (cached per device)
 int fa_fwd_impl();         // b200_set_fa_fwd_impl(): 2 = wgmma kernel, 1 = mma.sync kernel (cross-check)
 int fa_bwd_impl();         // b200_set_fa_bwd_impl(): 2 = wgmma kernel, 1 = mma.sync kernel (cross-check)
-// fa_fwd.cu, paged instantiation: prefill half of b200_append_attention
-int launch_fa_prefill_paged(const void* qkv, const void* key_cache, const void* value_cache, void* out, const int32_t* cu_seqlens_q,
+// Attention launchers over a KV cache view (kv_cache.cuh); the prefill one serves b200_append_attention
+struct KvCache;
+int launch_fa_prefill_paged(const KvCache& kv, const void* qkv, void* out, const int32_t* cu_seqlens_q,
                             const int32_t* seq_lens_encoder, const int32_t* seq_lens_decoder, const int32_t* seq_lens_this_time,
-                            const int32_t* block_tables, int64_t B, int64_t token_num, int64_t max_q_len, int64_t num_heads,
-                            int64_t num_kv_heads, int64_t head_dim, int64_t num_blocks, int64_t block_size,
-                            int64_t max_blocks_per_seq, int64_t ldq, int64_t ldo, float softmax_scale, cudaStream_t stream);
+                            int64_t B, int64_t max_q_len, int64_t num_heads, int64_t ldq, int64_t ldo, float softmax_scale,
+                            cudaStream_t stream);   // fa_fwd.cu
+// decode_attn_tc.cu, dense or paged view: the checks (message names `what`), then the launch of checked arguments
+int check_decode_attention(const char* what, const KvCache& kv, const void* qkv, const int32_t* seq_lens, const void* out,
+                           const void* workspace, int64_t B, int64_t num_heads, int64_t ld, int64_t num_splits);
+int launch_decode_attention(const KvCache& kv, const void* qkv, const int32_t* seq_lens, void* out, void* workspace, int64_t B,
+                            int64_t num_heads, int64_t ld, float softmax_scale, int64_t num_splits, cudaStream_t stream);
 bool pdl_enabled();   // b200_set_pdl(): launch GEMMs with programmatic dependent launch (decode-step kernel chains)
 
 // Launch `kern` on `stream`; when PDL is enabled the launch carries the programmatic-stream-serialization attribute, so the

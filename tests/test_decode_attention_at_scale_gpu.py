@@ -1,7 +1,7 @@
 """Decode and append attention per (sequence, head) against fp64, at every shipped preset's GQA ratio.
 
 The decode kernels (the bulk-copy kernel of decode_attn_tc.cu over the dense and the paged cache, and the CUDA-core kernel
-of generation.cu that cross-checks it) and append_attention stream the cache in 32-row chunks, clamp the length to
+in decode_attn_tc.cu that cross-checks it) and append_attention stream the cache in 32-row chunks, clamp the length to
 seq_lens + 1 and split long sequences across CTAs.  The bugs such code grows (a dropped partial chunk, rows attended past
 the length, the new token left out, a lost split, the wrong kv head) move a long sequence's output by a small amount in
 absolute terms, because that output is an average of thousands of V rows (elements ~0.04) while a sequence with no
