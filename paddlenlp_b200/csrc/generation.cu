@@ -390,10 +390,15 @@ __global__ void update_inputs_kernel(bool* not_need_stop, int* seq_lens_this_tim
 }
 
 // One fused per-step state update for the dense-cache generate loop
-// (GenerationInferenceModel.update_model_kwargs_for_generation, experimental/transformers/generation_utils.py:185-260):
-//   step_idx += !stop ; stop |= step_idx >= max_dec_len ; next = stop ? eos[0] : next ; stop |= next in eos ;
-//   pre_ids[b, step_idx] = next (set_value_by_flags_and_idx of the following step) ; seq_len_decoder += !stop ;
-//   tgt_ids = next ; stop_count = sum(stop)
+// (GenerationInferenceModel.update_model_kwargs_for_generation, experimental/transformers/generation_utils.py:185-260).
+// `was` is the stop flag on entry:
+//   step_idx += !was ; next = was ? eos[0] : next ; stop = was || step_idx >= max_dec_len || next in eos ;
+//   if !was: pre_ids[b, step_idx] = next (set_value_by_flags_and_idx of the following step) ; seq_len_decoder += !stop ;
+//   tgt_ids = next ; out_tokens[b, col] = next ; stop_count = sum(stop)
+// Only a row stopped before this call emits eos[0].  A row whose step reaches max_dec_len here keeps (and records) the token it
+// chose: the last generated token is a real one, as in oracle/generation_ref.greedy_generate.  This differs on purpose from
+// the reference, which sets the max_dec_len flag first (generation_utils.py:185-205) and then substitutes eos for every flagged
+// row (stop_generation_multi_ends.cu:48).
 __global__ void generate_step_update_kernel(int64_t* next_tokens, bool* stop_flags, int64_t* step_idx,
                                             const int64_t* max_dec_len, int* seq_len_decoder, int64_t* pre_ids,
                                             int64_t pre_len, const int64_t* eos_ids, int eos_len, int64_t* out_tokens,

@@ -107,19 +107,6 @@ def test_rebuild_padding_vs_oracle():
     assert np.array_equal(out.float().cpu().numpy(), ref)
 
 
-def test_add_rmsnorm():
-    o = ops()
-    g = torch.Generator().manual_seed(0)
-    x = torch.randn(70, 4096, generator=g).to(BF16)
-    r = torch.randn(70, 4096, generator=g).to(BF16)
-    w = (1 + 0.1 * torch.randn(4096, generator=g)).to(BF16)
-    n, ro = o.add_rmsnorm(x.to(DEV), r.to(DEV), w.to(DEV), 1e-5)
-    rr = (x.float() + r.float()).to(BF16).float()
-    ref = R.rms_norm(rr, w.float(), 1e-5, "bf16")
-    assert torch.equal(ro.float().cpu(), rr)
-    assert (n.float().cpu() != ref).float().mean().item() < 0.01
-
-
 @pytest.mark.parametrize("impl", ["tc", "simt"])
 @pytest.mark.parametrize("nh,kvh", [(4, 1), (8, 2), (7, 1)])
 def test_decode_rope_append_and_attention(nh, kvh, impl):
