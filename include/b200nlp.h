@@ -341,6 +341,48 @@ int b200_step_paddle(bool* stop_flags, int32_t* seq_lens_this_time, const int32_
                      int64_t block_num_per_seq, int64_t length, int64_t pre_id_length, int64_t first_token_id,
                      cudaStream_t stream);
 
+/* retire_admit: the continuous-batching step step_paddle leaves to its caller (the reference's serving stack does it on the
+ * host); call it right after b200_step_paddle on the same state, with a device-resident request queue: prompt_ids int64 packed,
+ * prompt_offsets int32 [num_requests + 1], req_max_dec_len / req_min_dec_len int64 [num_requests], *cursor = next request.
+ *   - a slot step_paddle recovered this step gets input_ids[b, 0] = its prompt's first token back;
+ *   - a parked slot (is_block_step) returns its encoder blocks to free_list and adds them to used_list_len, so that
+ *     step_paddle's recovery re-attaches all of its pages from position 0;
+ *   - a stopped, not parked slot with slot_request[b] = r >= 0 retires: out_ids[r, :n] = pre_ids[b, 1:n] + next_tokens[b] with
+ *     n = step_idx[b], out_lens[r] = n, the encoder blocks left in its row (step_paddle freed the decoder blocks and zeroed
+ *     encoder_block_lens) back to free_list, slot_request = -1;
+ *   - while no slot is parked (*step_lens == 0), empty slots take requests FIFO, in slot order, while the free list holds
+ *     ceil(prompt / block_size) blocks for the head request (popped from its tail): input_ids row, seq_lens_this_time =
+ *     seq_lens_encoder = ori_seq_lens_encoder = prompt, seq_lens_decoder = step_idx = 0, stop flag cleared, pre_ids row = -1,
+ *     max/min_dec_len, slot_request;
+ *   - header (int32 [B200_RA_HEADER_INTS], pinned device-mapped host memory, zeroed before the first call) receives the next
+ *     step's token_num / max_q_len and the counters below.
+ * One CTA (bsz <= 1024), list positions by prefix sums in slot order, no host synchronisation, graph-replayable.
+ * max_prompt_len / max_seq_len = the queue's longest prompt / prompt + max_dec_len (host bounds, checked against the table
+ * and input_ids widths); out_stride >= every max_dec_len, pre_id_length >= out_stride. */
+enum {
+  B200_RA_TOKEN_NUM = 0,    /* sum of seq_lens_this_time: rows of the next step */
+  B200_RA_MAX_Q_LEN = 1,    /* max of seq_lens_this_time (1: a decode-only step) */
+  B200_RA_RUNNING = 2,      /* slots with seq_lens_this_time > 0 */
+  B200_RA_PENDING = 3,      /* requests not yet admitted */
+  B200_RA_PARKED = 4,       /* *step_lens */
+  B200_RA_DONE = 5,         /* 1 once every request has retired */
+  B200_RA_FREE_BLOCKS = 6,  /* *free_list_len */
+  B200_RA_PREEMPTIONS = 7,  /* cumulative over the calls since the header was zeroed */
+  B200_RA_RECOVERIES = 8,   /* cumulative */
+  B200_RA_ADMITTED = 9,     /* this call */
+  B200_RA_RETIRED = 10,     /* this call */
+  B200_RA_HEADER_INTS = 16
+};
+int b200_retire_admit(bool* stop_flags, bool* is_block_step, int32_t* seq_lens_this_time, int32_t* seq_lens_encoder,
+                      int32_t* ori_seq_lens_encoder, int32_t* seq_lens_decoder, int64_t* step_idx, int64_t* pre_ids,
+                      const int64_t* next_tokens, int64_t* input_ids, int32_t* block_tables, int32_t* encoder_block_lens,
+                      int32_t* used_list_len, int32_t* free_list, int32_t* free_list_len, const int32_t* step_lens,
+                      int64_t* max_dec_len, int64_t* min_dec_len, int32_t* slot_request, const int64_t* prompt_ids,
+                      const int32_t* prompt_offsets, const int64_t* req_max_dec_len, const int64_t* req_min_dec_len,
+                      int32_t* cursor, int64_t* out_ids, int32_t* out_lens, int32_t* header, int64_t bsz, int64_t block_size,
+                      int64_t block_num_per_seq, int64_t length, int64_t pre_id_length, int64_t num_requests,
+                      int64_t out_stride, int64_t max_prompt_len, int64_t max_seq_len, cudaStream_t stream);
+
 /* save_output(x, not_need_stop, rank_id) replacement: csrc/gpu/save_with_output_msg.cc:28-52 (producer) / csrc/gpu/get_output.cc
  * (consumer), reader loop paddlenlp/utils/llm_utils.py:753-776.  Writes the step's message {flag, bsz, tokens...} (flag 1 =
  * running, -1 = finished: *stop_count >= bs or step >= last_step) into slot (step % num_slots) of `ring`, an int32 buffer of

@@ -84,6 +84,7 @@ _SIGNATURES = {
     "b200_set_stop_value_multi_ends": [P, P, P, P, P, I64, I64, I, P],
     "b200_fused_get_rotary_embedding": [P, P, I64, I64, I64, I64, I64, F, I, P],
     "b200_step_paddle": [P] * 21 + [I64] * 6 + [P],
+    "b200_retire_admit": [P] * 27 + [I64] * 9 + [P],
     "b200_save_output_stream": [P, P, P, I64, I64, P, I64, I64, P],
     "b200_append_attention_workspace_bytes": [I64, I64, I64, I64, I64],
     "b200_append_attention": [P] * 12 + [I64] * 12 + [F, I64, P],

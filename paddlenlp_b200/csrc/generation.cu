@@ -1156,6 +1156,191 @@ extern "C" int b200_step_paddle(bool* stop_flags, int32_t* seq_lens_this_time, c
 }
 
 // ------------------------------------------------------------------------------------------------------------------
+// retire_admit: the continuous-batching half step_paddle leaves to its caller, run right after it every step.  One CTA, one
+// thread per slot, list positions from prefix sums in slot order (deterministic), no host synchronisation.
+//   0. a slot recovered by step_paddle this step gets its first prompt token back in input_ids[b, 0] (update_inputs wrote the
+//      last generated token there; step_paddle restores one first_token_id for every slot)
+//   1. a parked slot (is_block_step) hands its encoder blocks back too and counts them as decoder blocks: step_paddle then
+//      recovers it with a fresh table of used + 1 blocks from position 0.  A parked slot so holds no block, and a pool of at
+//      least the largest request's pages can always recover the last-parked sequence once nothing else runs.
+//   2. a slot that stopped (and is not parked) retires: its tokens pre_ids[b, 1 .. step_idx-1] + next_tokens[b] go to row
+//      slot_request[b] of out_ids, its encoder blocks to the free list (step_paddle freed the decoder blocks and zeroed
+//      encoder_block_lens, leaving the encoder blocks in the row), the slot empties
+//   3. FIFO admission while no sequence is parked: the k-th empty slot takes request cursor + k if the free list holds the
+//      blocks of it and of every request before it, and the pool keeps one spare block per resident slot; the blocks are
+//      popped from the tail of the free list
+//   4. the step header in (pinned, device-mapped) host memory
+// ------------------------------------------------------------------------------------------------------------------
+namespace b200 {
+namespace gen {
+
+__global__ void __launch_bounds__(STEP_THREADS, 1)
+retire_admit_kernel(bool* stop_flags, bool* is_block_step, int* seq_lens_this_time, int* seq_lens_encoder,
+                    int* ori_seq_lens_encoder, int* seq_lens_decoder, int64_t* step_idx, int64_t* pre_ids,
+                    const int64_t* next_tokens, int64_t* input_ids, int* block_tables, int* encoder_block_lens, int* used_list_len,
+                    int* free_list, int* free_list_len, const int* step_lens, int64_t* max_dec_len, int64_t* min_dec_len,
+                    int* slot_request, const int64_t* prompt_ids, const int* prompt_offsets, const int64_t* req_max_dec_len,
+                    const int64_t* req_min_dec_len, int* cursor, int64_t* out_ids, int* out_lens, volatile int* header, int bsz,
+                    int block_size, int block_num_per_seq, int length, int pre_id_length, int num_requests, int out_stride) {
+  __shared__ int s_warp[32];
+  __shared__ int s_slot[STEP_THREADS], s_req[STEP_THREADS];
+  __shared__ int s_max_q;
+  const int tid = threadIdx.x;
+  const bool valid = tid < bsz;
+  int* tbl = block_tables + static_cast<int64_t>(valid ? tid : 0) * block_num_per_seq;
+  if (tid == 0) s_max_q = 0;
+  const int req = valid ? slot_request[tid] : -1;
+
+  // ---- 0 / 1 / 2: recovered, parked and retiring slots ----
+  const bool parked = valid && is_block_step[tid];
+  const bool retire = valid && req >= 0 && stop_flags[tid] && !parked;
+  const bool recovered = valid && req >= 0 && !stop_flags[tid] && seq_lens_encoder[tid] > 0 && step_idx[tid] > 0;
+  if (recovered) input_ids[static_cast<int64_t>(tid) * length] = prompt_ids[prompt_offsets[req]];
+  // the blocks a parked or stopped slot still holds are its encoder blocks, a prefix of its row: step_paddle cleared the
+  // decoder entries (and, for a stopped slot, zeroed encoder_block_lens too)
+  int n_push = 0;
+  if (parked || retire)
+    while (n_push < block_num_per_seq && tbl[n_push] >= 0) ++n_push;
+  int total_push;
+  const int push_pos = block_exclusive_scan(n_push, s_warp, &total_push);
+  const int free0 = *free_list_len;
+  for (int i = 0; i < n_push; ++i) {
+    free_list[free0 + push_pos + i] = tbl[i];
+    tbl[i] = -1;
+  }
+  if (parked || retire) encoder_block_lens[tid] = 0;
+  if (parked) used_list_len[tid] += n_push;
+  if (retire) slot_request[tid] = -1;
+  int n_retire;
+  const int rpos = block_exclusive_scan(retire ? 1 : 0, s_warp, &n_retire);
+  if (retire) { s_slot[rpos] = tid; s_req[rpos] = req; }
+  int n_recovered;
+  block_exclusive_scan(recovered ? 1 : 0, s_warp, &n_recovered);
+  __syncthreads();
+  for (int k = 0; k < n_retire; ++k) {
+    const int b = s_slot[k], r = s_req[k];
+    int n = static_cast<int>(step_idx[b]);
+    n = n < out_stride ? n : out_stride;
+    const int64_t* pre = pre_ids + static_cast<int64_t>(b) * pre_id_length;
+    int64_t* out = out_ids + static_cast<int64_t>(r) * out_stride;
+    for (int i = tid; i < n; i += STEP_THREADS) out[i] = i + 1 < n ? pre[i + 1] : next_tokens[b];
+    if (tid == 0) out_lens[r] = n;
+  }
+
+  // ---- 3: FIFO admission into the empty slots, in slot order ----
+  const int free1 = free0 + total_push;
+  const int cur = *cursor;
+  const bool empty = valid && (retire || req < 0);
+  int n_empty, occupied0, held_dec;
+  const int epos = block_exclusive_scan(empty ? 1 : 0, s_warp, &n_empty);
+  block_exclusive_scan(valid && !empty ? 1 : 0, s_warp, &occupied0);
+  block_exclusive_scan(valid && !empty && !parked ? used_list_len[tid] : 0, s_warp, &held_dec);
+  const int r = cur + epos;
+  const bool cand = empty && *step_lens == 0 && r < num_requests;
+  const int plen = cand ? prompt_offsets[r + 1] - prompt_offsets[r] : 0;
+  const int need = (plen + block_size - 1) / block_size;
+  int total_need;
+  const int excl = block_exclusive_scan(need, s_warp, &total_need);
+  // the blocks must be free now, and the pool must keep one block per resident slot beyond every encoder block: step_paddle
+  // can only pre-empt decoder blocks, so a step in which each resident asks for one more block is always served.  Needs are
+  // >= 1 and the candidates a prefix of the empty slots: the admitted are a prefix too (epos = admissions before this one)
+  const bool admit = cand && excl + need <= free1 && excl + need + occupied0 + epos + 1 <= free1 + held_dec;
+  int n_admit;
+  block_exclusive_scan(admit ? 1 : 0, s_warp, &n_admit);
+  int popped;
+  block_exclusive_scan(admit ? need : 0, s_warp, &popped);
+  if (admit) {
+    for (int j = 0; j < need; ++j) tbl[j] = free_list[free1 - 1 - excl - j];
+    encoder_block_lens[tid] = need;
+    used_list_len[tid] = 0;
+    seq_lens_this_time[tid] = plen;
+    seq_lens_encoder[tid] = plen;
+    ori_seq_lens_encoder[tid] = plen;
+    seq_lens_decoder[tid] = 0;
+    step_idx[tid] = 0;
+    stop_flags[tid] = false;
+    max_dec_len[tid] = req_max_dec_len[r];
+    min_dec_len[tid] = req_min_dec_len[r];
+    slot_request[tid] = r;
+    s_slot[epos] = tid;
+    s_req[epos] = r;
+  }
+  __syncthreads();
+  for (int k = 0; k < n_admit; ++k) {
+    const int b = s_slot[k], rq = s_req[k];
+    const int64_t* src = prompt_ids + prompt_offsets[rq];
+    const int n = prompt_offsets[rq + 1] - prompt_offsets[rq];
+    int64_t* ids = input_ids + static_cast<int64_t>(b) * length;
+    for (int i = tid; i < n; i += STEP_THREADS) ids[i] = src[i];
+    int64_t* pre = pre_ids + static_cast<int64_t>(b) * pre_id_length;
+    for (int i = tid; i < pre_id_length; i += STEP_THREADS) pre[i] = -1;
+  }
+
+  // ---- 4: step header ----
+  const int this_time = valid ? seq_lens_this_time[tid] : 0;
+  if (this_time > 0) atomicMax(&s_max_q, this_time);
+  int token_num, running, occupied;
+  block_exclusive_scan(this_time, s_warp, &token_num);
+  block_exclusive_scan(this_time > 0 ? 1 : 0, s_warp, &running);
+  block_exclusive_scan(valid && slot_request[tid] >= 0 ? 1 : 0, s_warp, &occupied);
+  __syncthreads();
+  if (tid == 0) {
+    const int new_cursor = cur + n_admit;
+    const int parked_now = *step_lens;
+    *cursor = new_cursor;
+    *free_list_len = free1 - popped;
+    header[B200_RA_PREEMPTIONS] = header[B200_RA_PREEMPTIONS] + parked_now - header[B200_RA_PARKED] + n_recovered;
+    header[B200_RA_RECOVERIES] = header[B200_RA_RECOVERIES] + n_recovered;
+    header[B200_RA_TOKEN_NUM] = token_num;
+    header[B200_RA_MAX_Q_LEN] = s_max_q;
+    header[B200_RA_RUNNING] = running;
+    header[B200_RA_PENDING] = num_requests - new_cursor;
+    header[B200_RA_PARKED] = parked_now;
+    header[B200_RA_FREE_BLOCKS] = free1 - popped;
+    header[B200_RA_ADMITTED] = n_admit;
+    header[B200_RA_RETIRED] = n_retire;
+    header[B200_RA_DONE] = (occupied == 0 && new_cursor >= num_requests) ? 1 : 0;
+    __threadfence_system();
+  }
+}
+}  // namespace gen
+}  // namespace b200
+
+extern "C" int b200_retire_admit(bool* stop_flags, bool* is_block_step, int32_t* seq_lens_this_time, int32_t* seq_lens_encoder,
+                                 int32_t* ori_seq_lens_encoder, int32_t* seq_lens_decoder, int64_t* step_idx, int64_t* pre_ids,
+                                 const int64_t* next_tokens, int64_t* input_ids, int32_t* block_tables, int32_t* encoder_block_lens,
+                                 int32_t* used_list_len, int32_t* free_list, int32_t* free_list_len, const int32_t* step_lens,
+                                 int64_t* max_dec_len, int64_t* min_dec_len, int32_t* slot_request, const int64_t* prompt_ids,
+                                 const int32_t* prompt_offsets, const int64_t* req_max_dec_len, const int64_t* req_min_dec_len,
+                                 int32_t* cursor, int64_t* out_ids, int32_t* out_lens, int32_t* header, int64_t bsz,
+                                 int64_t block_size, int64_t block_num_per_seq, int64_t length, int64_t pre_id_length,
+                                 int64_t num_requests, int64_t out_stride, int64_t max_prompt_len, int64_t max_seq_len,
+                                 cudaStream_t stream) {
+  using namespace b200;
+  B200_CHECK_ARG(stop_flags && is_block_step && seq_lens_this_time && seq_lens_encoder && ori_seq_lens_encoder && seq_lens_decoder &&
+                     step_idx && pre_ids && next_tokens && input_ids && block_tables && encoder_block_lens && used_list_len &&
+                     free_list && free_list_len && step_lens && max_dec_len && min_dec_len && slot_request && prompt_ids &&
+                     prompt_offsets && req_max_dec_len && req_min_dec_len && cursor && out_ids && out_lens && header,
+                 "retire_admit: null pointer");
+  B200_CHECK_ARG(bsz > 0 && bsz <= gen::STEP_THREADS, "retire_admit: need 0 < bsz <= %d (got %lld)", gen::STEP_THREADS,
+                 (long long)bsz);
+  B200_CHECK_ARG(block_size > 0 && block_num_per_seq > 0 && num_requests > 0 && out_stride > 0 && max_prompt_len > 0 &&
+                     max_seq_len >= max_prompt_len && pre_id_length >= out_stride,
+                 "retire_admit: need positive sizes, max_seq_len >= max_prompt_len and pre_id_length >= out_stride");
+  B200_CHECK_ARG(max_prompt_len <= block_num_per_seq * block_size,
+                 "retire_admit: a prompt of %lld tokens does not fit block_num_per_seq %lld x block_size %lld",
+                 (long long)max_prompt_len, (long long)block_num_per_seq, (long long)block_size);
+  B200_CHECK_ARG(max_seq_len <= length, "retire_admit: input_ids rows of %lld tokens are too narrow for prompt + max length %lld",
+                 (long long)length, (long long)max_seq_len);
+  gen::retire_admit_kernel<<<1, gen::STEP_THREADS, 0, stream>>>(
+      stop_flags, is_block_step, seq_lens_this_time, seq_lens_encoder, ori_seq_lens_encoder, seq_lens_decoder, step_idx, pre_ids,
+      next_tokens, input_ids, block_tables, encoder_block_lens, used_list_len, free_list, free_list_len, step_lens, max_dec_len,
+      min_dec_len, slot_request, prompt_ids, prompt_offsets, req_max_dec_len, req_min_dec_len, cursor, out_ids, out_lens, header,
+      (int)bsz, (int)block_size, (int)block_num_per_seq, (int)length, (int)pre_id_length, (int)num_requests, (int)out_stride);
+  return check_launch("retire_admit");
+}
+
+// ------------------------------------------------------------------------------------------------------------------
 // save_output / get_output replacement (csrc/gpu/save_with_output_msg.cc:28-52, csrc/gpu/get_output.cc:28-60).
 // The reference copies the step's tokens to the host synchronously (two blocking D2H copies per decode step) and pushes them
 // into a SysV message queue as  int mtext[MAX_BSZ + 2] = {not_need_stop ? 1 : -1, bsz, tokens...}.  Here the decode step's own

@@ -235,6 +235,14 @@ class FusedBlockMultiTransformer(FusedMultiTransformerBase):
                                     self.nh, max_q_len=S)
 
     def compute_fmha(self, qkv, caches, i, B, S, seq_lens_encoder, kw):
+        packed = kw.get("packed")
+        if packed is not None:
+            # continuous batching: rows are already packed (get_padding_offset) — prompts, recovered sequences and decode rows
+            # of one step in one call; packed = (seq_lens_encoder, seq_lens_decoder, seq_lens_this_time, cu_seqlens_q, max_q_len)
+            enc, dec, this_time, cu, max_q_len = packed
+            cos, sin = self.rope
+            return ops.append_attention(qkv, caches[2 * i], caches[2 * i + 1], enc, dec, this_time, cu, self._tables(kw), cos, sin,
+                                        self.nh, max_q_len=max_q_len)
         if not self.config.append_attn:
             return super().compute_fmha(qkv, caches, i, B, S, seq_lens_encoder, kw)
         enc = (seq_lens_encoder if seq_lens_encoder is not None

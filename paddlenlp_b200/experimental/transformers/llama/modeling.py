@@ -137,6 +137,15 @@ class LlamaForCausalLMInferenceModel(GenerationInferenceModel):
                                         **self._cache_kw())
         return self._head(hidden)
 
+    def _forward_packed(self, ids, caches, block_tables, enc, dec, this_time, cu_seqlens_q, cum_offsets, max_q_len, max_len):
+        """One continuous-batching step over the packed rows `ids` [token_num] of every slot (append_attention), then each
+        slot's last row (rebuild_padding; an idle slot gives a zero row) through the head: logits [slots, V]."""
+        emb = ops.embedding_fwd(ids, self.embed_tokens)
+        hidden = self.transformer_block(emb, caches, B=this_time.numel(), S=0, block_tables=block_tables,
+                                        packed=(enc, dec, this_time, cu_seqlens_q, max_q_len))
+        last = ops.rebuild_padding(hidden, cum_offsets, dec, enc, max_len)
+        return self._head(last, decode=max_q_len == 1)
+
     @torch.no_grad()
     def forward_logits_prefill(self, input_ids):
         """All-position logits of the prefill pass (parity checks against the training-path forward)."""

@@ -168,6 +168,13 @@ def gemm_skinny(a: torch.Tensor, b: torch.Tensor, out: Optional[torch.Tensor] = 
     return out
 
 
+def reserve_gemm_skinny_workspace(max_rows: int, max_cols: int, device) -> None:
+    """Size gemm_skinny's split-K workspace for every call up to max_rows x max_cols now.  The buffer grows with the row
+    count, and a CUDA graph captured later bakes in its address: it must not be reallocated while such a graph lives."""
+    device = torch.empty(0, device=device).device        # the key gemm_skinny uses: a tensor's device, index included
+    _zero_workspace(int(max_rows) * int(max_cols) * 4, device, "splitk")
+
+
 def gemm_skinny_f32(a: torch.Tensor, b: torch.Tensor, *, trans_b: bool = False, split_k: int = 0, tag: str = "splitk_f32"):
     """Split-K GEMM that leaves its result as fp32 sums in a (zero-on-entry) workspace [M, N]; the consumer kernel
     (add_rmsnorm_f32 / decode_rope_append_f32) rounds once and re-zeroes it.  Returns the fp32 workspace view."""
@@ -766,6 +773,32 @@ def step_paddle(stop_flags, seq_lens_this_time, ori_seq_lens_encoder, seq_lens_e
          ptr(recover_block_list), ptr(recover_lens), ptr(need_block_list), ptr(need_block_len), ptr(used_list_len), ptr(free_list),
          ptr(free_list_len), ptr(input_ids), ptr(pre_ids), ptr(step_idx), ptr(next_tokens), bsz, int(block_size),
          block_tables.shape[1], input_ids.shape[1], pre_ids.shape[1], int(first_token_id), stream_ptr())
+
+
+RETIRE_ADMIT_ORDER = ("stop_flags", "is_block_step", "seq_lens_this_time", "seq_lens_encoder", "ori_seq_lens_encoder",
+                      "seq_lens_decoder", "step_idx", "pre_ids", "next_tokens", "input_ids", "block_tables", "encoder_block_lens",
+                      "used_list_len", "free_list", "free_list_len", "step_lens", "max_dec_len", "min_dec_len", "slot_request",
+                      "prompt_ids", "prompt_offsets", "req_max_dec_len", "req_min_dec_len", "cursor", "out_ids", "out_lens")
+# int32 words of the step header retire_admit writes (enum B200_RA_* of include/b200nlp.h)
+RA_TOKEN_NUM, RA_MAX_Q_LEN, RA_RUNNING, RA_PENDING, RA_PARKED, RA_DONE, RA_FREE_BLOCKS, RA_PREEMPTIONS, RA_RECOVERIES, \
+    RA_ADMITTED, RA_RETIRED = range(11)
+RA_HEADER_INTS = 16
+
+
+def retire_admit(st: dict, header: torch.Tensor, block_size: int, max_prompt_len: int, max_seq_len: int):
+    """Retire the finished slots and admit queued requests (b200_retire_admit; call right after step_paddle).  `st` maps every
+    name of RETIRE_ADMIT_ORDER to its device tensor (updated in place); `header` is a pinned int32 [RA_HEADER_INTS] host tensor.
+    max_prompt_len / max_seq_len: the queue's longest prompt and prompt + max_dec_len."""
+    dtypes = {"stop_flags": torch.bool, "is_block_step": torch.bool, "step_idx": torch.int64, "pre_ids": torch.int64,
+              "next_tokens": torch.int64, "input_ids": torch.int64, "max_dec_len": torch.int64, "min_dec_len": torch.int64,
+              "prompt_ids": torch.int64, "req_max_dec_len": torch.int64, "req_min_dec_len": torch.int64, "out_ids": torch.int64}
+    for name in RETIRE_ADMIT_ORDER:
+        _chk(st[name], name, dtypes.get(name, torch.int32))
+        assert st[name].is_contiguous(), name
+    assert header.dtype == torch.int32 and header.is_pinned() and header.numel() >= RA_HEADER_INTS
+    call("b200_retire_admit", *[ptr(st[k]) for k in RETIRE_ADMIT_ORDER], ptr(header), st["seq_lens_this_time"].numel(),
+         int(block_size), st["block_tables"].shape[1], st["input_ids"].shape[1], st["pre_ids"].shape[1],
+         st["req_max_dec_len"].numel(), st["out_ids"].shape[1], int(max_prompt_len), int(max_seq_len), stream_ptr())
 
 
 def generate_step_update(next_tokens, stop_flags, step_idx, max_dec_len, seq_len_decoder, pre_ids, eos_ids, out_tokens,
