@@ -15,14 +15,16 @@ STEP_ORDER = ("stop_flags", "seq_lens_this_time", "ori_seq_lens_encoder", "seq_l
               "step_idx", "next_tokens")
 
 
-def make_queue_state(seed, bsz=6, block_size=4, num_requests=24, max_prompt=12, max_dec=24, spare_blocks=3):
-    """Empty slots, a free list of every block, and a queue of `num_requests` requests; the pool is `spare_blocks` above the
-    largest single request's pages, so that pre-emption and recovery happen."""
+def make_queue_state(seed, bsz=6, block_size=4, num_requests=24, max_prompt=12, max_dec=24, spare_blocks=3, num_blocks=None,
+                     prompt_lens=None):
+    """Empty slots, a free list of every block, and a queue of `num_requests` requests (prompt lengths U{1..max_prompt}, or
+    `prompt_lens(rng, num_requests)`); the pool is `spare_blocks` above the largest single request's pages (or `num_blocks`,
+    if given and larger), so that pre-emption and recovery happen."""
     rng = np.random.RandomState(seed)
-    plens = rng.randint(1, max_prompt + 1, size=num_requests)
+    plens = rng.randint(1, max_prompt + 1, size=num_requests) if prompt_lens is None else prompt_lens(rng, num_requests)
     decs = rng.randint(1, max_dec + 1, size=num_requests)
     need = int(max((p + d + block_size - 1) // block_size for p, d in zip(plens, decs)))
-    num_blocks = need + spare_blocks
+    num_blocks = max(need + spare_blocks, num_blocks or 0)
     bnps = need + 1                                   # one spare column: step_paddle recovers with used + 1 blocks
     length = bnps * block_size
     prompts = [rng.randint(5, 1000, size=int(p)).astype(np.int64) for p in plens]
@@ -47,14 +49,19 @@ def make_queue_state(seed, bsz=6, block_size=4, num_requests=24, max_prompt=12, 
     return st, rng, num_blocks, prompts
 
 
-def model_step(st, rng, emitted, p_eos=0.04):
-    """One model step over the running slots: the token each one 'generates' is random (EOS with probability p_eos), logged in
-    emitted[request]; then the reference's bookkeeping up to update_inputs."""
+def draw_tokens(rng, bsz, p_eos=0.04):
+    """The token each slot 'generates': random, EOS with probability p_eos."""
+    topk = rng.randint(5, 1000, size=bsz).astype(np.int64)
+    topk[rng.rand(bsz) < p_eos] = EOS
+    return topk
+
+
+def apply_tokens(st, topk, emitted):
+    """The reference's bookkeeping of one model step over the running slots, given the tokens they chose (logged in
+    emitted[request]), up to update_inputs.  Returns update_inputs' not_need_stop (stop_nums = the slot count)."""
     running = ~st["stop_flags"]
     st["pre_ids"][:] = G.set_value_by_flags_and_idx_v2(st["pre_ids"], st["input_ids"], st["seq_lens_encoder"],
                                                        st["seq_lens_decoder"], st["step_idx"], st["stop_flags"])
-    topk = rng.randint(5, 1000, size=running.shape[0]).astype(np.int64)
-    topk[rng.rand(running.shape[0]) < p_eos] = EOS
     st["step_idx"] += running
     topk, sf, nxt = G.set_stop_value_multi_ends_v2(topk, st["stop_flags"], st["seq_lens_this_time"], np.array([EOS]),
                                                    st["next_tokens"])
@@ -62,10 +69,16 @@ def model_step(st, rng, emitted, p_eos=0.04):
     st["stop_flags"][:], st["next_tokens"][:] = sf, nxt
     for b in np.nonzero(running)[0]:
         emitted.setdefault(int(st["slot_request"][b]), []).append(int(topk[b]))
-    _, stt, enc, dec, ids = G.update_inputs(st["stop_flags"], st["seq_lens_this_time"], st["seq_lens_encoder"],
-                                            st["seq_lens_decoder"], st["input_ids"], np.array([running.shape[0]]), st["next_tokens"],
-                                            st["is_block_step"])
+    nns, stt, enc, dec, ids = G.update_inputs(st["stop_flags"], st["seq_lens_this_time"], st["seq_lens_encoder"],
+                                              st["seq_lens_decoder"], st["input_ids"], np.array([running.shape[0]]),
+                                              st["next_tokens"], st["is_block_step"])
     st["seq_lens_this_time"][:], st["seq_lens_encoder"][:], st["seq_lens_decoder"][:], st["input_ids"][:] = stt, enc, dec, ids
+    return nns
+
+
+def model_step(st, rng, emitted, p_eos=0.04):
+    """One model step over the running slots: draw_tokens, then apply_tokens."""
+    apply_tokens(st, draw_tokens(rng, st["stop_flags"].shape[0], p_eos), emitted)
 
 
 def check_blocks(st, num_blocks):
