@@ -159,7 +159,10 @@ def top_p_sampling_reject(probs, top_p, uniform, max_rounds=32):
             valid = p > pivot
             cdf = np.cumsum(np.where(valid, p, np.float32(0)), dtype=np.float32)
             hit = np.nonzero((cdf > u) & valid)[0]
-            sid = int(hit[0]) if hit.size else d - 1            # :313 default sampled_id = d - 1
+            # deviation from :313, whose default sampled_id = d - 1 can be a token of probability 0 when the row's fp32
+            # total is at most u: fall back to the largest index with p > pivot (d - 1 only if there is none)
+            last = np.nonzero(valid)[0]
+            sid = int(hit[0]) if hit.size else (int(last[-1]) if last.size else d - 1)
             pivot = max(pivot, p[sid])
             above = p > pivot
             q = np.float32(p[above].sum(dtype=np.float32))

@@ -284,14 +284,17 @@ __global__ void set_value_by_flags_v2_kernel(const bool* __restrict__ stop_flags
 
 // get_token_penalty_multi_scores(_v2) (csrc/gpu/token_penalty_multi_scores_v2.cu:19-139; CPU twin
 // csrc/cpu/src/token_penalty_multi_scores.cc:18-85).  One CTA per sequence; repeat counts in a caller workspace.
+// Precondition: each row of pre_ids is its history as a prefix of ids >= 0 followed only by -1 padding.  The count stops at
+// the first negative entry, so a row whose entry 0 is -1 has an empty history whatever follows it (the callers write the
+// last prompt token into entry 0 before the first token is chosen).
 __global__ void penalty_count_kernel(const int64_t* __restrict__ pre_ids, const int64_t* __restrict__ cur_len,
                                      int* __restrict__ repeat_times, int64_t length, int64_t length_id) {
   const int bi = blockIdx.x;
   if (cur_len[bi] < 0) return;
   const int64_t* ids = pre_ids + static_cast<size_t>(bi) * length_id;
   int* rt = repeat_times + static_cast<size_t>(bi) * length;
-  // the reference breaks at the first negative id PER THREAD stride; ids are -1 padded at the tail, so scanning
-  // until the first negative entry is equivalent.
+  // the reference breaks at the first negative id PER THREAD stride; under the precondition above, scanning until the
+  // first negative entry is equivalent.
   for (int64_t i = threadIdx.x; i < length_id; i += blockDim.x) {
     const int64_t id = ids[i];
     if (id < 0) break;
@@ -511,8 +514,11 @@ __global__ void __launch_bounds__(1024) softmax_f32_kernel(float* __restrict__ x
 }
 
 // One CTA (1024 threads) per row.  Round r: u = uniform[r, b] * q; sampled = first index whose inclusive CDF over
-// {p_j > pivot} exceeds u (vocab-1 if none); pivot = max(pivot, p[sampled]); (q, count) = mass / number of {p_j > pivot};
+// {p_j > pivot} exceeds u; pivot = max(pivot, p[sampled]); (q, count) = mass / number of {p_j > pivot};
 // stop when 0 < q < top_p, or when count == 0 (covers top_p == 0 -> arg max).
+// When no CDF value exceeds u (the row's fp32 total is at most u: a softmax row sums to 1 only within rounding, and u can be
+// as large as 1 - 2^-24), sampled is the largest index with p > pivot, the last token the CDF reaches.  The reference falls
+// back to vocab - 1 (sampling.cuh:313), which can emit a token of probability zero (e.g. an EOS banned by min_length).
 __global__ void __launch_bounds__(1024) top_p_sampling_reject_kernel(const float* __restrict__ probs, const float* __restrict__ top_p,
                                                                      const float* __restrict__ uniform, int64_t* __restrict__ out,
                                                                      int vocab, int64_t ld, int bs, int max_rounds) {
@@ -527,7 +533,7 @@ __global__ void __launch_bounds__(1024) top_p_sampling_reject_kernel(const float
   float q = 1.f, pivot = 0.f;
   int sampled = vocab - 1;
   for (int round = 0; round < max_rounds; ++round) {
-    if (tx == 0) s_sampled = vocab - 1;
+    if (tx == 0) s_sampled = vocab;                  // "no index found"
     const float u = uniform[static_cast<size_t>(round) * bs + b] * q;
     float aggregate = 0.f;
     for (int it = 0; it < iters; ++it) {
@@ -575,6 +581,21 @@ __global__ void __launch_bounds__(1024) top_p_sampling_reject_kernel(const float
     }
     __syncthreads();
     sampled = s_sampled;
+    if (sampled == vocab) {                          // block-uniform: every thread read the same s_sampled
+      int last = -1;                                 // this thread's largest index with p > pivot (its i4 only grow)
+      for (int i4 = tx; i4 < n4; i4 += 1024) {
+        const float4 v = reinterpret_cast<const float4*>(row)[i4];
+        if (v.w > pivot) last = i4 * 4 + 3;
+        else if (v.z > pivot) last = i4 * 4 + 2;
+        else if (v.y > pivot) last = i4 * 4 + 1;
+        else if (v.x > pivot) last = i4 * 4;
+      }
+      last = __reduce_max_sync(0xffffffffu, last);
+      if (lane == 0) s_cnt[warp] = last;
+      __syncthreads();
+      last = __reduce_max_sync(0xffffffffu, s_cnt[lane]);
+      sampled = last >= 0 ? last : vocab - 1;        // nothing above the pivot: only a row without positive mass
+    }
     pivot = fmaxf(pivot, row[sampled]);
     float mass = 0.f;
     int cnt = 0;

@@ -113,6 +113,9 @@ class GenerationInferenceModel:
 
         if token_stream is not None:
             token_stream.reset(total_steps=max_length)
+        # the penalty history of the first token is the last prompt token (entry 0; update() writes generated token k at entry
+        # k), as set_value_by_flags_and_idx_v2 writes it in continuous_generate: the count stops at the first -1 entry
+        st["pre_ids"][:, 0] = ids.gather(1, (enc - 1).to(torch.int64)[:, None])[:, 0]
         # ---- prefill ("encoder" step) ----
         logits = self._prefill(ids, enc, cache_kvs)              # [B, V], last valid position of each prompt
         tgt = self._choose(logits, st)

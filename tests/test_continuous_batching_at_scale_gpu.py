@@ -64,11 +64,13 @@ def ops():
 # ----------------------------------------------------------------------------------------------------------
 # Teacher-forced checker
 # ----------------------------------------------------------------------------------------------------------
-def teacher_forced_check(forward, requests, outs, tau=TAU, max_copy=MAX_COPY):
+def teacher_forced_check(forward, requests, outs, tau=TAU, max_copy=MAX_COPY, transform=None):
     """Check every generated token against `forward(ids 1-D) -> logits [len(ids), V]` of its request's prompt + output.
 
     For request (prompt, max_length) with output o: len(o) == max_length, and at every position t the logit of o[t] in the
-    row that predicts it is within tau * max|row| of that row's maximum.  The reference must depend on the context, not only
+    row that predicts it is within tau * max|row| of that row's maximum.  `transform(r, rows, prompt, out) -> rows`, if given,
+    maps request r's fp64 rows [max_length, V] (row t predicts o[t]) before the check, e.g. to apply the penalties of each
+    position's history; it may set banned entries to -inf, and max|row| is taken over the finite entries.  The reference must depend on the context, not only
     on the row's own input token: over the (random) prompt rows its arg-max may be that input token at no more than max_copy
     of the rows.  A model that copies its input predicts the same output from any context, so no attention or cache error
     could move its tokens.  (Generated rows are not counted: a model's own output may repeat itself legitimately.)
@@ -84,7 +86,9 @@ def teacher_forced_check(forward, requests, outs, tau=TAU, max_copy=MAX_COPY):
         copies += int((full[:p].argmax(-1) == prompt).sum())
         prompt_rows += p
         lg = full[p - 1:p - 1 + max_len]
-        scale = lg.abs().amax(-1)
+        if transform is not None:
+            lg = transform(r, lg, prompt, out)
+        scale = lg.masked_fill(~torch.isfinite(lg), 0.0).abs().amax(-1)
         top2 = lg.topk(2, dim=-1).values
         gap = (top2[:, 0] - lg.gather(1, out[:, None])[:, 0]) / (tau * scale)
         bad = ~(gap <= 1.0)                                   # NaN fails
