@@ -91,6 +91,36 @@ int b200_gemm_bf16_splitk(const void* A, const void* B, void* C, const float* bi
                           int64_t K, int64_t lda, int64_t ldb, int64_t ldc, int a_mn_major, int b_mn_major, int split_k,
                           cudaStream_t stream);
 
+/* ---- weight-only int8 linear layers (--quant_type weight_only_int8, llm/predict/predictor.py:86,1250): weight_quantize /
+ * weight_only_linear of FusedMultiTransformerWeightOnly (fused_transformer_layers.py:1221-1440) --------------------------
+ * Quantisation of a bf16 W [K, N] (Paddle's [in, out] layout, row stride ldw), one scale per output channel:
+ *   a[n] = max_k |W[k, n]| (fp32, exact), scale[n] = bf16_rn(a[n] / 127.0f) (bf16 [N]),
+ *   q[k, n] = clamp(rint(W[k, n] / float(scale[n])), -127, 127) (IEEE fp32 division, half to even); scale 0 gives q = 0.
+ * Packed layout of q (exactly N * K bytes; this library's own, not Paddle's CUTLASS interleave): 128-byte units, one per
+ * 8 output channels x 16 k, unit (g, s) at byte (g * K/16 + s) * 128 for channels 8g .. 8g+7 and k 16s .. 16s+15.  Inside a
+ * unit, lane l (0..31) owns bytes 4l .. 4l+3 = q[16s + c][n], q[16s + c + 1][n], q[16s + c + 8][n], q[16s + c + 9][n] with
+ * n = 8g + l/4, c = 2 (l % 4): the two bf16 pairs of the tensor-core A fragment of row l/4, so a thread reads each half of its
+ * fragment with one 32-bit shared-memory load and converts it in registers.
+ * Requires K % 16 == 0, N % 8 == 0, ldw >= N, Q 4-byte aligned.  Runs on the device (load time, not a hot path). */
+int b200_weight_quantize_int8(const void* W, void* Q, void* scale, int64_t K, int64_t N, int64_t ldw, cudaStream_t stream);
+/* y[m, n] = scale[n] * sum_k X[m, k] q[k, n] (+ bias[n]): X bf16 [M, K] (row stride ldx), Q / scale from
+ * b200_weight_quantize_int8, fp32 sums (int8 -> bf16 is exact, the weights are never rounded), the scale multiplies the fp32
+ * sum (or each split-K partial before it is reduced), ONE rounding to bf16 into C [M, ldc].  One kernel for every M: the
+ * weights are the wgmma A operand (converted in registers), the tokens its N dimension (8 to 128 wide).
+ *   split_k: 0 chooses (K is split across CTAs only when the output tiles leave SMs idle), 1 = no split, > 1 explicit.  A
+ *   split needs `workspace` (b200_gemm_splitk_workspace_bytes(M, N), ZERO on entry, returned zeroed, as for
+ *   b200_gemm_bf16_splitk); workspace == NULL means no split (split_k > 1 is then an argument error).
+ *   bias: optional fp32 [N] (Qwen2 q/k/v bias).
+ * Requires M, N, K > 0, K % 16 == 0, N % 8 == 0, ldx and ldc multiples of 8, X, Q, C and workspace 16-byte aligned; any other
+ * is an argument error. */
+int b200_weight_only_gemm_bf16(const void* X, const void* Q, const void* scale, const float* bias, void* C, void* workspace,
+                               int64_t M, int64_t N, int64_t K, int64_t ldx, int64_t ldc, int split_k, cudaStream_t stream);
+/* Same product left as fp32 sums: workspace [M, N] (contiguous, ZERO on entry) += scale[n] * sum_k X[m, k] q[k, n], by TMA
+ * reduce-add of each (split-K) partial.  The consumer (b200_add_rmsnorm_f32, b200_decode_rope_append_f32, b200_swiglu_fwd_f32)
+ * rounds once and re-zeroes it, as after b200_gemm_bf16_splitk with C == NULL. */
+int b200_weight_only_gemm_f32(const void* X, const void* Q, const void* scale, float* workspace, int64_t M, int64_t N, int64_t K,
+                              int64_t ldx, int split_k, cudaStream_t stream);
+
 /* gate|up projection + SwiGLU in ONE kernel — LlamaMLP.forward with fuse_attention_ffn (llama/modeling.py:632-652, swiglu :38-45):
  *   GU[M, 2I] = bf16(X[M,K] * W[K,2I])  (gate columns [0,I), up columns [I,2I); kept for the backward),
  *   Mout[M, I] = bf16(silu(gate) * up)  with gate/up rounded to bf16 first (the unfused rounding points).

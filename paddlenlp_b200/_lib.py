@@ -33,6 +33,9 @@ _SIGNATURES = {
     "b200_gemm_swiglu_bwd_bf16": [P, P, P, P, I64, I64, I64, I64, I64, I64, I64, P],
     "b200_gemm_splitk_workspace_bytes": [I64, I64],
     "b200_gemm_bf16_splitk": [P, P, P, P, P, I64, I64, I64, I64, I64, I64, I, I, I, P],
+    "b200_weight_quantize_int8": [P, P, P, I64, I64, I64, P],
+    "b200_weight_only_gemm_bf16": [P, P, P, P, P, P, I64, I64, I64, I64, I64, I, P],
+    "b200_weight_only_gemm_f32": [P, P, P, P, I64, I64, I64, I64, I, P],
     "b200_rmsnorm_fwd": [P, P, P, P, I64, I64, F, P],
     "b200_rmsnorm_bwd_workspace_bytes": [I64, I64],
     "b200_rmsnorm_bwd": [P, P, P, P, P, P, P, I, P, I64, I64, P],

@@ -81,6 +81,10 @@ int encode_tmap_f32(CUtensorMap* out, const void* base, int rank, const uint64_t
                     const uint32_t* box) {
   return encode_tmap(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, base, rank, dims, strides, box);
 }
+int encode_tmap_u8(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides,
+                   const uint32_t* box) {
+  return encode_tmap(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, base, rank, dims, strides, box);
+}
 
 static int encode_tmap(CUtensorMap* out, CUtensorMapDataType dtype, const void* base, int rank, const uint64_t* dims,
                        const uint64_t* strides, const uint32_t* box) {

@@ -106,6 +106,13 @@ __device__ __forceinline__ void bulk_load(void* smem_dst, const void* src, uint3
                "l"(src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
+// global -> shared, 3D tile, completion on an mbarrier in this CTA.
+__device__ __forceinline__ void tma_load_3d(const CUtensorMap* tm, uint64_t* bar, void* smem_dst, int c0, int c1, int c2) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
+      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
+      : "memory");
+}
 __device__ __forceinline__ void tma_load_4d(const CUtensorMap* tm, uint64_t* bar, void* smem_dst, int c0, int c1,
                                             int c2, int c3) {
   asm volatile(
@@ -150,6 +157,18 @@ __device__ __forceinline__ void tma_store_wait_read() {
 template <int N>
 __device__ __forceinline__ void tma_store_wait() {
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
+}
+
+// Persistent-GEMM tile order: GM consecutive m-tiles share each n-tile column, so that concurrently running CTAs reuse
+// A and B tiles out of L2.
+__device__ __forceinline__ void tile_coords(int t, int num_m, int num_n, int& m_blk, int& n_blk, int GM) {
+  const int per_group = GM * num_n;
+  const int g = t / per_group;
+  const int first_m = g * GM;
+  const int gsize = min(GM, num_m - first_m);
+  const int r = t - g * per_group;
+  m_blk = first_m + (r % gsize);
+  n_blk = r / gsize;
 }
 
 // ------------------------------------------------------------------------------------------------

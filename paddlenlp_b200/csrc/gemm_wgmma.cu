@@ -77,18 +77,6 @@ struct Params {
   float* ws;               // mode 3: fp32 [M, N] accumulation buffer; modes 6, 7: the fp32 output (leading dimension ldc)
 };
 
-__device__ __forceinline__ void tile_coords(int t, int num_m, int num_n, int& m_blk, int& n_blk, int GM) {
-  // Grouped ordering: GM consecutive m-tiles share each n-tile column so that concurrently running CTAs reuse
-  // A and B tiles out of L2.
-  const int per_group = GM * num_n;
-  const int g = t / per_group;
-  const int first_m = g * GM;
-  const int gsize = min(GM, num_m - first_m);
-  const int r = t - g * per_group;
-  m_blk = first_m + (r % gsize);
-  n_blk = r / gsize;
-}
-
 // Compiler-level fence on the accumulator registers (wgmma reads and writes them asynchronously): no access to them may be
 // scheduled across it.
 __device__ __forceinline__ void fence_acc(float (&acc)[128]) {
@@ -690,6 +678,15 @@ __global__ void splitk_finish_kernel(float* __restrict__ ws, const float* __rest
   }
 }
 }  // namespace gemm
+
+int splitk_finish(float* ws, const float* bias, void* out, int64_t M, int64_t N, int64_t ldc, cudaStream_t stream) {
+  const int64_t total = M * (N / 8);
+  int64_t blocks = (total + 255) / 256;
+  if (blocks > sm_count() * 8) blocks = sm_count() * 8;
+  gemm::splitk_finish_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(ws, bias, static_cast<bf16*>(out), M, N, ldc);
+  return check_launch("gemm_splitk(finish)");
+}
+
 }  // namespace b200
 
 extern "C" int64_t b200_gemm_splitk_workspace_bytes(int64_t M, int64_t N) { return M * N * 4; }
@@ -726,12 +723,7 @@ extern "C" int b200_gemm_bf16_splitk(const void* A, const void* B, void* C, cons
   // `workspace` must be all-zero on entry; the finish kernel leaves it zeroed again (no memset per GEMM).
   if ((rc = dispatch(a_mn_major, b_mn_major, tmA, tmB, p, 0, stream)) != 0) return rc;
   if (C == nullptr) return 0;   // C == NULL: the consumer kernel reads (and re-zeroes) the fp32 workspace itself
-  const int64_t total = M * (N / 8);
-  int64_t blocks = (total + 255) / 256;
-  if (blocks > sm_count() * 8) blocks = sm_count() * 8;
-  splitk_finish_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(static_cast<float*>(workspace), bias,
-                                                                         static_cast<bf16*>(C), M, N, ldc);
-  return check_launch("gemm_splitk(finish)");
+  return splitk_finish(static_cast<float*>(workspace), bias, C, M, N, ldc, stream);
 }
 
 extern "C" int b200_gemm_bf16(const void* A, const void* B, void* C, const float* bias, int64_t M, int64_t N, int64_t K,

@@ -58,6 +58,12 @@ int encode_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_
 // Same for fp32 elements (box[0] * 4 must be <= 128); used for TMA reduce-add into fp32 accumulation buffers.
 int encode_tmap_f32(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides,
                     const uint32_t* box);
+// Same for 1-byte elements (int8 weights of the weight-only GEMM; box[0] must be <= 128).
+int encode_tmap_u8(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides,
+                   const uint32_t* box);
+// out[m, n] = bf16(ws[m, n] + bias[n]) for the split-K GEMMs (N % 8 == 0, ws [M, N] contiguous); re-zeroes ws
+// (gemm_wgmma.cu).
+int splitk_finish(float* ws, const float* bias, void* out, int64_t M, int64_t N, int64_t ldc, cudaStream_t stream);
 // Attention operand [B, S, heads, D] bf16 with token stride ld (elements), box {64 d, 1 head, rows, 1}: one 128-byte swizzled
 // block of `rows` rows.  Rows past S read as zeros, so a box never reaches into the next batch row.
 inline int make_bf16_map(CUtensorMap* tm, const void* base, int64_t B, int64_t S, int64_t heads, int64_t D, int64_t ld,

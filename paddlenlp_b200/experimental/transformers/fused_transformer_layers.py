@@ -1,6 +1,7 @@
 """FusedMultiTransformer — the stacked-layer inference block of
 paddlenlp/experimental/transformers/fused_transformer_layers.py (:205-345 config, :348-792 weights, :1027-1182 forward)
-for the bf16, non-quantised, rmsnorm + swiglu + rotate-half-RoPE case, on the native sm_90a kernels.
+for the rmsnorm + swiglu + rotate-half-RoPE case, on the native sm_90a kernels: bf16 layer weights, or weight-only int8
+(quant_type="weight_only_int8": FusedMultiTransformerWeightOnly / FusedBlockMultiTransformerWeightOnly, :1221-1440).
 
 Weight layouts are the reference's (SURVEY.md Appendix B):
     qkv_weight    [(nh + 2*kvh) * d, h]   (transposed, trans_qkvw=True)      -> GEMM with B stored [N, K]
@@ -39,6 +40,7 @@ class FusedMultiTransformerConfig:
     nranks: int = 1
     trans_qkvw: bool = True
     append_attn: bool = False                # FusedBlockMultiTransformer: route attention through the unified append_attention op
+    quant_type: str = ""                     # "" (bf16 layer weights) or "weight_only_int8" (FusedMultiTransformerWeightOnly)
 
     def __post_init__(self):
         if self.kv_num_heads <= 0:
@@ -52,6 +54,11 @@ class FusedMultiTransformerConfig:
         if not self.trans_qkvw:
             raise NotImplementedError("trans_qkvw=False")
         ops.check_head_dim(self.embed_dim // self.num_heads, "FusedMultiTransformerConfig")
+        qt = self.quant_type
+        if qt not in ("", "weight_only_int8"):
+            if qt == "weight_only_int4" or qt.startswith("a8w8") or "fp8" in qt:
+                raise NotImplementedError(f"quant_type {qt!r} is not implemented (weight_only_int8 is)")
+            raise ValueError(f"unknown quant_type {qt!r}")
 
 
 class FusedMultiTransformerBase:
@@ -75,18 +82,29 @@ class FusedMultiTransformerBase:
         self.d = self.h // self.nh
         self.qkv_n = (self.nh + 2 * self.kvh) * self.d
 
-        def z(*shape):
-            return torch.zeros(*shape, dtype=BF16, device=self.device)
-
         self.ln_scales = [torch.ones(self.h, dtype=BF16, device=self.device) for _ in range(self.L)]
-        self.qkv_weights = [z(self.qkv_n, self.h) for _ in range(self.L)]
-        self.qkv_biases: List[Optional[torch.Tensor]] = [z(self.qkv_n) if c.qkv_bias else None for _ in range(self.L)]
-        self.linear_weights = [z(self.nh * self.d, self.h) for _ in range(self.L)]
+        self.qkv_biases: List[Optional[torch.Tensor]] = [torch.zeros(self.qkv_n, dtype=BF16, device=self.device) if c.qkv_bias
+                                                         else None for _ in range(self.L)]
         self.ffn_ln_scales = [torch.ones(self.h, dtype=BF16, device=self.device) for _ in range(self.L)]
-        self.ffn1_weights = [z(self.h, 2 * self.I) for _ in range(self.L)]
-        self.ffn2_weights = [z(self.I, self.h) for _ in range(self.L)]
+        self._alloc_layer_matrices()
         self._bias_f32 = [None] * self.L
         self.rope = ops.rope_tables(self.d, c.max_position_embeddings, float(c.rope_theta), self.device)
+
+    MATRICES = ("qkv", "linear", "ffn1", "ffn2")
+
+    def layer_matrix_shape(self, name):
+        """Shape of layer matrix `name` in the bf16 block (the reference's layouts above: qkv is stored transposed)."""
+        return {"qkv": (self.qkv_n, self.h), "linear": (self.nh * self.d, self.h), "ffn1": (self.h, 2 * self.I),
+                "ffn2": (self.I, self.h)}[name]
+
+    def _alloc_layer_matrices(self):
+        for name in self.MATRICES:
+            setattr(self, name + "_weights", [torch.zeros(*self.layer_matrix_shape(name), dtype=BF16, device=self.device)
+                                              for _ in range(self.L)])
+
+    def set_layer_matrix(self, name, i, w):
+        """Load layer i's matrix `name` from a bf16 tensor of layer_matrix_shape(name)."""
+        getattr(self, name + "_weights")[i].copy_(w)
 
     def ensure_rope(self, positions: int):
         """Grow the fp32 cos/sin tables to cover `positions` rows.  The decode kernels index them with the running sequence
@@ -116,9 +134,27 @@ class FusedMultiTransformerBase:
             return ops.gemm_skinny(a, w, trans_b=trans_b, bias=bias)
         return ops.gemm(a, w, trans_b=trans_b, bias=bias)
 
+    # ---- per-matrix hooks (overridden by the weight-only blocks); `name` is one of MATRICES ----
+    def linear(self, x, name, i, bias=None):
+        """bf16 output of layer i's matrix `name` applied to x (+ fp32 bias)."""
+        return self._mm(x, getattr(self, name + "_weights")[i], trans_b=name == "qkv", bias=bias)
+
+    def linear_f32(self, x, name, i, tag):
+        """The decode step's form: fp32 sums left in the workspace `tag` for the consumer kernel to round and re-zero."""
+        return ops.gemm_skinny_f32(x, getattr(self, name + "_weights")[i], trans_b=name == "qkv", tag=tag)
+
+    def ffn1_act(self, x, i):
+        """The decode step's ffn1 + SwiGLU."""
+        if self.I % 64 == 0:
+            # SwiGLU in the ffn1 epilogue of the persistent kernel: the 256-column tile pairs 128 gate columns with the
+            # 128 up columns of the same channels straight from the reference-layout weight; only the activation is stored
+            _, act = ops.gemm_swiglu(x, self.ffn1_weights[i], store_gate_up=False)
+            return act
+        return ops.swiglu_fwd(self.linear(x, "ffn1", i))
+
     # compute_qkv (:817-820): linear(ln_out, qkv_weight, transpose_weight=True)
     def compute_qkv(self, ln_out, i):
-        return self._mm(ln_out, self.qkv_weights[i], trans_b=True, bias=self._bias(i))
+        return self.linear(ln_out, "qkv", i, bias=self._bias(i))
 
     # ---- the three places that touch the KV cache (overridden by FusedBlockMultiTransformer) ----
     def _write_cache(self, qkv, caches, i, B, S, seq_lens_encoder, kw):
@@ -165,19 +201,13 @@ class FusedMultiTransformerBase:
             if fused:
                 # decode step: the split-K GEMMs leave fp32 sums that the next kernel rounds once (same rounding points,
                 # three launches fewer per layer)
-                acc = ops.gemm_skinny_f32(ln_out, self.qkv_weights[i], trans_b=True, tag="splitk_qkv")
+                acc = self.linear_f32(ln_out, "qkv", i, "splitk_qkv")
                 qkv = self._rope_append(None, acc, caches, i, seq_lens_decoder, kw)
                 attn = self._attend(qkv, caches, i, seq_lens_decoder, kw)
-                acc = ops.gemm_skinny_f32(attn, self.linear_weights[i], tag="splitk_h")
+                acc = self.linear_f32(attn, "linear", i, "splitk_h")
                 ln_out, residual = ops.add_rmsnorm_f32(acc, residual, self.ffn_ln_scales[i], eps)
-                if self.I % 64 == 0:
-                    # SwiGLU in the ffn1 epilogue of the persistent kernel: the 256-column tile pairs 128 gate columns with the
-                    # 128 up columns of the same channels straight from the reference-layout weight; only the activation is stored
-                    _, act = ops.gemm_swiglu(ln_out, self.ffn1_weights[i], store_gate_up=False)
-                else:
-                    ffn1 = self._mm(ln_out, self.ffn1_weights[i])
-                    act = ops.swiglu_fwd(ffn1)
-                acc = ops.gemm_skinny_f32(act, self.ffn2_weights[i], tag="splitk_h")
+                act = self.ffn1_act(ln_out, i)
+                acc = self.linear_f32(act, "ffn2", i, "splitk_h")
                 if i != self.L - 1:
                     ln_out, residual = ops.add_rmsnorm_f32(acc, residual, self.ln_scales[i + 1], eps)
                 else:
@@ -188,11 +218,11 @@ class FusedMultiTransformerBase:
                 attn = self.compute_mmha(qkv, caches, i, seq_lens_decoder, kw)
             else:
                 attn = self.compute_fmha(qkv, caches, i, B, S, seq_lens_encoder, kw)
-            out = self._mm(attn, self.linear_weights[i])                                      # compute_out_linear (:895-896)
+            out = self.linear(attn, "linear", i)                                              # compute_out_linear (:895-896)
             ln_out, residual = ops.add_rmsnorm(out, residual, self.ffn_ln_scales[i], eps)     # compute_ffn_layernorm (:937-949)
-            ffn1 = self._mm(ln_out, self.ffn1_weights[i])
+            ffn1 = self.linear(ln_out, "ffn1", i)
             act = ops.swiglu_fwd(ffn1)                                                        # fused_bias_act("swiglu") (:100-168)
-            ffn2 = self._mm(act, self.ffn2_weights[i])
+            ffn2 = self.linear(act, "ffn2", i)
             if i != self.L - 1:                                                               # compute_bias_residual_layernorm (:976-999)
                 ln_out, residual = ops.add_rmsnorm(ffn2, residual, self.ln_scales[i + 1], eps)
             else:
@@ -255,3 +285,48 @@ class FusedBlockMultiTransformer(FusedMultiTransformerBase):
         B = qkv.shape[0]
         one = torch.ones(B, dtype=torch.int32, device=qkv.device)
         return self._append(qkv, caches, i, B, 1, torch.zeros_like(one), seq_lens_decoder, one, kw)
+
+
+class WeightOnlyInt8Mixin:
+    """Layer matrices as int8 weights with one bf16 scale per output channel (quant_type="weight_only_int8";
+    FusedMultiTransformerWeightOnly, fused_transformer_layers.py:1221-1440: weight_quantize at load, weight_only_linear in the
+    forward).  `<name>_weights[i]` holds the packed int8 weights of the [in, out] matrix W (ops.weight_quantize: [out, in],
+    exactly out * in bytes) and `<name>_weights_scale[i]` the bf16 [out] scales; no bf16 copy of a layer matrix is kept.
+    Only the per-matrix hooks differ from the bf16 block: the forward, the cache paths and the bf16 head are shared."""
+
+    def _alloc_layer_matrices(self):
+        for name in self.MATRICES:
+            k, n = self._in_out(name)
+            setattr(self, name + "_weights", [torch.zeros(n, k, dtype=torch.int8, device=self.device) for _ in range(self.L)])
+            setattr(self, name + "_weights_scale", [torch.zeros(n, dtype=BF16, device=self.device) for _ in range(self.L)])
+
+    def _in_out(self, name):
+        rows, cols = self.layer_matrix_shape(name)
+        return (cols, rows) if name == "qkv" else (rows, cols)
+
+    def set_layer_matrix(self, name, i, w):
+        """Quantise a bf16 matrix of layer_matrix_shape(name) into layer i's int8 weights and scales (on its device)."""
+        w_in_out = (w.t() if name == "qkv" else w).to(device=self.device, dtype=BF16).contiguous()
+        q, scale = ops.weight_quantize(w_in_out, algo=self.config.quant_type)
+        getattr(self, name + "_weights")[i].copy_(q)
+        getattr(self, name + "_weights_scale")[i].copy_(scale)
+
+    def linear(self, x, name, i, bias=None):
+        return ops.weight_only_linear(x, getattr(self, name + "_weights")[i], bias=bias,
+                                      weight_scale=getattr(self, name + "_weights_scale")[i], weight_dtype="int8")
+
+    def linear_f32(self, x, name, i, tag):
+        return ops.weight_only_linear_f32(x, getattr(self, name + "_weights")[i], getattr(self, name + "_weights_scale")[i],
+                                          tag=tag)
+
+    def ffn1_act(self, x, i):
+        # no int8 twin of the fused gate|up + SwiGLU epilogue: fp32 sums, then SwiGLU rounds them and re-zeroes the workspace
+        return ops.swiglu_fwd_f32(self.linear_f32(x, "ffn1", i, "splitk_ffn1"))
+
+
+class FusedMultiTransformerWeightOnly(WeightOnlyInt8Mixin, FusedMultiTransformerBase):
+    """Dense-cache block with weight-only int8 layer matrices."""
+
+
+class FusedBlockMultiTransformerWeightOnly(WeightOnlyInt8Mixin, FusedBlockMultiTransformer):
+    """Paged-cache block with weight-only int8 layer matrices."""

@@ -8,17 +8,21 @@ from typing import Dict, List
 import torch
 
 from .... import ops
-from ..fused_transformer_layers import FusedBlockMultiTransformer, FusedMultiTransformerBase, FusedMultiTransformerConfig
+from ..fused_transformer_layers import (FusedBlockMultiTransformer, FusedBlockMultiTransformerWeightOnly, FusedMultiTransformerBase,
+                                        FusedMultiTransformerConfig, FusedMultiTransformerWeightOnly)
 from ..generation_utils import GenerationInferenceModel
 
 BF16 = torch.bfloat16
 
 
 class LlamaForCausalLMInferenceModel(GenerationInferenceModel):
-    def __init__(self, config, device=None, block_attn: bool = False, block_size: int = 64, append_attn: bool = False):
+    def __init__(self, config, device=None, block_attn: bool = False, block_size: int = 64, append_attn: bool = False,
+                 quant_type=None):
         """block_attn=True selects the paged KV cache (`--block_attn` of llm/predict/predictor.py:1507-1520:
         LlamaBlockInferenceModel on FusedBlockMultiTransformer); append_attn=True (`--append_attn`) additionally routes prefill
-        and decode attention through the unified append_attention op."""
+        and decode attention through the unified append_attention op.  quant_type (`--quant_type`, predictor.py:86,1250; None
+        reads config.quant_type, where the predictor puts it): "weight_only_int8" holds the layer matrices as int8 with
+        per-channel scales (FusedMultiTransformerWeightOnly); embeddings, norms and the head stay bf16."""
         if append_attn and not block_attn:
             raise ValueError("append_attn needs block_attn=True (the op works on the paged cache)")
         self.config = config
@@ -31,8 +35,13 @@ class LlamaForCausalLMInferenceModel(GenerationInferenceModel):
             embed_dim=c.hidden_size, num_heads=c.num_attention_heads, dim_feedforward=c.intermediate_size,
             kv_num_heads=c.num_key_value_heads, num_layers=c.num_hidden_layers, epsilon=c.rms_norm_eps,
             rope_theta=c.rope_theta, max_position_embeddings=max(int(getattr(c, "max_position_embeddings", 4096)), 128),
-            qkv_bias=(c.model_type == "qwen2"), append_attn=bool(append_attn))
-        self.transformer_block = (FusedBlockMultiTransformer if self.block_attn else FusedMultiTransformerBase)(fcfg, device)
+            qkv_bias=(c.model_type == "qwen2"), append_attn=bool(append_attn),
+            quant_type=(getattr(c, "quant_type", "") if quant_type is None else quant_type) or "")
+        if fcfg.quant_type:
+            block = FusedBlockMultiTransformerWeightOnly if self.block_attn else FusedMultiTransformerWeightOnly
+        else:
+            block = FusedBlockMultiTransformer if self.block_attn else FusedMultiTransformerBase
+        self.transformer_block = block(fcfg, device)
         self.device = self.transformer_block.device
         self.embed_tokens = torch.zeros(c.vocab_size, c.hidden_size, dtype=BF16, device=self.device)
         self.norm_weight = torch.ones(c.hidden_size, dtype=BF16, device=self.device)
@@ -46,7 +55,8 @@ class LlamaForCausalLMInferenceModel(GenerationInferenceModel):
     def set_state_dict(self, sd: Dict[str, torch.Tensor]):
         """Accepts the training-format names (`llama.layers.N.self_attn.q_proj.weight` [in,out], ...) and fuses them into
         the FusedMultiTransformer layouts: qkv_weight = concat([Wq,Wk,Wv],-1).T, ffn1_weight = concat([Wg,Wu],-1).
-        A tied model reads no `lm_head.weight` (one in `sd` is ignored)."""
+        A tied model reads no `lm_head.weight` (one in `sd` is ignored).  A weight-only block quantises each fused matrix on
+        the device as it is built: one bf16 fused matrix is staged at a time."""
         t = self.transformer_block
         pre = self.prefix
         dev = self.device
@@ -54,34 +64,54 @@ class LlamaForCausalLMInferenceModel(GenerationInferenceModel):
         def g(name):
             return sd[name].to(device=dev, dtype=BF16)
 
+        def cat_cols(names):
+            """concat(..., -1) built in one device buffer: no device copy of the parts is staged beside it."""
+            parts = [sd[n] for n in names]
+            out = torch.empty(parts[0].shape[0], sum(p.shape[1] for p in parts), dtype=BF16, device=dev)
+            c0 = 0
+            for p in parts:
+                out[:, c0:c0 + p.shape[1]].copy_(p)
+                c0 += p.shape[1]
+            return out
+
         self.embed_tokens.copy_(g(f"{pre}.embed_tokens.weight"))
         self.norm_weight.copy_(g(f"{pre}.norm.weight"))
         if not self.tied:
             self.lm_head_weight.copy_(g("lm_head.weight"))
         for i in range(t.L):
             lp = f"{pre}.layers.{i}."
-            qkv = torch.cat([g(lp + "self_attn.q_proj.weight"), g(lp + "self_attn.k_proj.weight"),
-                             g(lp + "self_attn.v_proj.weight")], dim=-1)
-            t.qkv_weights[i].copy_(qkv.t())
+            qkv = cat_cols([lp + "self_attn.q_proj.weight", lp + "self_attn.k_proj.weight", lp + "self_attn.v_proj.weight"])
+            t.set_layer_matrix("qkv", i, qkv.t())
+            del qkv
             if t.qkv_biases[i] is not None:
                 t.qkv_biases[i].copy_(torch.cat([g(lp + "self_attn.q_proj.bias"), g(lp + "self_attn.k_proj.bias"),
                                                  g(lp + "self_attn.v_proj.bias")]))
                 t._bias_f32[i] = None
-            t.linear_weights[i].copy_(g(lp + "self_attn.o_proj.weight"))
-            t.ffn1_weights[i].copy_(torch.cat([g(lp + "mlp.gate_proj.weight"), g(lp + "mlp.up_proj.weight")], dim=-1))
-            t.ffn2_weights[i].copy_(g(lp + "mlp.down_proj.weight"))
+            t.set_layer_matrix("linear", i, g(lp + "self_attn.o_proj.weight"))
+            t.set_layer_matrix("ffn1", i, cat_cols([lp + "mlp.gate_proj.weight", lp + "mlp.up_proj.weight"]))
+            t.set_layer_matrix("ffn2", i, g(lp + "mlp.down_proj.weight"))
             t.ln_scales[i].copy_(g(lp + "input_layernorm.weight"))
             t.ffn_ln_scales[i].copy_(g(lp + "post_attention_layernorm.weight"))
         t.weights_changed()
 
     @torch.no_grad()
     def init_random(self, seed: int = 42, std: float = 0.02):
+        """Normal(0, std) weights.  A weight-only block draws each layer matrix in the bf16 block's shape from the same generator
+        sequence and quantises it: bf16 and int8 models of one seed hold the same underlying weights."""
         gen = torch.Generator(device=self.device)
         gen.manual_seed(seed)
         t = self.transformer_block
         head = [] if self.tied else [self.lm_head_weight]
-        for w in [self.embed_tokens] + head + t.qkv_weights + t.linear_weights + t.ffn1_weights + t.ffn2_weights:
+        for w in [self.embed_tokens] + head:
             w.normal_(0.0, std, generator=gen)
+        for name in t.MATRICES:
+            for i in range(t.L):
+                if t.config.quant_type:
+                    w = torch.empty(t.layer_matrix_shape(name), dtype=BF16, device=self.device).normal_(0.0, std, generator=gen)
+                    t.set_layer_matrix(name, i, w)
+                    del w
+                else:
+                    getattr(t, name + "_weights")[i].normal_(0.0, std, generator=gen)
         t.weights_changed()
 
     def allocate_caches(self, batch: int, max_len: int) -> List[torch.Tensor]:

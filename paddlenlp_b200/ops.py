@@ -188,6 +188,79 @@ def gemm_skinny_f32(a: torch.Tensor, b: torch.Tensor, *, trans_b: bool = False, 
 
 
 # ----------------------------------------------------------------------------------------------------------
+# Weight-only int8 (weight_quantize / weight_only_linear, --quant_type weight_only_int8)
+# ----------------------------------------------------------------------------------------------------------
+SKINNY_M = 128     # at or below this many token rows the weight-only GEMM may split K (the decode-step workspace covers it)
+
+
+def weight_quantize(x: torch.Tensor, algo: str = "weight_only_int8"):
+    """(weight, weight_scale) of a bf16 [K, N] matrix (Paddle's [in, out] layout): per-output-channel scales bf16 [N] and the
+    int8 weights in the GEMM's packed layout (include/b200nlp.h), int8 [N, K] holding exactly N * K bytes."""
+    if algo == "weight_only_int4":
+        raise NotImplementedError("weight_quantize: weight_only_int4 is not implemented")
+    if algo != "weight_only_int8":
+        raise ValueError(f"weight_quantize: unknown algo {algo!r}")
+    _chk(x, "x")
+    assert x.dim() == 2 and x.stride(1) == 1
+    K, N = x.shape
+    weight = torch.empty(N, K, dtype=torch.int8, device=x.device)
+    scale = torch.empty(N, dtype=BF16, device=x.device)
+    call("b200_weight_quantize_int8", ptr(x), ptr(weight), ptr(scale), K, N, x.stride(0), stream_ptr())
+    return weight, scale
+
+
+def _weight_only_args(x, weight, weight_scale, weight_dtype):
+    if weight_dtype != "int8":
+        raise NotImplementedError(f"weight_only_linear: weight_dtype {weight_dtype!r} is not implemented (int8 only)")
+    if weight_scale is None:
+        raise ValueError("weight_only_linear: weight_scale is required")
+    _chk(x, "x"); _chk(weight, "weight", torch.int8); _chk(weight_scale, "weight_scale")
+    if x.dim() != 2 or x.stride(1) != 1 or weight.dim() != 2 or not weight.is_contiguous():
+        raise ValueError("weight_only_linear: x [M, K] with unit inner stride and a packed weight [N, K] are required")
+    M, K = x.shape
+    N = weight.shape[0]
+    if weight.shape[1] != K or weight_scale.shape != (N,):
+        raise ValueError(f"weight_only_linear: shapes x {tuple(x.shape)}, weight {tuple(weight.shape)}, "
+                         f"weight_scale {tuple(weight_scale.shape)}")
+    return M, N, K
+
+
+def weight_only_linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] = None,
+                       weight_scale: Optional[torch.Tensor] = None, weight_dtype: str = "int8",
+                       out: Optional[torch.Tensor] = None, split_k: int = 0) -> torch.Tensor:
+    """y = bf16(scale * (x @ q) + bias): x bf16 [M, K], (weight, weight_scale) from weight_quantize, bias fp32 [N].
+    At M <= SKINNY_M the kernel may split K (split_k 0 = choose) through the "splitk" workspace that gemm_skinny uses; a wider
+    call never splits, so it never grows that buffer (a captured CUDA graph may hold its address)."""
+    M, N, K = _weight_only_args(x, weight, weight_scale, weight_dtype)
+    if out is None:
+        out = torch.empty(M, N, dtype=BF16, device=x.device)
+    assert out.shape == (M, N) and out.stride(1) == 1
+    if bias is not None:
+        _chk(bias, "bias", torch.float32)
+        assert bias.numel() == N
+    ws = None
+    if M <= SKINNY_M:
+        ws = _zero_workspace(M * N * 4, x.device, "splitk")
+    elif split_k > 1:
+        raise ValueError(f"weight_only_linear: split_k={split_k} at {M} rows (K is split at most {SKINNY_M} rows)")
+    call("b200_weight_only_gemm_bf16", ptr(x), ptr(weight), ptr(weight_scale), ptr(bias), ptr(out), ptr(ws), M, N, K,
+         x.stride(0), out.stride(0), split_k, stream_ptr())
+    return out
+
+
+def weight_only_linear_f32(x: torch.Tensor, weight: torch.Tensor, weight_scale: torch.Tensor, *, tag: str = "splitk_f32",
+                           split_k: int = 0) -> torch.Tensor:
+    """weight_only_linear whose result stays as fp32 sums in a (zero-on-entry) workspace [M, N]; the consumer kernel
+    (add_rmsnorm_f32 / decode_rope_append_f32 / swiglu_fwd_f32) rounds once and re-zeroes it, as after gemm_skinny_f32.
+    Returns the fp32 workspace view."""
+    M, N, K = _weight_only_args(x, weight, weight_scale, "int8")
+    ws = _zero_workspace(M * N * 4, x.device, tag)
+    call("b200_weight_only_gemm_f32", ptr(x), ptr(weight), ptr(weight_scale), ptr(ws), M, N, K, x.stride(0), split_k,
+         stream_ptr())
+    return ws[: M * N * 4].view(torch.float32).view(M, N)
+
+
+# ----------------------------------------------------------------------------------------------------------
 # RMSNorm
 # ----------------------------------------------------------------------------------------------------------
 def rmsnorm_fwd(x: torch.Tensor, w: torch.Tensor, eps: float, out: Optional[torch.Tensor] = None,

@@ -20,19 +20,19 @@ from paddlenlp_b200.experimental.transformers import LlamaForCausalLMInferenceMo
 PRESETS = {"llama3_8b": T.LlamaConfig.llama3_8b, "llama3_2_1b": T.LlamaConfig.llama3_2_1b, "qwen2_0_5b": T.Qwen2Config.qwen2_0_5b}
 
 
-def run(batch=64, prompt=128, gen=1920, layers=0, graph=True, pdl=True, block_attn=False, preset="llama3_8b"):
+def run(batch=64, prompt=128, gen=1920, layers=0, graph=True, pdl=True, block_attn=False, preset="llama3_8b", quant_type=""):
     class A:
         pass
     a = A()
     a.batch, a.prompt, a.gen, a.layers, a.no_graph, a.no_pdl, a.block_attn = batch, prompt, gen, layers, not graph, not pdl, block_attn
-    a.preset = preset
+    a.preset, a.quant_type = preset, quant_type
     return _run(a)
 
 
 def _run(a):
     make = PRESETS[a.preset]
     cfg = make(num_hidden_layers=a.layers) if a.layers else make()
-    m = LlamaForCausalLMInferenceModel(cfg, block_attn=a.block_attn)
+    m = LlamaForCausalLMInferenceModel(cfg, block_attn=a.block_attn, quant_type=a.quant_type)
     m.init_random(seed=42)
     g = torch.Generator().manual_seed(1234)
     ids = torch.randint(0, cfg.vocab_size, (a.batch, a.prompt), generator=g).cuda()
@@ -60,7 +60,9 @@ def _run(a):
     L = cfg.num_hidden_layers
     h, I, V = cfg.hidden_size, cfg.intermediate_size, cfg.vocab_size
     kvd = cfg.num_key_value_heads * (h // cfg.num_attention_heads)
-    w_bytes = L * (h * (h + 2 * kvd) + h * h + 3 * h * I) * 2 + V * h * 2
+    layer_params = L * (h * (h + 2 * kvd) + h * h + 3 * h * I)
+    # int8 layer weights: one byte each plus a bf16 scale per output channel; embeddings and head stay bf16
+    w_bytes = (layer_params + L * (h + 2 * kvd + h + 2 * I + h) * 2 if a.quant_type else layer_params * 2) + V * h * 2
     kv_per_tok = 2 * L * a.batch * kvd * 2
     mean_t = a.prompt + steps / 2.0
     bytes_per_step = w_bytes + kv_per_tok * mean_t
@@ -71,7 +73,8 @@ def _run(a):
     rec = dict(workload="Llama-3-8B generation decode, batch 64, prompt 128 -> +1920, FusedMultiTransformer KV-cache path "
                         "(BASELINE.json configs[4])" if (a.batch, a.prompt, a.gen, a.layers, a.preset) == (64, 128, 1920, 0, "llama3_8b")
                else f"{a.preset} decode, batch {a.batch}, prompt {a.prompt} -> +{a.gen}",
-               batch=a.batch, prompt=a.prompt, gen=a.gen, layers=L, paged_kv=bool(a.block_attn), prefill_ms=prefill_ms, decode_ms=decode_ms,
+               batch=a.batch, prompt=a.prompt, gen=a.gen, layers=L, paged_kv=bool(a.block_attn), quant_type=a.quant_type,
+               prefill_ms=prefill_ms, decode_ms=decode_ms,
                ms_per_step=ms_step,
                decode_tokens_per_s=a.batch * steps / (decode_ms / 1e3), bytes_per_step_gb=bytes_per_step / 1e9,
                achieved_gbs=achieved, hbm_peak_gbs=peaks["hbm_gbs"], roofline_frac=achieved / peaks["hbm_gbs"],
@@ -90,6 +93,8 @@ def main():
     ap.add_argument("--no-pdl", action="store_true")
     ap.add_argument("--preset", choices=sorted(PRESETS), default="llama3_8b")
     ap.add_argument("--block-attn", action="store_true", help="paged KV cache (FusedBlockMultiTransformer, 64-row blocks)")
+    ap.add_argument("--quant-type", default="", choices=["", "weight_only_int8"],
+                    help="weight_only_int8: int8 layer weights with per-channel scales (FusedMultiTransformerWeightOnly)")
     a = ap.parse_args()
     print(json.dumps(_run(a)), flush=True)
 

@@ -91,12 +91,13 @@ def main():
     ap.add_argument("--layers", type=int, default=0)
     ap.add_argument("--seed", type=int, default=1234)
     ap.add_argument("--rounds", type=int, default=2, help="rounds of all modes, alternating")
+    ap.add_argument("--quant-type", default="", choices=["", "weight_only_int8"], help="int8 layer weights (weight-only)")
     a = ap.parse_args()
     if a.requests % STATIC_BATCH:
         raise SystemExit(f"--requests must be a multiple of {STATIC_BATCH}")
     make = gen_bench.PRESETS[a.preset]
     cfg = make(num_hidden_layers=a.layers) if a.layers else make()
-    m = LlamaForCausalLMInferenceModel(cfg, block_attn=True, append_attn=True, block_size=64)
+    m = LlamaForCausalLMInferenceModel(cfg, block_attn=True, append_attn=True, block_size=64, quant_type=a.quant_type)
     m.init_random(seed=42)
     reqs = make_requests(a.requests, cfg.vocab_size, a.seed, a.prompt, a.out)
     max_prompt, max_out = a.prompt[1], a.out[1]
@@ -116,8 +117,9 @@ def main():
             r["useful_tokens_per_s"] = useful / r["seconds"]
     del m
     torch.cuda.empty_cache()
-    ref = gen_bench.run(batch=STATIC_BATCH, prompt=128, gen=256, block_attn=True, preset=a.preset, layers=a.layers)
-    print(json.dumps(dict(preset=a.preset, requests=a.requests, prompt=a.prompt, out=a.out, useful_tokens=useful, **card(),
+    ref = gen_bench.run(batch=STATIC_BATCH, prompt=128, gen=256, block_attn=True, preset=a.preset, layers=a.layers,
+                        quant_type=a.quant_type)
+    print(json.dumps(dict(preset=a.preset, quant_type=a.quant_type, requests=a.requests, prompt=a.prompt, out=a.out, useful_tokens=useful, **card(),
                           runs=runs, gen_bench_block_attn=dict(batch=STATIC_BATCH, ms_per_step=ref["ms_per_step"])),
                      indent=1), flush=True)
 
