@@ -442,6 +442,40 @@ int b200_append_attention(void* qkv, void* key_cache, void* value_cache, const i
                           int64_t rope_positions, int64_t ldq, int64_t ldo, float softmax_scale, int64_t num_splits,
                           cudaStream_t stream);
 
+/* int8 paged KV cache (cachekv_int8_type="static"; append_attention's cache_int8 mode, append_attention_kernel.h:224).
+ * key_cache / value_cache: uint8 [num_blocks, kvh, block_size, head_dim], the bf16 cache's shape and row formula with 1-byte
+ * elements.  Per kv head a quantise scale s (cache_k_scale / cache_v_scale) and a dequantise scale o = 1 / s
+ * (cache_k_out_scale / cache_v_out_scale), each bf16 [kvh].  A cache byte holds
+ *     u = clamp(rne(bf16(s * x)), -127, 127) + 128
+ * of the post-RoPE bf16 value x that the bf16 cache would hold (bf16 product, then round to nearest integer with ties to
+ * even), for prompt and decode rows alike, and reads back as (u - 128) * o.  The attention kernels apply o once per kv head:
+ * o_k on the softmax scale, o_v on the output; a dequantised value is never rounded to bf16.  Each entry point mirrors its bf16
+ * twin above; a null scale array, an unsupported shape or an unsupported block size is an argument error before any launch.
+ * head_dim must also be a multiple of 16.  The writers take the quantise scales, decode attention the dequantise scales,
+ * b200_append_attention_c8 (which writes and reads) all four.  Workspaces are the bf16 twins'. */
+int b200_write_cache_kv_paged_c8(const void* qkv, void* key_cache, void* value_cache, const int32_t* block_tables,
+                                 const void* cache_k_scale, const void* cache_v_scale, const int32_t* seq_lens, int64_t B,
+                                 int64_t S, int64_t num_heads, int64_t num_kv_heads, int64_t head_dim, int64_t block_size,
+                                 int64_t max_blocks_per_seq, int64_t ld, cudaStream_t stream);
+int b200_decode_rope_append_paged_c8(void* qkv, float* acc_f32_ws, const float* bias, void* key_cache, void* value_cache,
+                                     const int32_t* block_tables, const void* cache_k_scale, const void* cache_v_scale,
+                                     const float* cos_table, const float* sin_table, const int32_t* seq_lens, int64_t B,
+                                     int64_t num_heads, int64_t num_kv_heads, int64_t head_dim, int64_t block_size,
+                                     int64_t max_blocks_per_seq, int64_t ld, cudaStream_t stream);
+int b200_decode_attention_paged_c8(const void* qkv, const void* key_cache, const void* value_cache, const int32_t* block_tables,
+                                   const void* cache_k_out_scale, const void* cache_v_out_scale, const int32_t* seq_lens,
+                                   void* out, void* workspace, int64_t B, int64_t num_heads, int64_t num_kv_heads,
+                                   int64_t head_dim, int64_t num_blocks, int64_t block_size, int64_t max_blocks_per_seq,
+                                   int64_t ld, float softmax_scale, int64_t num_splits, cudaStream_t stream);
+int b200_append_attention_c8(void* qkv, void* key_cache, void* value_cache, const void* cache_k_scale, const void* cache_v_scale,
+                             const void* cache_k_out_scale, const void* cache_v_out_scale, const int32_t* seq_lens_encoder,
+                             const int32_t* seq_lens_decoder, const int32_t* seq_lens_this_time, const int32_t* cu_seqlens_q,
+                             const int32_t* block_tables, const float* cos_table, const float* sin_table, void* out,
+                             void* workspace, int64_t B, int64_t token_num, int64_t max_q_len, int64_t num_heads,
+                             int64_t num_kv_heads, int64_t head_dim, int64_t num_blocks, int64_t block_size,
+                             int64_t max_blocks_per_seq, int64_t rope_positions, int64_t ldq, int64_t ldo, float softmax_scale,
+                             int64_t num_splits, cudaStream_t stream);
+
 /* update_inputs: csrc/gpu/update_inputs.cu:18-82 */
 int b200_update_inputs(bool* not_need_stop, int32_t* seq_lens_this_time, int32_t* seq_lens_encoder,
                        int32_t* seq_lens_decoder, int64_t* input_ids, const int64_t* stop_nums, const bool* stop_flags,

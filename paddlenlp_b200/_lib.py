@@ -91,6 +91,10 @@ _SIGNATURES = {
     "b200_save_output_stream": [P, P, P, I64, I64, P, I64, I64, P],
     "b200_append_attention_workspace_bytes": [I64, I64, I64, I64, I64],
     "b200_append_attention": [P] * 12 + [I64] * 12 + [F, I64, P],
+    "b200_write_cache_kv_paged_c8": [P] * 7 + [I64] * 8 + [P],
+    "b200_decode_rope_append_paged_c8": [P] * 11 + [I64] * 7 + [P],
+    "b200_decode_attention_paged_c8": [P] * 9 + [I64] * 8 + [F, I64, P],
+    "b200_append_attention_c8": [P] * 16 + [I64] * 12 + [F, I64, P],
     "b200_update_inputs": [P, P, P, P, P, P, P, P, P, I64, I64, I64, P],
     "b200_generate_step_update": [P, P, P, P, P, P, I64, P, I64, P, I64, I64, P, P, I64, P],
     "b200_argmax_f32": [P, P, I64, I64, I64, P],
@@ -141,6 +145,7 @@ KERNELS_PER_CALL = {
     "b200_rope_inplace": 1, "b200_swiglu_fwd": 1, "b200_swiglu_bwd": 1, "b200_embedding_fwd": 1, "b200_embedding_bwd": 1,
     "b200_fa_fwd": 1, "b200_fa_bwd": 5, "b200_fa_fwd_flashmask": 1, "b200_fa_bwd_flashmask": 5, "b200_ce_fwd": 2, "b200_ce_bwd": 1, "b200_ce_rows_fwd": 1, "b200_ce_reduce": 1, "b200_argmax_bf16": 1, "b200_grad_sqnorm": 2, "b200_grad_sqnorm_f32": 2,
     "b200_adamw_step": 1, "b200_bf16_to_f32": 1, "b200_token_penalty_multi_scores": 2, "b200_generate_step_update": 2, "b200_decode_attention": 2, "b200_decode_attention_tc": 2, "b200_decode_attention_paged": 2, "b200_append_attention": 5,
+    "b200_decode_attention_paged_c8": 2, "b200_append_attention_c8": 5,
 }
 launch_count = 0       # kernels launched through this module since import
 call_hook = None       # optional callable(name, args) -> context manager, used by bench.py to time one kernel family

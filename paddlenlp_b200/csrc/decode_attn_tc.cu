@@ -17,8 +17,15 @@
 //     through shared memory at the end;
 //   * split-KV partials ([B*nh, nsplit, 132] fp32: unnormalised o in the first d columns, running max and sum at columns 128
 //     and 129, whatever d is) are merged by decode_attention_merge_kernel.
+// The int8 paged cache (KvCacheC8, cachekv_int8_type="static") runs the same kernel with 1-byte elements: a chunk keeps its
+// row count (so a lane's rows x G scores, where the registers grow, are the bf16 kernel's) and is 4 KB, and the ring has 8
+// stages instead of 4, so the bytes in flight per SM are unchanged.  Each lane turns its 8 bytes of a row into the exact fp32
+// u - 128 (dequant_c8); the per-head dequantise scales are applied once: o_k on the query scale, o_v on the merged output
+// before the normalisation and before a split-KV partial is written.
 // b200_decode_attention (decode_attention_kernel below, plain global loads, dense cache) computes the same function and is the
 // cross-check.  Cache rows are addressed through KvCache (kv_cache.cuh).
+#include <type_traits>
+
 #include "../../include/b200nlp.h"
 #include "common.cuh"
 #include "host_util.h"
@@ -27,14 +34,25 @@
 namespace b200 {
 namespace dab {
 
-constexpr int CHUNK_BYTES = 8192;              // K (and as much V) per stage: 32 rows at d = 128, 64 rows at d = 64
-constexpr int NST = 4;                         // ring stages
-constexpr int SMEM_BYTES = NST * 2 * CHUNK_BYTES;
+constexpr int SMEM_BYTES = 65536;              // the ring: NST stages of a K and a V chunk
 constexpr int NUM_THREADS = 160;               // 4 consumer warps + 1 producer warp
+// K (and as much V) per stage: 32 rows at d = 128, 64 rows at d = 64, whatever the element type: 8 KB in 4 stages (bf16),
+// 4 KB in 8 stages (uint8)
+template <typename T>
+constexpr int CHUNK_BYTES = 4096 * static_cast<int>(sizeof(T));
+template <typename T>
+constexpr int NST = SMEM_BYTES / (2 * CHUNK_BYTES<T>);
 
+__device__ __forceinline__ uint2 ld_shared_v2(uint32_t saddr) {
+  uint2 v;
+  asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(saddr));
+  return v;
+}
+
+template <typename T>
 struct Params {
   const bf16* qkv;
-  KvCache kv;         // dense or paged, as the PAGED instantiation says
+  KvCacheT<T> kv;     // dense or paged, as the PAGED instantiation says; uint8 only paged
   const int* seq_lens;
   bf16* out;          // [B, nh*d]
   float* partial;     // [B*nh, nsplit, 132] or null
@@ -43,13 +61,27 @@ struct Params {
   float scale_log2;
 };
 
-template <int D, int G, bool PAGED>
-__global__ void __launch_bounds__(NUM_THREADS, (G <= 4 ? 2 : 1)) decode_attention_bulk_kernel(const Params p) {
-  constexpr int ROWS = CHUNK_BYTES / (D * 2);                // cache rows per chunk
+// A lane's 8 cache elements of one row -> fp32: bf16 as they are, uint8 as the exact u - 128 (kv_cache.cuh)
+__device__ __forceinline__ void row8_to_f32(const uint4& x, float (&f)[8]) {
+  const uint32_t* xi = reinterpret_cast<const uint32_t*>(&x);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) { const float2 a = unpack_bf16x2(xi[j]); f[2 * j] = a.x; f[2 * j + 1] = a.y; }
+}
+__device__ __forceinline__ void row8_to_f32(const uint2& x, float (&f)[8]) {
+  f[0] = dequant_c8<0>(x.x); f[1] = dequant_c8<1>(x.x); f[2] = dequant_c8<2>(x.x); f[3] = dequant_c8<3>(x.x);
+  f[4] = dequant_c8<0>(x.y); f[5] = dequant_c8<1>(x.y); f[6] = dequant_c8<2>(x.y); f[7] = dequant_c8<3>(x.y);
+}
+
+template <int D, int G, bool PAGED, typename T>
+__global__ void __launch_bounds__(NUM_THREADS, (G <= 4 ? 2 : 1)) decode_attention_bulk_kernel(const Params<T> p) {
+  constexpr bool C8 = sizeof(T) == 1;
+  constexpr int ES = static_cast<int>(sizeof(T));            // bytes per cache element
+  constexpr int CHUNK = CHUNK_BYTES<T>, NSTAGE = NST<T>;
+  constexpr int ROWS = CHUNK / (D * ES);                     // cache rows per chunk
   constexpr int LPR = D / 8, LPR_LOG2 = D == 128 ? 4 : 3;   // lanes per cache row
   constexpr int NG = 128 / LPR;                              // row groups of the four consumer warps
   extern __shared__ __align__(128) uint8_t ring[];
-  __shared__ uint64_t full_bar[NST], empty_bar[NST];
+  __shared__ uint64_t full_bar[NSTAGE], empty_bar[NSTAGE];
   __shared__ float s_m[NG][G], s_l[NG][G];
   __shared__ float s_o[NG][G][D];
   const int b = blockIdx.x / p.kv.kvh, kh = blockIdx.x % p.kv.kvh;
@@ -61,7 +93,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (G <= 4 ? 2 : 1)) decode_attentio
   const int nchunks = len > t_begin ? (len - t_begin + ROWS - 1) / ROWS : 0;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
-    for (int i = 0; i < NST; ++i) {
+    for (int i = 0; i < NSTAGE; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 4);
     }
@@ -75,26 +107,26 @@ __global__ void __launch_bounds__(NUM_THREADS, (G <= 4 ? 2 : 1)) decode_attentio
     // ------------------------------- producer -------------------------------
     if (lane == 0) {
       for (int c = 0; c < nchunks; ++c) {
-        const int st = c % NST;
-        mbar_wait(&empty_bar[st], ((c / NST) & 1) ^ 1);
+        const int st = c % NSTAGE;
+        mbar_wait(&empty_bar[st], ((c / NSTAGE) & 1) ^ 1);
         const int t0 = t_begin + c * ROWS;
-        const uint32_t bytes = static_cast<uint32_t>(min(ROWS, len - t0)) * D * 2;
+        const uint32_t bytes = static_cast<uint32_t>(min(ROWS, len - t0)) * D * ES;
         if constexpr (PAGED && ROWS > 32) {
           // t0 is a multiple of ROWS, so the chunk starts on a page and spans ROWS / block_size pages when those are shorter
           mbar_arrive_expect_tx(&full_bar[st], 2 * bytes);
           const int n = min(ROWS, len - t0);
           for (int r0 = 0; r0 < n; r0 += p.kv.block_size) {
-            const size_t off = p.kv.offset<true, D>(b, kh, t0 + r0);
-            const uint32_t piece = static_cast<uint32_t>(min(p.kv.block_size, n - r0)) * D * 2;
-            bulk_load(ring + st * 2 * CHUNK_BYTES + r0 * D * 2, p.kv.k + off, piece, &full_bar[st]);
-            bulk_load(ring + st * 2 * CHUNK_BYTES + CHUNK_BYTES + r0 * D * 2, p.kv.v + off, piece, &full_bar[st]);
+            const size_t off = p.kv.template offset<true, D>(b, kh, t0 + r0);
+            const uint32_t piece = static_cast<uint32_t>(min(p.kv.block_size, n - r0)) * D * ES;
+            bulk_load(ring + st * 2 * CHUNK + r0 * D * ES, p.kv.k + off, piece, &full_bar[st]);
+            bulk_load(ring + st * 2 * CHUNK + CHUNK + r0 * D * ES, p.kv.v + off, piece, &full_bar[st]);
           }
           continue;
         }
-        const size_t off = p.kv.offset<PAGED, D>(b, kh, t0);
+        const size_t off = p.kv.template offset<PAGED, D>(b, kh, t0);
         mbar_arrive_expect_tx(&full_bar[st], 2 * bytes);
-        bulk_load(ring + st * 2 * CHUNK_BYTES, p.kv.k + off, bytes, &full_bar[st]);
-        bulk_load(ring + st * 2 * CHUNK_BYTES + CHUNK_BYTES, p.kv.v + off, bytes, &full_bar[st]);
+        bulk_load(ring + st * 2 * CHUNK, p.kv.k + off, bytes, &full_bar[st]);
+        bulk_load(ring + st * 2 * CHUNK + CHUNK, p.kv.v + off, bytes, &full_bar[st]);
       }
     }
     return;
@@ -107,6 +139,8 @@ __global__ void __launch_bounds__(NUM_THREADS, (G <= 4 ? 2 : 1)) decode_attentio
   if constexpr (D == 128) hmask = (lane < 16) ? 0x0000ffffu : 0xffff0000u;
   else hmask = 0xffu << (lane & 24);
   float q[G][8], o[G][8], m[G], l[G];
+  float q_scale = p.scale_log2;
+  if constexpr (C8) q_scale *= __bfloat162float(p.kv.k_out_scale[kh]);   // K = (u - 128) o_k: o_k folds into the query scale
 #pragma unroll
   for (int g = 0; g < G; ++g) {
     const uint4 qv = *reinterpret_cast<const uint4*>(p.qkv + static_cast<size_t>(b) * p.ld + (kh * G + g) * D + sub * 8);
@@ -114,7 +148,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (G <= 4 ? 2 : 1)) decode_attentio
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const float2 f = unpack_bf16x2(qi[j]);
-      q[g][2 * j] = f.x * p.scale_log2; q[g][2 * j + 1] = f.y * p.scale_log2;
+      q[g][2 * j] = f.x * q_scale; q[g][2 * j + 1] = f.y * q_scale;
     }
 #pragma unroll
     for (int j = 0; j < 8; ++j) o[g][j] = 0.f;
@@ -122,18 +156,25 @@ __global__ void __launch_bounds__(NUM_THREADS, (G <= 4 ? 2 : 1)) decode_attentio
   }
   constexpr int U = ROWS / NG;                         // rows per row group and chunk
   const uint32_t ring_s = smem_u32(ring);
+  // a lane's 8 elements of a row: one 16-byte word of bf16, or the first half of one of uint8
+  using Row8 = typename std::conditional<C8, uint2, uint4>::type;
   for (int c = 0; c < nchunks; ++c) {
-    const int st = c % NST;
+    const int st = c % NSTAGE;
     const int rows = min(ROWS, len - (t_begin + c * ROWS));
-    mbar_wait(&full_bar[st], (c / NST) & 1);
-    const uint32_t kb = ring_s + st * 2 * CHUNK_BYTES, vb = kb + CHUNK_BYTES;
-    uint4 kv[U], vv[U];
+    mbar_wait(&full_bar[st], (c / NSTAGE) & 1);
+    const uint32_t kb = ring_s + st * 2 * CHUNK, vb = kb + CHUNK;
+    Row8 kv[U], vv[U];
 #pragma unroll
     for (int u = 0; u < U; ++u) {
       const int r = hw + NG * u;
       if (r < rows) {
-        kv[u] = ld_shared_v4(kb + r * (D * 2) + sub * 16);
-        vv[u] = ld_shared_v4(vb + r * (D * 2) + sub * 16);
+        if constexpr (C8) {
+          kv[u] = ld_shared_v2(kb + r * D + sub * 8);
+          vv[u] = ld_shared_v2(vb + r * D + sub * 8);
+        } else {
+          kv[u] = ld_shared_v4(kb + r * (D * 2) + sub * 16);
+          vv[u] = ld_shared_v4(vb + r * (D * 2) + sub * 16);
+        }
       }
     }
     __syncwarp();
@@ -141,10 +182,8 @@ __global__ void __launch_bounds__(NUM_THREADS, (G <= 4 ? 2 : 1)) decode_attentio
     float sc[U][G];
 #pragma unroll
     for (int u = 0; u < U; ++u) {
-      const uint32_t* ki = reinterpret_cast<const uint32_t*>(&kv[u]);
       float kf[8];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) { const float2 a = unpack_bf16x2(ki[j]); kf[2 * j] = a.x; kf[2 * j + 1] = a.y; }
+      row8_to_f32(kv[u], kf);
 #pragma unroll
       for (int g = 0; g < G; ++g) {
         float sdot = 0.f;
@@ -176,10 +215,8 @@ __global__ void __launch_bounds__(NUM_THREADS, (G <= 4 ? 2 : 1)) decode_attentio
 #pragma unroll
     for (int u = 0; u < U; ++u) {
       if (hw + NG * u < rows) {                        // uniform within the row group
-        const uint32_t* vi = reinterpret_cast<const uint32_t*>(&vv[u]);
         float vf[8];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) { const float2 cc = unpack_bf16x2(vi[j]); vf[2 * j] = cc.x; vf[2 * j + 1] = cc.y; }
+        row8_to_f32(vv[u], vf);
 #pragma unroll
         for (int g = 0; g < G; ++g) {
           const float pr = fast_exp2(sc[u][g] - m[g]);
@@ -198,6 +235,8 @@ __global__ void __launch_bounds__(NUM_THREADS, (G <= 4 ? 2 : 1)) decode_attentio
     for (int j = 0; j < 8; ++j) s_o[hw][g][sub * 8 + j] = o[g][j];
   }
   named_bar_sync(1, 128);
+  float v_scale = 1.f;
+  if constexpr (C8) v_scale = __bfloat162float(p.kv.v_out_scale[kh]);      // V = (u - 128) o_v
   for (int idx = threadIdx.x; idx < G * D; idx += 128) {
     const int g = idx / D, dd = idx % D;
     float mm = -INFINITY;
@@ -210,6 +249,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (G <= 4 ? 2 : 1)) decode_attentio
       acc += s_o[w][g][dd] * f;
       lt += s_l[w][g] * f;
     }
+    if constexpr (C8) acc *= v_scale;
     if (nsplit == 1) {
       p.out[static_cast<size_t>(b) * p.nh * D + (kh * G + g) * D + dd] = __float2bfloat16_rn(lt > 0.f ? acc / lt : 0.f);
     } else {
@@ -407,14 +447,14 @@ static int launch_merge(const float* partial, bf16* out, int rows, int nsplit, i
   return check_launch("decode_attention(merge)");
 }
 
-template <int D, bool PAGED>
-static int launch(const Params& p, int G, int64_t num_splits, cudaStream_t stream) {
+template <int D, bool PAGED, typename T>
+static int launch(const Params<T>& p, int G, int64_t num_splits, cudaStream_t stream) {
   const dim3 grid(static_cast<unsigned>(p.B * p.kv.kvh), static_cast<unsigned>(num_splits));
 #define B200_DAB(GG)                                                                                                 \
   case GG: {                                                                                                         \
     static bool attr_set = false;                                                                                    \
     if (!attr_set) {                                                                                                 \
-      cudaError_t e = cudaFuncSetAttribute(decode_attention_bulk_kernel<D, GG, PAGED>,                               \
+      cudaError_t e = cudaFuncSetAttribute(decode_attention_bulk_kernel<D, GG, PAGED, T>,                               \
                                            cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);                \
       if (e != cudaSuccess) {                                                                                        \
         set_last_error("decode_attention smem attr: %s", cudaGetErrorString(e));                                     \
@@ -422,7 +462,7 @@ static int launch(const Params& p, int G, int64_t num_splits, cudaStream_t strea
       }                                                                                                              \
       attr_set = true;                                                                                               \
     }                                                                                                                \
-    launch_pdl(decode_attention_bulk_kernel<D, GG, PAGED>, grid, dim3(NUM_THREADS), SMEM_BYTES, stream, p);             \
+    launch_pdl(decode_attention_bulk_kernel<D, GG, PAGED, T>, grid, dim3(NUM_THREADS), SMEM_BYTES, stream, p);             \
   } break;
   switch (G) {   // 1 to 8: check_decode_attention()
     B200_DAB(1) B200_DAB(2) B200_DAB(3) B200_DAB(4) B200_DAB(5) B200_DAB(6) B200_DAB(7) B200_DAB(8)
@@ -436,7 +476,8 @@ static int launch(const Params& p, int G, int64_t num_splits, cudaStream_t strea
 }  // namespace dab
 
 // The checks every decode-attention entry point makes beyond its cache view; `what` names the entry point in the message.
-int check_decode_attention(const char* what, const KvCache& kv, const void* qkv, const int32_t* seq_lens, const void* out,
+template <typename T>
+int check_decode_attention(const char* what, const KvCacheT<T>& kv, const void* qkv, const int32_t* seq_lens, const void* out,
                            const void* workspace, int64_t B, int64_t num_heads, int64_t ld, int64_t num_splits) {
   B200_CHECK_ARG(qkv && seq_lens && out, "%s: null pointer", what);
   B200_CHECK_ARG(num_splits >= 1 && num_splits <= 64 && (num_splits == 1 || workspace), "%s: bad num_splits / workspace", what);
@@ -447,10 +488,12 @@ int check_decode_attention(const char* what, const KvCache& kv, const void* qkv,
   return 0;
 }
 
-// Streaming-kernel decode attention over a dense or paged view whose arguments passed check_decode_attention().
-int launch_decode_attention(const KvCache& kv, const void* qkv, const int32_t* seq_lens, void* out, void* workspace, int64_t B,
+// Streaming-kernel decode attention over a dense or paged view whose arguments passed check_decode_attention().  The uint8
+// view is paged only.
+template <typename T>
+int launch_decode_attention(const KvCacheT<T>& kv, const void* qkv, const int32_t* seq_lens, void* out, void* workspace, int64_t B,
                             int64_t num_heads, int64_t ld, float softmax_scale, int64_t num_splits, cudaStream_t stream) {
-  dab::Params p = {};
+  dab::Params<T> p = {};
   p.qkv = static_cast<const bf16*>(qkv);
   p.kv = kv;
   p.seq_lens = seq_lens;
@@ -460,10 +503,22 @@ int launch_decode_attention(const KvCache& kv, const void* qkv, const int32_t* s
   p.ld = ld;
   p.scale_log2 = softmax_scale * 1.4426950408889634f;
   const int G = static_cast<int>(num_heads / kv.kvh);
-  if (kv.block_tables != nullptr)
+  if constexpr (sizeof(T) == 1) {
     return kv.d == 64 ? dab::launch<64, true>(p, G, num_splits, stream) : dab::launch<128, true>(p, G, num_splits, stream);
-  return kv.d == 64 ? dab::launch<64, false>(p, G, num_splits, stream) : dab::launch<128, false>(p, G, num_splits, stream);
+  } else {
+    if (kv.block_tables != nullptr)
+      return kv.d == 64 ? dab::launch<64, true>(p, G, num_splits, stream) : dab::launch<128, true>(p, G, num_splits, stream);
+    return kv.d == 64 ? dab::launch<64, false>(p, G, num_splits, stream) : dab::launch<128, false>(p, G, num_splits, stream);
+  }
 }
+template int check_decode_attention(const char*, const KvCache&, const void*, const int32_t*, const void*, const void*, int64_t,
+                                    int64_t, int64_t, int64_t);
+template int check_decode_attention(const char*, const KvCacheC8&, const void*, const int32_t*, const void*, const void*, int64_t,
+                                    int64_t, int64_t, int64_t);
+template int launch_decode_attention(const KvCache&, const void*, const int32_t*, void*, void*, int64_t, int64_t, int64_t, float,
+                                     int64_t, cudaStream_t);
+template int launch_decode_attention(const KvCacheC8&, const void*, const int32_t*, void*, void*, int64_t, int64_t, int64_t, float,
+                                     int64_t, cudaStream_t);
 
 }  // namespace b200
 
@@ -529,6 +584,22 @@ extern "C" int b200_decode_attention_paged(const void* qkv, const void* key_cach
     return rc;
   B200_CHECK_ARG(num_blocks > 0, "decode_attention_paged: bad shape");
   if (int rc = check_decode_attention("decode_attention_paged", kv, qkv, seq_lens, out, workspace, B, num_heads, ld, num_splits))
+    return rc;
+  return launch_decode_attention(kv, qkv, seq_lens, out, workspace, B, num_heads, ld, softmax_scale, num_splits, stream);
+}
+
+extern "C" int b200_decode_attention_paged_c8(const void* qkv, const void* key_cache, const void* value_cache,
+                                              const int32_t* block_tables, const void* cache_k_out_scale,
+                                              const void* cache_v_out_scale, const int32_t* seq_lens, void* out, void* workspace,
+                                              int64_t B, int64_t num_heads, int64_t num_kv_heads, int64_t head_dim,
+                                              int64_t num_blocks, int64_t block_size, int64_t max_blocks_per_seq, int64_t ld,
+                                              float softmax_scale, int64_t num_splits, cudaStream_t stream) {
+  KvCacheC8 kv;
+  if (int rc = paged_kv_cache_c8(&kv, key_cache, value_cache, block_tables, nullptr, nullptr, cache_k_out_scale, cache_v_out_scale,
+                                 false, true, num_kv_heads, head_dim, block_size, max_blocks_per_seq, "decode_attention_paged_c8"))
+    return rc;
+  B200_CHECK_ARG(num_blocks > 0, "decode_attention_paged_c8: bad shape");
+  if (int rc = check_decode_attention("decode_attention_paged_c8", kv, qkv, seq_lens, out, workspace, B, num_heads, ld, num_splits))
     return rc;
   return launch_decode_attention(kv, qkv, seq_lens, out, workspace, B, num_heads, ld, softmax_scale, num_splits, stream);
 }

@@ -22,8 +22,11 @@
 //   The order of operations on (m, l, O) is the mma.sync kernel's: O = O corr_j + P_j V_j per tile.
 // impl 1, fa_fwd_kernel: the mma.sync cross-check, and the only kernel of the paged-cache prefill of append_attention.  8 warps
 //   of 16 q rows each; K/V tiles double-buffered in 128-byte-row-swizzled shared memory with cp.async; Q stays in registers as
-//   mma A fragments; S, P and the O accumulator never leave the registers of the warp that owns the rows.  Three modes: plain
-//   causal, FlashMask start rows, and the paged prefill.
+//   mma A fragments; S, P and the O accumulator never leave the registers of the warp that owns the rows.  Four modes: plain
+//   causal, FlashMask start rows, and the paged prefill over a bf16 or a uint8 cache.  Over the uint8 cache
+//   (cachekv_int8_type="static") the cp.async loads fill a double-buffered staging area of cache bytes, and each tile is
+//   converted into the one bf16 K and V tile as the exact integers u - 128, so ldmatrix and mma.sync run unchanged on exact
+//   values; the per-head dequantise scales are applied once, o_k on the softmax scale and o_v on O.
 #include <climits>
 
 #include "../../include/b200nlp.h"
@@ -41,7 +44,7 @@ constexpr int BQ = 16 * NW;    // q rows per CTA (both kernels)
 // at the same points, and the paged prefill (mma.sync) agrees with the training forward (wgmma) to summation-order noise.
 constexpr int BKV = 128;
 
-enum Mode { DENSE = 0, MASK = 1, PAGED = 2 };
+enum Mode { DENSE = 0, MASK = 1, PAGED = 2, PAGED_C8 = 3 };
 
 struct Params {
   const bf16* q;
@@ -64,6 +67,7 @@ struct Params {
   const int* seq_this;
   const int* seq_enc;
   KvCache kv;
+  KvCacheC8 kv8;      // PAGED_C8: the uint8 cache and its scales (kv unused)
 };
 
 // With a document mask the leading kv tiles whose every column belongs to a document that ended at or before the q tile's
@@ -79,20 +83,42 @@ __device__ __forceinline__ int first_visible_kv_tile(const int* ms, int S, int q
 template <int D>
 __device__ __forceinline__ uint32_t swz(int row, int chunk) { return static_cast<uint32_t>(row * (D * 2) + ((chunk ^ (row & 7)) << 4)); }
 
+// Shared memory of fa_fwd_kernel: Q, then two K and two V bf16 tiles; over the uint8 cache one K and one V bf16 tile and the
+// staging area [2][K, V] of cache bytes (the same total).
+template <int D, int MODE>
+constexpr int fa_smem_bytes() {
+  return MODE == PAGED_C8 ? BQ * D * 2 + 2 * BKV * D * 2 + 4 * BKV * D : BQ * D * 2 + 4 * BKV * D * 2;
+}
+
+// 16 cache bytes -> 16 bf16 (two 16-byte chunks) holding the exact u - 128
+__device__ __forceinline__ void c8x16_to_bf16(const uint4& x, uint4& lo, uint4& hi) {
+  const uint32_t* xi = reinterpret_cast<const uint32_t*>(&x);
+  uint32_t r[8];
+#pragma unroll
+  for (int w = 0; w < 4; ++w) {
+    r[2 * w] = pack_bf16x2(dequant_c8<0>(xi[w]), dequant_c8<1>(xi[w]));
+    r[2 * w + 1] = pack_bf16x2(dequant_c8<2>(xi[w]), dequant_c8<3>(xi[w]));
+  }
+  lo = make_uint4(r[0], r[1], r[2], r[3]);
+  hi = make_uint4(r[4], r[5], r[6], r[7]);
+}
+
 template <int D, int MODE>
 __global__ void __launch_bounds__(NW * 32, 1) fa_fwd_kernel(const Params p) {
+  constexpr bool C8 = MODE == PAGED_C8;
   constexpr int CH = D / 8, CH_LOG2 = D == 128 ? 4 : 3;   // 16-byte chunks per row
   constexpr int KV_TILE_BYTES = BKV * D * 2;
   extern __shared__ __align__(128) uint8_t smem[];
   const uint32_t sQ = smem_u32(smem);
-  const uint32_t sK = sQ + BQ * D * 2;            // [2] K tiles
-  const uint32_t sV = sK + 2 * KV_TILE_BYTES;     // [2] V tiles
+  const uint32_t sK = sQ + BQ * D * 2;                     // [2] K tiles ([1] over the uint8 cache)
+  const uint32_t sV = sK + (C8 ? 1 : 2) * KV_TILE_BYTES;   // [2] V tiles ([1])
+  const uint32_t sS = sV + KV_TILE_BYTES;                  // uint8 cache: staging [2][K, V] of BKV * D bytes
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int head = blockIdx.y, batch = blockIdx.z;
   const int kv_head = head / (p.nh / p.kvh);
   int n_rows = p.S, pos0 = 0, tok0 = batch * p.S;
-  if constexpr (MODE == PAGED) {
+  if constexpr (MODE == PAGED || MODE == PAGED_C8) {
     n_rows = p.seq_this[batch];
     // decode rows (one new token on top of a cache, no prompt) belong to the decode kernel; idle slots to nobody
     if (n_rows <= 0 || (n_rows == 1 && p.seq_enc[batch] <= 0)) return;
@@ -108,13 +134,28 @@ __global__ void __launch_bounds__(NW * 32, 1) fa_fwd_kernel(const Params p) {
   int j_lo = 0;
   if constexpr (MODE == MASK) j_lo = first_visible_kv_tile(p.mask_start + static_cast<size_t>(batch) * p.S, p.S, q0, n_kv, BKV);
 
-  const bf16* kbase = MODE == PAGED ? p.kv.k : p.k;
+  const bf16* kbase = MODE == PAGED ? p.kv.k : p.k;   // (PAGED_C8: unused)
   const bf16* vbase = MODE == PAGED ? p.kv.v : p.v;
   auto kv_row = [&](const bf16* base, int64_t ld, int c) -> const bf16* {
     if constexpr (MODE == PAGED) return base + p.kv.offset<true, D>(batch, kv_head, c);
     else return base + static_cast<size_t>(tok0 + c) * ld + kv_head * D;
   };
   auto load_kv = [&](int j, int buf) {
+    if constexpr (C8) {
+      constexpr int CH8 = D / 16, CH8_LOG2 = D == 128 ? 3 : 2;    // 16-byte chunks per cache row
+      const uint8_t* kc = p.kv8.k;
+      const uint8_t* vc = p.kv8.v;
+      const uint32_t st = sS + buf * 2 * BKV * D;
+      for (int i = threadIdx.x; i < BKV * CH8; i += NW * 32) {
+        const int r = i >> CH8_LOG2, ch = i & (CH8 - 1), c = j * BKV + r;
+        const bool ok = c < kv_total;
+        const size_t off = ok ? p.kv8.offset<true, D>(batch, kv_head, c) + ch * 16 : 0;
+        // rows past the sequence read as u = 0 (-128 after the conversion): masked in S, and P = 0 in P V
+        cp_async_16(st + r * D + ch * 16, kc + off, ok ? 16u : 0u);
+        cp_async_16(st + BKV * D + r * D + ch * 16, vc + off, ok ? 16u : 0u);
+      }
+      return;
+    }
     for (int i = threadIdx.x; i < BKV * CH; i += NW * 32) {
       const int r = i >> CH_LOG2, ch = i & (CH - 1), c = j * BKV + r;
       const bool ok = c < kv_total;
@@ -137,6 +178,8 @@ __global__ void __launch_bounds__(NW * 32, 1) fa_fwd_kernel(const Params p) {
   for (int i = 0; i < D / 8; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
   uint32_t qf[D / 16][4];
+  float scale_log2 = p.scale_log2;
+  if constexpr (C8) scale_log2 *= __bfloat162float(p.kv8.k_out_scale[kv_head]);   // K = (u - 128) o_k
 
   for (int j = j_lo; j < n_kv; ++j) {
     const int buf = (j - j_lo) & 1;
@@ -148,6 +191,23 @@ __global__ void __launch_bounds__(NW * 32, 1) fa_fwd_kernel(const Params p) {
       cp_async_wait<0>();
     }
     __syncthreads();
+    if constexpr (C8) {
+      // staging buffer `buf` -> the bf16 K and V tiles (free: the previous tile's readers passed the barrier at the loop's end)
+      constexpr int CH8 = D / 16, CH8_LOG2 = D == 128 ? 3 : 2;
+      const uint32_t st = sS + buf * 2 * BKV * D;
+      for (int i = threadIdx.x; i < 2 * BKV * CH8; i += NW * 32) {
+        const int t = i / (BKV * CH8), ii = i % (BKV * CH8);
+        const int r = ii >> CH8_LOG2, ch = ii & (CH8 - 1);
+        uint4 lo, hi;
+        c8x16_to_bf16(ld_shared_v4(st + t * BKV * D + r * D + ch * 16), lo, hi);
+        const uint32_t dst = t == 0 ? sK : sV;
+        asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(dst + swz<D>(r, 2 * ch)), "r"(lo.x), "r"(lo.y), "r"(lo.z),
+                     "r"(lo.w) : "memory");
+        asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(dst + swz<D>(r, 2 * ch + 1)), "r"(hi.x), "r"(hi.y), "r"(hi.z),
+                     "r"(hi.w) : "memory");
+      }
+      __syncthreads();
+    }
     if (j == j_lo) {
 #pragma unroll
       for (int kc = 0; kc < D / 16; ++kc) ldsm_x4(sQ + swz<D>(warp * 16 + (lane & 15), kc * 2 + (lane >> 4)), qf[kc]);
@@ -156,7 +216,7 @@ __global__ void __launch_bounds__(NW * 32, 1) fa_fwd_kernel(const Params p) {
     float s[BKV / 8][4];
 #pragma unroll
     for (int i = 0; i < BKV / 8; ++i) s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f;
-    const uint32_t kb = sK + buf * KV_TILE_BYTES, vb = sV + buf * KV_TILE_BYTES;
+    const uint32_t kb = sK + (C8 ? 0 : buf) * KV_TILE_BYTES, vb = sV + (C8 ? 0 : buf) * KV_TILE_BYTES;
 #pragma unroll
     for (int kc = 0; kc < D / 16; ++kc) {
 #pragma unroll
@@ -195,7 +255,7 @@ __global__ void __launch_bounds__(NW * 32, 1) fa_fwd_kernel(const Params p) {
       for (int nt = 0; nt < BKV / 8; ++nt) mx = fmaxf(mx, fmaxf(s[nt][2 * h], s[nt][2 * h + 1]));
       mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
       mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-      const float m_new = fmaxf(m[h], mx * p.scale_log2);
+      const float m_new = fmaxf(m[h], mx * scale_log2);
       const float corr = (m[h] == -INFINITY) ? 0.f : fast_exp2(m[h] - m_new);
       m[h] = m_new;
       // a row can be fully masked in its first tiles (documents): exp2(-inf - (-inf)) must not be evaluated
@@ -203,8 +263,8 @@ __global__ void __launch_bounds__(NW * 32, 1) fa_fwd_kernel(const Params p) {
       float rs = 0.f;
 #pragma unroll
       for (int nt = 0; nt < BKV / 8; ++nt) {
-        const float p0 = fast_exp2(fmaf(s[nt][2 * h], p.scale_log2, neg_m));
-        const float p1 = fast_exp2(fmaf(s[nt][2 * h + 1], p.scale_log2, neg_m));
+        const float p0 = fast_exp2(fmaf(s[nt][2 * h], scale_log2, neg_m));
+        const float p1 = fast_exp2(fmaf(s[nt][2 * h + 1], scale_log2, neg_m));
         rs += p0 + p1;
         pa[nt >> 1][(nt & 1) * 2 + h] = pack_bf16x2(p0, p1);
       }
@@ -233,12 +293,13 @@ __global__ void __launch_bounds__(NW * 32, 1) fa_fwd_kernel(const Params p) {
     lt += __shfl_xor_sync(0xffffffffu, lt, 2);
     const int r = row_a + 8 * h;
     if (r >= n_rows) continue;
-    const float inv = 1.f / lt;
+    float inv = 1.f / lt;
+    if constexpr (C8) inv = __bfloat162float(p.kv8.v_out_scale[kv_head]) / lt;   // V = (u - 128) o_v
     bf16* orow = p.o + static_cast<size_t>(tok0 + r) * p.ldo + head * D;
 #pragma unroll
     for (int dt = 0; dt < D / 8; ++dt)
       *reinterpret_cast<uint32_t*>(orow + dt * 8 + 2 * tq) = pack_bf16x2(o[dt][2 * h] * inv, o[dt][2 * h + 1] * inv);
-    if constexpr (MODE != PAGED) {
+    if constexpr (MODE == DENSE || MODE == MASK) {
       if (tq == 0) p.lse[(static_cast<size_t>(batch) * p.nh + head) * p.S + r] = (m[h] + log2f(lt)) * 0.6931471805599453f;
     }
   }
@@ -246,7 +307,7 @@ __global__ void __launch_bounds__(NW * 32, 1) fa_fwd_kernel(const Params p) {
 
 template <int D, int MODE>
 static int launch(const Params& p, int q_rows, cudaStream_t stream) {
-  constexpr int SMEM = BQ * D * 2 + 4 * BKV * D * 2;
+  constexpr int SMEM = fa_smem_bytes<D, MODE>();
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(fa_fwd_kernel<D, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
@@ -531,7 +592,8 @@ static int launch(const CUtensorMap (&tm)[3], const Params& p, cudaStream_t stre
 // Prefill half of append_attention: causal attention of the NEW token rows of every prompt / prompt-chunk sequence over its paged
 // cache `kv` (cached prefix + the rows themselves, already appended).  qkv: packed projection [token_num, ldq] (q heads first,
 // rotated); out [token_num, ldo].  max_q_len bounds seq_lens_this_time (grid size).  kv.d is 64 or 128 (checked by the caller).
-int launch_fa_prefill_paged(const KvCache& kv, const void* qkv, void* out, const int32_t* cu_seqlens_q,
+template <typename T>
+int launch_fa_prefill_paged(const KvCacheT<T>& kv, const void* qkv, void* out, const int32_t* cu_seqlens_q,
                             const int32_t* seq_lens_encoder, const int32_t* seq_lens_decoder, const int32_t* seq_lens_this_time,
                             int64_t B, int64_t max_q_len, int64_t num_heads, int64_t ldq, int64_t ldo, float softmax_scale,
                             cudaStream_t stream) {
@@ -544,10 +606,20 @@ int launch_fa_prefill_paged(const KvCache& kv, const void* qkv, void* out, const
   p.kvh = kv.kvh;
   p.scale_log2 = softmax_scale * 1.4426950408889634f;
   p.cu_q = cu_seqlens_q; p.seq_dec = seq_lens_decoder; p.seq_this = seq_lens_this_time; p.seq_enc = seq_lens_encoder;
-  p.kv = kv;
-  if (kv.d == 64) return launch<64, PAGED>(p, static_cast<int>(max_q_len), stream);
-  return launch<128, PAGED>(p, static_cast<int>(max_q_len), stream);
+  if constexpr (sizeof(T) == 1) {
+    p.kv8 = kv;
+    if (kv.d == 64) return launch<64, PAGED_C8>(p, static_cast<int>(max_q_len), stream);
+    return launch<128, PAGED_C8>(p, static_cast<int>(max_q_len), stream);
+  } else {
+    p.kv = kv;
+    if (kv.d == 64) return launch<64, PAGED>(p, static_cast<int>(max_q_len), stream);
+    return launch<128, PAGED>(p, static_cast<int>(max_q_len), stream);
+  }
 }
+template int launch_fa_prefill_paged(const KvCache&, const void*, void*, const int32_t*, const int32_t*, const int32_t*,
+                                     const int32_t*, int64_t, int64_t, int64_t, int64_t, int64_t, float, cudaStream_t);
+template int launch_fa_prefill_paged(const KvCacheC8&, const void*, void*, const int32_t*, const int32_t*, const int32_t*,
+                                     const int32_t*, int64_t, int64_t, int64_t, int64_t, int64_t, float, cudaStream_t);
 
 }  // namespace b200
 

@@ -121,9 +121,11 @@ __global__ void __launch_bounds__(128) add_rmsnorm_kernel(const bf16* __restrict
 // ------------------------------------------------------------------------------------------------
 // Prefill: copy the (already rotated) K and the V rows of the packed QKV projection into the dense or paged cache
 // (kv_cache.cuh; reference: write_cache_kv, csrc/gpu/write_cache_kv.cu:23-99; here K keeps the plain [max_len, d] row
-// layout — the transposed x=8 layout there is private to Paddle's MMHA kernel).
+// layout — the transposed x=8 layout there is private to Paddle's MMHA kernel).  Every cache writer stores through
+// KvCacheT::store8, which quantises the same bf16 values into a uint8 cache.
 // ------------------------------------------------------------------------------------------------
-__global__ void write_cache_kv_kernel(const bf16* __restrict__ qkv, const KvCache cv, const int* __restrict__ seq_lens,
+template <typename T>
+__global__ void write_cache_kv_kernel(const bf16* __restrict__ qkv, const KvCacheT<T> cv, const int* __restrict__ seq_lens,
                                       int S, int nh, int64_t ld) {
   const int tok = blockIdx.x;          // b * S + s
   const int b = tok / S, s = tok % S;
@@ -136,7 +138,7 @@ __global__ void write_cache_kv_kernel(const bf16* __restrict__ qkv, const KvCach
     const int cc = c % chunks;
     const int head = (cc * 8) / d, off = (cc * 8) % d;
     const uint4 v = *reinterpret_cast<const uint4*>(qkv + static_cast<size_t>(tok) * ld + (nh + which * kvh) * d + cc * 8);
-    *reinterpret_cast<uint4*>((which != 0 ? cv.v : cv.k) + cv.offset(b, head, s) + off) = v;
+    cv.store8(which, head, cv.offset(b, head, s) + off, v);
   }
 }
 
@@ -161,8 +163,9 @@ __device__ __forceinline__ uint4 take_f32_chunk(float* acc, const float* bias, i
   return make_uint4(pack_bf16x2(a.x, a.y), pack_bf16x2(a.z, a.w), pack_bf16x2(b.x, b.y), pack_bf16x2(b.z, b.w));
 }
 
+template <typename T>
 __global__ void decode_rope_append_kernel(bf16* __restrict__ qkv, float* __restrict__ acc_f32, const float* __restrict__ bias,
-                                          const KvCache cv, const float* __restrict__ cos_t,
+                                          const KvCacheT<T> cv, const float* __restrict__ cos_t,
                                           const float* __restrict__ sin_t, const int* __restrict__ seq_lens, int nh,
                                           int64_t ld) {
   // ONE pass, no block barrier: thread = one (head, 8-column chunk pair) of q / k, or one 8-column chunk of v.  Each thread takes
@@ -198,9 +201,9 @@ __global__ void decode_rope_append_kernel(bf16* __restrict__ qkv, float* __restr
     *reinterpret_cast<uint4*>(base + j8) = a;
     *reinterpret_cast<uint4*>(base + half + j8) = bb;
     if (pos_ok && head >= nh) {   // rotated k -> cache
-      bf16* dst = cv.k + cv.offset(b, head - nh, pos);
-      *reinterpret_cast<uint4*>(dst + j8) = a;
-      *reinterpret_cast<uint4*>(dst + half + j8) = bb;
+      const size_t dst = cv.offset(b, head - nh, pos);
+      cv.store8(0, head - nh, dst + j8, a);
+      cv.store8(0, head - nh, dst + half + j8, bb);
     }
   } else {
     // v -> projection row (fp32 path) and cache (16-byte chunks)
@@ -217,7 +220,7 @@ __global__ void decode_rope_append_kernel(bf16* __restrict__ qkv, float* __restr
     }
     if (pos_ok) {
       const int head = (c * 8) / d, off = (c * 8) % d;
-      *reinterpret_cast<uint4*>(cv.v + cv.offset(b, head, pos) + off) = v;
+      cv.store8(1, head, cv.offset(b, head, pos) + off, v);
     }
   }
 }
@@ -628,7 +631,8 @@ using namespace b200::gen;
 
 static int add_rmsnorm_launch(const void* x, float* x_f32, const void* residual, const void* w, void* normed,
                               void* residual_out, int64_t rows, int64_t h, float eps, cudaStream_t stream);
-static int rope_append_launch(void* qkv, float* acc_f32_ws, const float* bias, const KvCache& cv, const float* cos_table,
+template <typename T>
+static int rope_append_launch(void* qkv, float* acc_f32_ws, const float* bias, const KvCacheT<T>& cv, const float* cos_table,
                               const float* sin_table, const int32_t* seq_lens, int64_t B, int64_t num_heads, int64_t ld,
                               cudaStream_t stream);
 
@@ -691,6 +695,20 @@ extern "C" int b200_write_cache_kv_paged(const void* qkv, void* key_cache, void*
   return check_launch("write_cache_kv_paged");
 }
 
+extern "C" int b200_write_cache_kv_paged_c8(const void* qkv, void* key_cache, void* value_cache, const int32_t* block_tables,
+                                            const void* cache_k_scale, const void* cache_v_scale, const int32_t* seq_lens,
+                                            int64_t B, int64_t S, int64_t num_heads, int64_t num_kv_heads, int64_t head_dim,
+                                            int64_t block_size, int64_t max_blocks_per_seq, int64_t ld, cudaStream_t stream) {
+  KvCacheC8 cv;
+  if (int rc = paged_kv_cache_c8(&cv, key_cache, value_cache, block_tables, cache_k_scale, cache_v_scale, nullptr, nullptr, true,
+                                 false, num_kv_heads, head_dim, block_size, max_blocks_per_seq, "write_cache_kv_paged_c8"))
+    return rc;
+  B200_CHECK_ARG(qkv && ld % 8 == 0 && B > 0 && S > 0 && S <= cv.max_len, "write_cache_kv_paged_c8: bad sizes");
+  write_cache_kv_kernel<<<static_cast<unsigned>(B * S), 128, 0, stream>>>(static_cast<const bf16*>(qkv), cv, seq_lens, (int)S,
+                                                                          (int)num_heads, ld);
+  return check_launch("write_cache_kv_paged_c8");
+}
+
 extern "C" int b200_decode_rope_append_f32(void* qkv, float* acc_f32_ws, const float* bias, void* cache,
                                            const float* cos_table, const float* sin_table, const int32_t* seq_lens,
                                            int64_t B, int64_t num_heads, int64_t num_kv_heads, int64_t head_dim,
@@ -713,14 +731,15 @@ extern "C" int b200_decode_rope_append_f32(void* qkv, float* acc_f32_ws, const f
   return rope_append_launch(qkv, acc_f32_ws, bias, cv, cos_table, sin_table, seq_lens, B, num_heads, ld, stream);
 }
 
-static int rope_append_launch(void* qkv, float* acc_f32_ws, const float* bias, const KvCache& cv, const float* cos_table,
+template <typename T>
+static int rope_append_launch(void* qkv, float* acc_f32_ws, const float* bias, const KvCacheT<T>& cv, const float* cos_table,
                               const float* sin_table, const int32_t* seq_lens, int64_t B, int64_t num_heads, int64_t ld,
                               cudaStream_t stream) {
   B200_CHECK_ARG(cv.d % 16 == 0 && ld % 8 == 0, "decode_rope_append: head_dim %% 16, ld %% 8");
   const int threads_needed = static_cast<int>((num_heads + cv.kvh) * (cv.d / 16) + (cv.kvh * cv.d) / 8);   // rope pairs + v chunks
   B200_CHECK_ARG(threads_needed <= 1024, "decode_rope_append: too many heads");
   const int threads = (threads_needed + 31) / 32 * 32;
-  launch_pdl(decode_rope_append_kernel, dim3(static_cast<unsigned>(B)), dim3(threads), 0, stream, static_cast<bf16*>(qkv),
+  launch_pdl(decode_rope_append_kernel<T>, dim3(static_cast<unsigned>(B)), dim3(threads), 0, stream, static_cast<bf16*>(qkv),
              acc_f32_ws, bias, cv, cos_table, sin_table, seq_lens, (int)num_heads, ld);
   return check_launch("decode_rope_append");
 }
@@ -735,6 +754,20 @@ extern "C" int b200_decode_rope_append_paged(void* qkv, float* acc_f32_ws, const
                               "decode_rope_append_paged"))
     return rc;
   B200_CHECK_ARG(qkv && cos_table && sin_table && seq_lens, "decode_rope_append_paged: null pointer");
+  return rope_append_launch(qkv, acc_f32_ws, bias, cv, cos_table, sin_table, seq_lens, B, num_heads, ld, stream);
+}
+
+extern "C" int b200_decode_rope_append_paged_c8(void* qkv, float* acc_f32_ws, const float* bias, void* key_cache,
+                                                void* value_cache, const int32_t* block_tables, const void* cache_k_scale,
+                                                const void* cache_v_scale, const float* cos_table, const float* sin_table,
+                                                const int32_t* seq_lens, int64_t B, int64_t num_heads, int64_t num_kv_heads,
+                                                int64_t head_dim, int64_t block_size, int64_t max_blocks_per_seq, int64_t ld,
+                                                cudaStream_t stream) {
+  KvCacheC8 cv;
+  if (int rc = paged_kv_cache_c8(&cv, key_cache, value_cache, block_tables, cache_k_scale, cache_v_scale, nullptr, nullptr, true,
+                                 false, num_kv_heads, head_dim, block_size, max_blocks_per_seq, "decode_rope_append_paged_c8"))
+    return rc;
+  B200_CHECK_ARG(qkv && cos_table && sin_table && seq_lens, "decode_rope_append_paged_c8: null pointer");
   return rope_append_launch(qkv, acc_f32_ws, bias, cv, cos_table, sin_table, seq_lens, B, num_heads, ld, stream);
 }
 
@@ -1427,7 +1460,8 @@ extern "C" int b200_save_output_stream(const int64_t* next_tokens, const int32_t
 namespace b200 {
 namespace gen {
 
-__global__ void append_rope_write_kernel(bf16* __restrict__ qkv, const KvCache cv, const float* __restrict__ cos_t,
+template <typename T>
+__global__ void append_rope_write_kernel(bf16* __restrict__ qkv, const KvCacheT<T> cv, const float* __restrict__ cos_t,
                                          const float* __restrict__ sin_t, const int* __restrict__ cu_q,
                                          const int* __restrict__ seq_enc, const int* __restrict__ seq_dec,
                                          const int* __restrict__ seq_this, bf16* __restrict__ q_dec, int* __restrict__ dec_len, int B,
@@ -1468,9 +1502,9 @@ __global__ void append_rope_write_kernel(bf16* __restrict__ qkv, const KvCache c
     *reinterpret_cast<uint4*>(base + j8) = a;
     *reinterpret_cast<uint4*>(base + half + j8) = bb;
     if (head >= nh) {
-      bf16* dst = cv.k + cv.offset(b, head - nh, pos);
-      *reinterpret_cast<uint4*>(dst + j8) = a;
-      *reinterpret_cast<uint4*>(dst + half + j8) = bb;
+      const size_t dst = cv.offset(b, head - nh, pos);
+      cv.store8(0, head - nh, dst + j8, a);
+      cv.store8(0, head - nh, dst + half + j8, bb);
     } else if (is_decode) {
       bf16* dst = q_dec + static_cast<size_t>(b) * ld + head * d;
       *reinterpret_cast<uint4*>(dst + j8) = a;
@@ -1481,7 +1515,7 @@ __global__ void append_rope_write_kernel(bf16* __restrict__ qkv, const KvCache c
     if (c >= (kvh * d) >> 3) return;
     const uint4 v = *reinterpret_cast<const uint4*>(row + (nh + kvh) * d + c * 8);
     const int head = (c * 8) / d, off = (c * 8) % d;
-    *reinterpret_cast<uint4*>(cv.v + cv.offset(b, head, pos) + off) = v;
+    cv.store8(1, head, cv.offset(b, head, pos) + off, v);
   }
 }
 
@@ -1506,21 +1540,15 @@ extern "C" int64_t b200_append_attention_workspace_bytes(int64_t B, int64_t num_
          (num_splits > 1 ? b200_decode_attention_workspace_bytes(B, num_heads, num_splits) : 0);
 }
 
-extern "C" int b200_append_attention(void* qkv, void* key_cache, void* value_cache, const int32_t* seq_lens_encoder,
-                                     const int32_t* seq_lens_decoder, const int32_t* seq_lens_this_time,
-                                     const int32_t* cu_seqlens_q, const int32_t* block_tables, const float* cos_table,
-                                     const float* sin_table, void* out, void* workspace, int64_t B, int64_t token_num,
-                                     int64_t max_q_len, int64_t num_heads, int64_t num_kv_heads, int64_t head_dim,
-                                     int64_t num_blocks, int64_t block_size, int64_t max_blocks_per_seq, int64_t rope_positions,
-                                     int64_t ldq, int64_t ldo, float softmax_scale, int64_t num_splits, cudaStream_t stream) {
+// The steps of append_attention over a checked paged view of either element type.
+template <typename T>
+static int append_attention_run(const KvCacheT<T>& cv, void* qkv, const int32_t* seq_lens_encoder, const int32_t* seq_lens_decoder,
+                                const int32_t* seq_lens_this_time, const int32_t* cu_seqlens_q, const float* cos_table,
+                                const float* sin_table, void* out, void* workspace, int64_t B, int64_t token_num,
+                                int64_t max_q_len, int64_t num_heads, int64_t num_kv_heads, int64_t head_dim, int64_t num_blocks,
+                                int64_t rope_positions, int64_t ldq, int64_t ldo, float softmax_scale, int64_t num_splits,
+                                cudaStream_t stream) {
   using namespace b200;
-  B200_CHECK_ARG(qkv && seq_lens_encoder && seq_lens_decoder && seq_lens_this_time && cu_seqlens_q && cos_table && sin_table && out &&
-                     workspace,
-                 "append_attention: null pointer");
-  KvCache cv;
-  if (int rc = paged_kv_cache(&cv, key_cache, value_cache, block_tables, num_kv_heads, head_dim, block_size, max_blocks_per_seq,
-                              "append_attention"))
-    return rc;
   B200_CHECK_ARG(head_dim == 64 || head_dim == 128, "append_attention: head_dim must be 64 or 128 (got %lld)", (long long)head_dim);
   B200_CHECK_ARG(B > 0 && token_num > 0 && max_q_len > 0 && num_heads % num_kv_heads == 0 && num_blocks > 0 && ldq % 8 == 0 &&
                      ldo % 8 == 0 && num_splits >= 1 && num_splits <= 64,
@@ -1549,4 +1577,45 @@ extern "C" int b200_append_attention(void* qkv, void* key_cache, void* value_cac
   gen::append_scatter_decode_kernel<<<static_cast<unsigned>(B), 128, 0, stream>>>(out_dec, static_cast<bf16*>(out), cu_seqlens_q,
                                                                                  dec_len, (int)(num_heads * head_dim), ldo);
   return check_launch("append_attention(scatter)");
+}
+
+extern "C" int b200_append_attention(void* qkv, void* key_cache, void* value_cache, const int32_t* seq_lens_encoder,
+                                     const int32_t* seq_lens_decoder, const int32_t* seq_lens_this_time,
+                                     const int32_t* cu_seqlens_q, const int32_t* block_tables, const float* cos_table,
+                                     const float* sin_table, void* out, void* workspace, int64_t B, int64_t token_num,
+                                     int64_t max_q_len, int64_t num_heads, int64_t num_kv_heads, int64_t head_dim,
+                                     int64_t num_blocks, int64_t block_size, int64_t max_blocks_per_seq, int64_t rope_positions,
+                                     int64_t ldq, int64_t ldo, float softmax_scale, int64_t num_splits, cudaStream_t stream) {
+  B200_CHECK_ARG(qkv && seq_lens_encoder && seq_lens_decoder && seq_lens_this_time && cu_seqlens_q && cos_table && sin_table && out &&
+                     workspace,
+                 "append_attention: null pointer");
+  KvCache cv;
+  if (int rc = paged_kv_cache(&cv, key_cache, value_cache, block_tables, num_kv_heads, head_dim, block_size, max_blocks_per_seq,
+                              "append_attention"))
+    return rc;
+  return append_attention_run(cv, qkv, seq_lens_encoder, seq_lens_decoder, seq_lens_this_time, cu_seqlens_q, cos_table, sin_table,
+                              out, workspace, B, token_num, max_q_len, num_heads, num_kv_heads, head_dim, num_blocks,
+                              rope_positions, ldq, ldo, softmax_scale, num_splits, stream);
+}
+
+extern "C" int b200_append_attention_c8(void* qkv, void* key_cache, void* value_cache, const void* cache_k_scale,
+                                        const void* cache_v_scale, const void* cache_k_out_scale, const void* cache_v_out_scale,
+                                        const int32_t* seq_lens_encoder, const int32_t* seq_lens_decoder,
+                                        const int32_t* seq_lens_this_time, const int32_t* cu_seqlens_q, const int32_t* block_tables,
+                                        const float* cos_table, const float* sin_table, void* out, void* workspace, int64_t B,
+                                        int64_t token_num, int64_t max_q_len, int64_t num_heads, int64_t num_kv_heads,
+                                        int64_t head_dim, int64_t num_blocks, int64_t block_size, int64_t max_blocks_per_seq,
+                                        int64_t rope_positions, int64_t ldq, int64_t ldo, float softmax_scale, int64_t num_splits,
+                                        cudaStream_t stream) {
+  B200_CHECK_ARG(qkv && seq_lens_encoder && seq_lens_decoder && seq_lens_this_time && cu_seqlens_q && cos_table && sin_table && out &&
+                     workspace,
+                 "append_attention_c8: null pointer");
+  KvCacheC8 cv;
+  if (int rc = paged_kv_cache_c8(&cv, key_cache, value_cache, block_tables, cache_k_scale, cache_v_scale, cache_k_out_scale,
+                                 cache_v_out_scale, true, true, num_kv_heads, head_dim, block_size, max_blocks_per_seq,
+                                 "append_attention_c8"))
+    return rc;
+  return append_attention_run(cv, qkv, seq_lens_encoder, seq_lens_decoder, seq_lens_this_time, cu_seqlens_q, cos_table, sin_table,
+                              out, workspace, B, token_num, max_q_len, num_heads, num_kv_heads, head_dim, num_blocks,
+                              rope_positions, ldq, ldo, softmax_scale, num_splits, stream);
 }

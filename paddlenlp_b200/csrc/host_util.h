@@ -2,6 +2,7 @@
 // through the driver entry point (no link-time dependency on libcuda), device attribute cache.
 #pragma once
 #include <cuda.h>
+#include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdarg.h>
 #include <stdint.h>
@@ -17,16 +18,23 @@ int check_launch(const char* what);  // cudaGetLastError() -> return code
 int sm_count();  // multiprocessors of the current device (cached per device)
 int fa_fwd_impl();         // b200_set_fa_fwd_impl(): 2 = wgmma kernel, 1 = mma.sync kernel (cross-check)
 int fa_bwd_impl();         // b200_set_fa_bwd_impl(): 2 = wgmma kernel, 1 = mma.sync kernel (cross-check)
-// Attention launchers over a KV cache view (kv_cache.cuh); the prefill one serves b200_append_attention
-struct KvCache;
-int launch_fa_prefill_paged(const KvCache& kv, const void* qkv, void* out, const int32_t* cu_seqlens_q,
+// Attention launchers over a KV cache view (kv_cache.cuh: KvCache holds bf16, KvCacheC8 uint8 with per-head scales); the
+// prefill one serves b200_append_attention
+template <typename T>
+struct KvCacheT;
+using KvCache = KvCacheT<__nv_bfloat16>;
+using KvCacheC8 = KvCacheT<uint8_t>;
+template <typename T>
+int launch_fa_prefill_paged(const KvCacheT<T>& kv, const void* qkv, void* out, const int32_t* cu_seqlens_q,
                             const int32_t* seq_lens_encoder, const int32_t* seq_lens_decoder, const int32_t* seq_lens_this_time,
                             int64_t B, int64_t max_q_len, int64_t num_heads, int64_t ldq, int64_t ldo, float softmax_scale,
-                            cudaStream_t stream);   // fa_fwd.cu
+                            cudaStream_t stream);   // fa_fwd.cu, instantiated for both element types
 // decode_attn_tc.cu, dense or paged view: the checks (message names `what`), then the launch of checked arguments
-int check_decode_attention(const char* what, const KvCache& kv, const void* qkv, const int32_t* seq_lens, const void* out,
+template <typename T>
+int check_decode_attention(const char* what, const KvCacheT<T>& kv, const void* qkv, const int32_t* seq_lens, const void* out,
                            const void* workspace, int64_t B, int64_t num_heads, int64_t ld, int64_t num_splits);
-int launch_decode_attention(const KvCache& kv, const void* qkv, const int32_t* seq_lens, void* out, void* workspace, int64_t B,
+template <typename T>
+int launch_decode_attention(const KvCacheT<T>& kv, const void* qkv, const int32_t* seq_lens, void* out, void* workspace, int64_t B,
                             int64_t num_heads, int64_t ld, float softmax_scale, int64_t num_splits, cudaStream_t stream);
 bool pdl_enabled();   // b200_set_pdl(): launch GEMMs with programmatic dependent launch (decode-step kernel chains)
 

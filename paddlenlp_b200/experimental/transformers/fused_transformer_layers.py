@@ -7,7 +7,8 @@ Weight layouts are the reference's (SURVEY.md Appendix B):
     qkv_weight    [(nh + 2*kvh) * d, h]   (transposed, trans_qkvw=True)      -> GEMM with B stored [N, K]
     linear_weight [nh * d, h]             ffn1_weight [h, 2*I] (gate | up)    ffn2_weight [I, h]
     ln_scale / ffn_ln_scale [h]
-KV cache per layer: bf16 [2, B, kvh, max_len, d].
+KV cache per layer: bf16 [2, B, kvh, max_len, d]; paged (FusedBlockMultiTransformer): bf16 pages, or uint8 pages with static
+per-kv-head scales (cachekv_int8_type="static", fused_transformer_layers.py:2389-2395).
 Layer loop (:1126-1174): the output norm of layer i is fused with the residual add and is layer i+1's input norm.
 """
 from __future__ import annotations
@@ -41,6 +42,7 @@ class FusedMultiTransformerConfig:
     trans_qkvw: bool = True
     append_attn: bool = False                # FusedBlockMultiTransformer: route attention through the unified append_attention op
     quant_type: str = ""                     # "" (bf16 layer weights) or "weight_only_int8" (FusedMultiTransformerWeightOnly)
+    cachekv_int8_type: Optional[str] = None  # None (bf16 cache) or "static": uint8 paged cache, per-kv-head scales
 
     def __post_init__(self):
         if self.kv_num_heads <= 0:
@@ -59,10 +61,18 @@ class FusedMultiTransformerConfig:
             if qt == "weight_only_int4" or qt.startswith("a8w8") or "fp8" in qt:
                 raise NotImplementedError(f"quant_type {qt!r} is not implemented (weight_only_int8 is)")
             raise ValueError(f"unknown quant_type {qt!r}")
+        ct = self.cachekv_int8_type
+        if ct == "dynamic":
+            raise NotImplementedError('cachekv_int8_type "dynamic" (per-step scales) is not implemented; "static" is')
+        if ct not in (None, "static"):
+            raise ValueError(f"unknown cachekv_int8_type {ct!r} (None or 'static')")
 
 
 class FusedMultiTransformerBase:
     def __init__(self, config: FusedMultiTransformerConfig, device=None):
+        if config.cachekv_int8_type is not None and not isinstance(self, FusedBlockMultiTransformer):
+            raise NotImplementedError(f"cachekv_int8_type {config.cachekv_int8_type!r} needs the paged cache (block_attn=True); "
+                                      f"the dense cache is bf16 only")
         # every cache path ends in the decode-attention kernels: refuse a head layout they do not cover now, not at the
         # first decode step after a prefill
         nh, kvh = config.num_heads, config.kv_num_heads
@@ -238,6 +248,53 @@ class FusedBlockMultiTransformer(FusedMultiTransformerBase):
     each [max_block_nums, kv_num_heads, block_size, head_dim]; `block_tables` [B, max_blocks_per_seq] int32 (-1 = unused)
     arrives as a keyword argument, as in the reference.  The math is the dense path's: only cache addressing changes."""
 
+    def __init__(self, config: FusedMultiTransformerConfig, device=None):
+        super().__init__(config, device)
+        self.cache_scales_set = False
+        if config.cachekv_int8_type is not None:
+            # the reference's names (fused_transformer_layers.py:2389-2395): quantise scales s and dequantise scales o = 1 / s,
+            # bf16 [kvh] per layer; zero until set_cache_scales()
+            for name in ("cache_k_scales", "cache_v_scales", "cache_k_out_scales", "cache_v_out_scales"):
+                setattr(self, name, [torch.zeros(self.kvh, dtype=BF16, device=self.device) for _ in range(self.L)])
+
+    @torch.no_grad()
+    def set_cache_scales(self, k_absmax, v_absmax):
+        """Static int8-cache scales from the absolute maxima of the cached K and V values, [L, kvh] each: s = 127 / absmax and
+        o = 1 / s in fp64, each cast to bf16 (CacheScaleLoader, experimental/model_utils.py:433-468).  A missing, non-finite or
+        non-positive absmax raises ValueError."""
+        if self.config.cachekv_int8_type is None:
+            raise ValueError("set_cache_scales: the block was built without cachekv_int8_type")
+        for name, a in (("k", k_absmax), ("v", v_absmax)):
+            a = torch.as_tensor(a, dtype=torch.float64).cpu()
+            if tuple(a.shape) != (self.L, self.kvh):
+                raise ValueError(f"set_cache_scales: {name} absmax must be [{self.L}, {self.kvh}], got {tuple(a.shape)}")
+            if not bool(torch.isfinite(a).all()) or not bool((a > 0).all()):
+                bad = [(int(i), int(j)) for i, j in zip(*torch.nonzero(~(torch.isfinite(a) & (a > 0)), as_tuple=True))]
+                raise ValueError(f"set_cache_scales: cache {name} absmax must be finite and positive; (layer, kv head) {bad[:8]}")
+            s = 127.0 / a
+            o = 1.0 / s
+            for i in range(self.L):
+                getattr(self, f"cache_{name}_scales")[i].copy_(s[i].to(BF16))
+                getattr(self, f"cache_{name}_out_scales")[i].copy_(o[i].to(BF16))
+        self.cache_scales_set = True
+
+    def check_cache_scales(self, caches):
+        """Raise unless a uint8 cache has its scales (the reference runs with -1 scales when the file lacks them)."""
+        if caches and caches[0].dtype == ops.CACHE_INT8 and not self.cache_scales_set:
+            raise ValueError("the int8 KV cache has no scales: call set_cache_scales() (the reference's cachekv_scales.json) or "
+                             "calibrate_cache_scales() first")
+
+    # the scale arguments of the paged ops for layer i: none for a bf16 cache (an int8 block calibrates through one)
+    def _write_scales(self, caches, i):
+        if caches[2 * i].dtype != ops.CACHE_INT8:
+            return {}
+        return dict(cache_k_scale=self.cache_k_scales[i], cache_v_scale=self.cache_v_scales[i])
+
+    def _read_scales(self, caches, i):
+        if caches[2 * i].dtype != ops.CACHE_INT8:
+            return {}
+        return dict(cache_k_out_scale=self.cache_k_out_scales[i], cache_v_out_scale=self.cache_v_out_scales[i])
+
     @staticmethod
     def _tables(kw):
         bt = kw.get("block_tables")
@@ -246,15 +303,18 @@ class FusedBlockMultiTransformer(FusedMultiTransformerBase):
         return bt
 
     def _write_cache(self, qkv, caches, i, B, S, seq_lens_encoder, kw):
-        ops.write_cache_kv_paged(qkv, caches[2 * i], caches[2 * i + 1], self._tables(kw), seq_lens_encoder, B, S, self.nh)
+        ops.write_cache_kv_paged(qkv, caches[2 * i], caches[2 * i + 1], self._tables(kw), seq_lens_encoder, B, S, self.nh,
+                                 **self._write_scales(caches, i))
 
     def _rope_append(self, qkv, acc, caches, i, seq_lens_decoder, kw):
         cos, sin = self.rope
         return ops.decode_rope_append_paged(qkv, caches[2 * i], caches[2 * i + 1], self._tables(kw), cos, sin, seq_lens_decoder,
-                                            self.nh, acc_f32=acc, bias=self._bias(i) if acc is not None else None)
+                                            self.nh, acc_f32=acc, bias=self._bias(i) if acc is not None else None,
+                                            **self._write_scales(caches, i))
 
     def _attend(self, qkv, caches, i, seq_lens_decoder, kw):
-        return ops.decode_attention_paged(qkv, caches[2 * i], caches[2 * i + 1], self._tables(kw), seq_lens_decoder, self.nh)
+        return ops.decode_attention_paged(qkv, caches[2 * i], caches[2 * i + 1], self._tables(kw), seq_lens_decoder, self.nh,
+                                          **self._read_scales(caches, i))
 
     # ---- config.append_attn (fused_transformer_layers.py:2215-2262): ONE op does RoPE + cache append + attention for the prompt
     # rows and the decode rows alike; the padded [B, S] prefill layout is the packed layout with cu_seqlens_q[b] = b * S ----
@@ -262,7 +322,7 @@ class FusedBlockMultiTransformer(FusedMultiTransformerBase):
         cos, sin = self.rope
         cu = torch.arange(0, (B + 1) * S, S, dtype=torch.int32, device=qkv.device)
         return ops.append_attention(qkv, caches[2 * i], caches[2 * i + 1], enc, dec, this_time, cu, self._tables(kw), cos, sin,
-                                    self.nh, max_q_len=S)
+                                    self.nh, max_q_len=S, **self._write_scales(caches, i), **self._read_scales(caches, i))
 
     def compute_fmha(self, qkv, caches, i, B, S, seq_lens_encoder, kw):
         packed = kw.get("packed")
@@ -272,7 +332,8 @@ class FusedBlockMultiTransformer(FusedMultiTransformerBase):
             enc, dec, this_time, cu, max_q_len = packed
             cos, sin = self.rope
             return ops.append_attention(qkv, caches[2 * i], caches[2 * i + 1], enc, dec, this_time, cu, self._tables(kw), cos, sin,
-                                        self.nh, max_q_len=max_q_len)
+                                        self.nh, max_q_len=max_q_len, **self._write_scales(caches, i),
+                                        **self._read_scales(caches, i))
         if not self.config.append_attn:
             return super().compute_fmha(qkv, caches, i, B, S, seq_lens_encoder, kw)
         enc = (seq_lens_encoder if seq_lens_encoder is not None

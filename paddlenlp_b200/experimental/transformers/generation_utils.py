@@ -66,6 +66,9 @@ class GenerationInferenceModel:
                else seq_len_encoder.to(dev, torch.int32).reshape(B).contiguous())
         if cache_kvs is None:
             cache_kvs = self.allocate_caches(B, S + max_length)
+        tb = getattr(self, "transformer_block", None)
+        if hasattr(tb, "check_cache_scales"):
+            tb.check_cache_scales(cache_kvs)
         if getattr(self, "block_attn", False):                   # paged cache: capacity = blocks per sequence x block size
             if self.block_tables is None or self.block_tables.shape[0] != B:
                 raise ValueError("block_attn: allocate the caches with allocate_caches(batch, max_len) for this batch size")
@@ -76,7 +79,6 @@ class GenerationInferenceModel:
             raise ValueError(f"cache max_len {max_len} < prompt {S} + max_length {max_length}")
         # the rotary tables must cover every position the decode steps will index (they have max_position_embeddings rows at
         # construction; the KV cache may be longer): grow them now, before any kernel or graph captures their pointers
-        tb = getattr(self, "transformer_block", None)
         if tb is not None and hasattr(tb, "ensure_rope"):
             tb.ensure_rope(S + max_length)
         eos = torch.tensor([eos_token_id] if isinstance(eos_token_id, int) else list(eos_token_id or [-1]),
@@ -234,7 +236,9 @@ class GenerationInferenceModel:
             cursor=i32(1), out_ids=i64(R, max_dec, fill=-1), out_lens=i32(R),
         )
         header = torch.zeros(ops.RA_HEADER_INTS, dtype=torch.int32).pin_memory()
-        caches = [torch.zeros(N, tb.kvh, bs, tb.d, dtype=torch.bfloat16, device=dev) for _ in range(2 * tb.L)]
+        caches = [torch.zeros(N, tb.kvh, bs, tb.d, dtype=getattr(self, "cache_dtype", torch.bfloat16), device=dev)
+                  for _ in range(2 * tb.L)]
+        tb.check_cache_scales(caches)
         eos = torch.tensor([eos_token_id] if isinstance(eos_token_id, int) else list(eos_token_id or [-1]),
                            dtype=torch.int64, device=dev)
         samp = dict(pre_ids=st["pre_ids"], step_idx=st["step_idx"], min_dec_len=st["min_dec_len"], eos=eos,

@@ -3,7 +3,9 @@
 Qwen2 (q/k/v bias) uses the same stack."""
 from __future__ import annotations
 
-from typing import Dict, List
+import json
+import os
+from typing import Dict, List, Optional, Union
 
 import torch
 
@@ -17,14 +19,23 @@ BF16 = torch.bfloat16
 
 class LlamaForCausalLMInferenceModel(GenerationInferenceModel):
     def __init__(self, config, device=None, block_attn: bool = False, block_size: int = 64, append_attn: bool = False,
-                 quant_type=None):
+                 quant_type=None, cachekv_int8_type=None):
         """block_attn=True selects the paged KV cache (`--block_attn` of llm/predict/predictor.py:1507-1520:
         LlamaBlockInferenceModel on FusedBlockMultiTransformer); append_attn=True (`--append_attn`) additionally routes prefill
         and decode attention through the unified append_attention op.  quant_type (`--quant_type`, predictor.py:86,1250; None
         reads config.quant_type, where the predictor puts it): "weight_only_int8" holds the layer matrices as int8 with
-        per-channel scales (FusedMultiTransformerWeightOnly); embeddings, norms and the head stay bf16."""
+        per-channel scales (FusedMultiTransformerWeightOnly); embeddings, norms and the head stay bf16.
+        cachekv_int8_type (`--cachekv_int8_type`, predictor.py:117-122; None reads config.cachekv_int8_type): "static" holds
+        the paged KV cache as uint8 with one static scale per layer and kv head, loaded with set_cache_scales() or measured
+        with calibrate_cache_scales(); it needs block_attn=True and composes with either quant_type."""
         if append_attn and not block_attn:
             raise ValueError("append_attn needs block_attn=True (the op works on the paged cache)")
+        ct = getattr(config, "cachekv_int8_type", None) if cachekv_int8_type is None else cachekv_int8_type
+        if ct is not None and not block_attn:
+            if ct == "dynamic":
+                raise NotImplementedError('cachekv_int8_type "dynamic" is not implemented; "static" is')
+            raise NotImplementedError(f"cachekv_int8_type {ct!r} is implemented for the paged cache only: build the model with "
+                                      f"block_attn=True")
         self.config = config
         self.block_attn = bool(block_attn)
         self.block_size = int(block_size)
@@ -36,13 +47,14 @@ class LlamaForCausalLMInferenceModel(GenerationInferenceModel):
             kv_num_heads=c.num_key_value_heads, num_layers=c.num_hidden_layers, epsilon=c.rms_norm_eps,
             rope_theta=c.rope_theta, max_position_embeddings=max(int(getattr(c, "max_position_embeddings", 4096)), 128),
             qkv_bias=(c.model_type == "qwen2"), append_attn=bool(append_attn),
-            quant_type=(getattr(c, "quant_type", "") if quant_type is None else quant_type) or "")
+            quant_type=(getattr(c, "quant_type", "") if quant_type is None else quant_type) or "", cachekv_int8_type=ct)
         if fcfg.quant_type:
             block = FusedBlockMultiTransformerWeightOnly if self.block_attn else FusedMultiTransformerWeightOnly
         else:
             block = FusedBlockMultiTransformer if self.block_attn else FusedMultiTransformerBase
         self.transformer_block = block(fcfg, device)
         self.device = self.transformer_block.device
+        self.cache_dtype = ops.CACHE_INT8 if ct is not None else BF16
         self.embed_tokens = torch.zeros(c.vocab_size, c.hidden_size, dtype=BF16, device=self.device)
         self.norm_weight = torch.ones(c.hidden_size, dtype=BF16, device=self.device)
         # tied embeddings (llama/modeling.py:1924-1938): the head reads embed_tokens [V, h] as the GEMM's K-major operand
@@ -136,7 +148,60 @@ class LlamaForCausalLMInferenceModel(GenerationInferenceModel):
             for j in range(per_seq):
                 tables[i, j] = free_list.pop()
         self.block_tables = tables.to(self.device)
-        return [torch.zeros(n, t.kvh, bs, t.d, dtype=BF16, device=self.device) for _ in range(2 * t.L)]
+        # zero pages: a uint8 cache byte of 128 reads back as 0 too, but every position a kernel reads has been written first
+        return [torch.zeros(n, t.kvh, bs, t.d, dtype=self.cache_dtype, device=self.device) for _ in range(2 * t.L)]
+
+    # ---- static int8 KV-cache scales (cachekv_int8_type="static") ----
+    def set_cache_scales(self, scales: Union[Dict[str, list], str]):
+        """Load the reference's cachekv_scales.json (a path or its parsed content): keys
+        `<model_type>.layers.<i>.self_attn.cachek_matmul.activation_quanter` and `...cachev_matmul...`, each holding
+        num_attention_heads absmax values.  Under GQA every group-th value is kept (one per kv head), then s = 127 / absmax and
+        o = 1 / s, both cast to bf16, as CacheScaleLoader does (experimental/model_utils.py:433-468).  A missing key or a
+        missing, non-finite or non-positive absmax raises ValueError (the reference fills in -1)."""
+        if isinstance(scales, (str, os.PathLike)):
+            with open(scales) as f:
+                scales = json.load(f)
+        t = self.transformer_block
+        nh = self.config.num_attention_heads
+        group = nh // t.kvh
+        out = {}
+        for kind in ("k", "v"):
+            rows = []
+            for i in range(t.L):
+                key = f"{self.prefix}.layers.{i}.self_attn.cache{kind}_matmul.activation_quanter"
+                if key not in scales:
+                    raise ValueError(f"set_cache_scales: no {key!r}")
+                vals = list(scales[key])
+                if len(vals) != nh:
+                    raise ValueError(f"set_cache_scales: {key!r} holds {len(vals)} values, expected num_attention_heads {nh}")
+                rows.append([float(vals[j]) for j in range(0, nh, group)])
+            out[kind] = torch.tensor(rows, dtype=torch.float64)
+        t.set_cache_scales(out["k"], out["v"])
+
+    @torch.no_grad()
+    def calibrate_cache_scales(self, input_ids: torch.Tensor, seq_len_encoder: Optional[torch.Tensor] = None):
+        """Measure static cache scales on sample prompts: one prefill of input_ids [B, S] (right padded to seq_len_encoder)
+        into a bf16 paged cache, then the absmax of the cached K and V per (layer, kv head).  Positions no prompt reaches stay
+        zero and do not move an absmax.  Returns the (k, v) absmax tensors [L, kvh] after setting the scales from them."""
+        t = self.transformer_block
+        if t.config.cachekv_int8_type is None:
+            raise ValueError("calibrate_cache_scales: the model was built without cachekv_int8_type")
+        B, S = input_ids.shape
+        ids = input_ids.to(self.device, torch.int64).contiguous()
+        enc = (torch.full((B,), S, dtype=torch.int32, device=self.device) if seq_len_encoder is None
+               else seq_len_encoder.to(self.device, torch.int32).reshape(B).contiguous())
+        t.ensure_rope(S)
+        saved_tables, saved_dtype = self.block_tables, self.cache_dtype
+        try:
+            self.cache_dtype = BF16
+            caches = self.allocate_block_caches(B, S)
+            self._prefill(ids, enc, caches)
+        finally:
+            self.block_tables, self.cache_dtype = saved_tables, saved_dtype
+        absmax = [torch.stack([caches[2 * i + w].abs().amax(dim=(0, 2, 3)).double() for i in range(t.L)]).cpu() for w in (0, 1)]
+        del caches
+        t.set_cache_scales(absmax[0], absmax[1])
+        return absmax[0], absmax[1]
 
     def _cache_kw(self):
         return {"block_tables": self.block_tables} if self.block_attn else {}

@@ -673,40 +673,82 @@ def decode_attention(qkv, cache, seq_lens, nh, kvh, d, softmax_scale=None, out=N
 
 
 # ---- paged ("block") KV cache: FusedBlockMultiTransformer / append_attention ----------------------------------------
+# The pages are bf16, or uint8 (cachekv_int8_type="static": include/b200nlp.h gives the formula).  Every paged op dispatches on
+# the cache dtype: a uint8 cache needs the per-kv-head bf16 [kvh] scales as keyword arguments (cache_k_scale / cache_v_scale to
+# write, cache_k_out_scale / cache_v_out_scale to read), and a bf16 cache refuses them.
+CACHE_INT8 = torch.uint8
+
+
 def _paged_geom(key_cache, value_cache, block_tables):
-    _chk(key_cache, "key_cache"); _chk(value_cache, "value_cache"); _chk(block_tables, "block_tables", torch.int32)
+    dt = CACHE_INT8 if key_cache.dtype == CACHE_INT8 else BF16
+    _chk(key_cache, "key_cache", dt); _chk(value_cache, "value_cache", dt); _chk(block_tables, "block_tables", torch.int32)
     assert key_cache.shape == value_cache.shape and key_cache.is_contiguous() and value_cache.is_contiguous()
     assert block_tables.dim() == 2 and block_tables.is_contiguous()
     num_blocks, kvh, block_size, d = key_cache.shape
     return num_blocks, kvh, block_size, d, block_tables.shape[1]
 
 
-def write_cache_kv_paged(qkv, key_cache, value_cache, block_tables, seq_lens, B, S, nh):
+def _cache_scales(key_cache, what, **scales):
+    """The scale arguments of a paged op: None for a bf16 cache (which must get none), the checked bf16 [kvh] tensors (in
+    argument order) for a uint8 cache (which must get all)."""
+    given = {k: v for k, v in scales.items() if v is not None}
+    if key_cache.dtype != CACHE_INT8:
+        if given:
+            raise ValueError(f"{what}: {', '.join(sorted(given))} given for a {key_cache.dtype} cache (scales belong to a uint8 cache)")
+        return None
+    kvh = key_cache.shape[1]
+    out = []
+    for name, t in scales.items():
+        if t is None:
+            raise ValueError(f"{what}: a uint8 cache needs {name}")
+        _chk(t, name)
+        if tuple(t.shape) != (kvh,) or not t.is_contiguous():
+            raise ValueError(f"{what}: {name} must be a contiguous bf16 [{kvh}] tensor, got {tuple(t.shape)}")
+        out.append(t)
+    return out
+
+
+def write_cache_kv_paged(qkv, key_cache, value_cache, block_tables, seq_lens, B, S, nh, *, cache_k_scale=None,
+                         cache_v_scale=None):
     nb, kvh, bs, d, mb = _paged_geom(key_cache, value_cache, block_tables)
+    sc = _cache_scales(key_cache, "write_cache_kv_paged", cache_k_scale=cache_k_scale, cache_v_scale=cache_v_scale)
+    if sc is not None:
+        call("b200_write_cache_kv_paged_c8", ptr(qkv), ptr(key_cache), ptr(value_cache), ptr(block_tables), ptr(sc[0]), ptr(sc[1]),
+             ptr(seq_lens), B, S, nh, kvh, d, bs, mb, qkv.stride(0), stream_ptr())
+        return
     call("b200_write_cache_kv_paged", ptr(qkv), ptr(key_cache), ptr(value_cache), ptr(block_tables), ptr(seq_lens), B, S, nh, kvh,
          d, bs, mb, qkv.stride(0), stream_ptr())
 
 
-def decode_rope_append_paged(qkv, key_cache, value_cache, block_tables, cos, sin, seq_lens, nh, acc_f32=None, bias=None):
+def decode_rope_append_paged(qkv, key_cache, value_cache, block_tables, cos, sin, seq_lens, nh, acc_f32=None, bias=None, *,
+                             cache_k_scale=None, cache_v_scale=None):
     """RoPE on the new token's q, k + append k, v at position seq_lens[b] of sequence b's block list.  With acc_f32 the packed
     projection arrives as the fp32 split-K workspace (rounded here, workspace re-zeroed) and `qkv` is created."""
     nb, kvh, bs, d, mb = _paged_geom(key_cache, value_cache, block_tables)
+    sc = _cache_scales(key_cache, "decode_rope_append_paged", cache_k_scale=cache_k_scale, cache_v_scale=cache_v_scale)
     if acc_f32 is not None:
         B = acc_f32.shape[0]
         qkv = torch.empty(B, (nh + 2 * kvh) * d, dtype=BF16, device=acc_f32.device)
     B = qkv.shape[0]
+    if sc is not None:
+        call("b200_decode_rope_append_paged_c8", ptr(qkv), ptr(acc_f32), ptr(bias), ptr(key_cache), ptr(value_cache),
+             ptr(block_tables), ptr(sc[0]), ptr(sc[1]), ptr(cos), ptr(sin), ptr(seq_lens), B, nh, kvh, d, bs, mb, qkv.stride(0),
+             stream_ptr())
+        return qkv
     call("b200_decode_rope_append_paged", ptr(qkv), ptr(acc_f32), ptr(bias), ptr(key_cache), ptr(value_cache), ptr(block_tables),
          ptr(cos), ptr(sin), ptr(seq_lens), B, nh, kvh, d, bs, mb, qkv.stride(0), stream_ptr())
     return qkv
 
 
 def decode_attention_paged(qkv, key_cache, value_cache, block_tables, seq_lens, nh, softmax_scale=None, out=None,
-                           num_splits: int = 0):
+                           num_splits: int = 0, *, cache_k_out_scale=None, cache_v_out_scale=None):
     """decode_attention over the paged cache: sequence b's row t lives in page block_tables[b, t // block_size] (entries
     past a sequence's pages may be -1); it attends to min(seq_lens[b] + 1, max_blocks_per_seq * block_size) rows.
     d = 64 or 128, block_size 32, 64 or 128."""
     _chk(qkv, "qkv"); _chk(seq_lens, "seq_lens", torch.int32)
     nb, kvh, bs, d, mb = _paged_geom(key_cache, value_cache, block_tables)
+    sc = _cache_scales(key_cache, "decode_attention_paged", cache_k_out_scale=cache_k_out_scale,
+                       cache_v_out_scale=cache_v_out_scale)
     B = qkv.shape[0]
     if out is None:
         out = torch.empty(B, nh * d, dtype=BF16, device=qkv.device)
@@ -717,6 +759,11 @@ def decode_attention_paged(qkv, key_cache, value_cache, block_tables, seq_lens, 
     ws = None
     if num_splits > 1:
         ws = _workspace(_lib.load().b200_decode_attention_workspace_bytes(B, nh, num_splits), qkv.device, "decode_attn")
+    if sc is not None:
+        call("b200_decode_attention_paged_c8", ptr(qkv), ptr(key_cache), ptr(value_cache), ptr(block_tables), ptr(sc[0]),
+             ptr(sc[1]), ptr(seq_lens), ptr(out), ptr(ws), B, nh, kvh, d, nb, bs, mb, qkv.stride(0), float(softmax_scale), num_splits,
+             stream_ptr())
+        return out
     call("b200_decode_attention_paged", ptr(qkv), ptr(key_cache), ptr(value_cache), ptr(block_tables), ptr(seq_lens), ptr(out),
          ptr(ws), B, nh, kvh, d, nb, bs, mb, qkv.stride(0), float(softmax_scale), num_splits, stream_ptr())
     return out
@@ -739,7 +786,8 @@ def fused_get_rotary_embedding(input_ids, position_ids, head_dim_shape_tensor, p
 
 
 def append_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_decoder, seq_lens_this_time, cu_seqlens_q,
-                     block_tables, cos, sin, nh: int, max_q_len: int, softmax_scale=None, out=None, num_splits: int = 0):
+                     block_tables, cos, sin, nh: int, max_q_len: int, softmax_scale=None, out=None, num_splits: int = 0, *,
+                     cache_k_scale=None, cache_v_scale=None, cache_k_out_scale=None, cache_v_out_scale=None):
     """append_attention of the reference (csrc/gpu/append_attention.cu:428-851) for a mixed batch over the paged cache: RoPE +
     cache append for every new token row of the packed projection qkv [token_num, (nh + 2 kvh) d] (modified in place), then
     attention of every row over its sequence's pages — prompts / prompt chunks and decode rows in one call.
@@ -750,6 +798,8 @@ def append_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_dec
         _chk(t, name, torch.int32)
         assert t.is_contiguous()
     nb, kvh, bs, d, mb = _paged_geom(key_cache, value_cache, block_tables)
+    sc = _cache_scales(key_cache, "append_attention", cache_k_scale=cache_k_scale, cache_v_scale=cache_v_scale,
+                       cache_k_out_scale=cache_k_out_scale, cache_v_out_scale=cache_v_out_scale)
     token_num, ld = qkv.shape
     B = seq_lens_this_time.numel()
     assert qkv.stride(1) == 1 and ld == (nh + 2 * kvh) * d and block_tables.shape[0] == B and cu_seqlens_q.numel() >= B
@@ -760,6 +810,12 @@ def append_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_dec
     if num_splits <= 0:
         num_splits = _decode_splits(B, kvh, mb * bs)
     ws = _workspace(_lib.load().b200_append_attention_workspace_bytes(B, nh, kvh, d, num_splits), qkv.device, "append_attn")
+    if sc is not None:
+        call("b200_append_attention_c8", ptr(qkv), ptr(key_cache), ptr(value_cache), *[ptr(t) for t in sc], ptr(seq_lens_encoder),
+             ptr(seq_lens_decoder), ptr(seq_lens_this_time), ptr(cu_seqlens_q), ptr(block_tables), ptr(cos), ptr(sin), ptr(out),
+             ptr(ws), B, token_num, int(max_q_len), nh, kvh, d, nb, bs, mb, cos.shape[0], qkv.stride(0), out.stride(0),
+             float(softmax_scale), num_splits, stream_ptr())
+        return out
     call("b200_append_attention", ptr(qkv), ptr(key_cache), ptr(value_cache), ptr(seq_lens_encoder), ptr(seq_lens_decoder),
          ptr(seq_lens_this_time), ptr(cu_seqlens_q), ptr(block_tables), ptr(cos), ptr(sin), ptr(out), ptr(ws), B, token_num,
          int(max_q_len), nh, kvh, d, nb, bs, mb, cos.shape[0], qkv.stride(0), out.stride(0), float(softmax_scale), num_splits,

@@ -20,22 +20,28 @@ from paddlenlp_b200.experimental.transformers import LlamaForCausalLMInferenceMo
 PRESETS = {"llama3_8b": T.LlamaConfig.llama3_8b, "llama3_2_1b": T.LlamaConfig.llama3_2_1b, "qwen2_0_5b": T.Qwen2Config.qwen2_0_5b}
 
 
-def run(batch=64, prompt=128, gen=1920, layers=0, graph=True, pdl=True, block_attn=False, preset="llama3_8b", quant_type=""):
+def run(batch=64, prompt=128, gen=1920, layers=0, graph=True, pdl=True, block_attn=False, preset="llama3_8b", quant_type="",
+        cachekv_int8=False):
     class A:
         pass
     a = A()
     a.batch, a.prompt, a.gen, a.layers, a.no_graph, a.no_pdl, a.block_attn = batch, prompt, gen, layers, not graph, not pdl, block_attn
-    a.preset, a.quant_type = preset, quant_type
+    a.preset, a.quant_type, a.cachekv_int8 = preset, quant_type, cachekv_int8
     return _run(a)
 
 
 def _run(a):
     make = PRESETS[a.preset]
     cfg = make(num_hidden_layers=a.layers) if a.layers else make()
-    m = LlamaForCausalLMInferenceModel(cfg, block_attn=a.block_attn, quant_type=a.quant_type)
+    if a.cachekv_int8 and not a.block_attn:
+        raise SystemExit("--cachekv-int8 needs --block-attn (the int8 cache is paged)")
+    m = LlamaForCausalLMInferenceModel(cfg, block_attn=a.block_attn, quant_type=a.quant_type,
+                                       cachekv_int8_type="static" if a.cachekv_int8 else None)
     m.init_random(seed=42)
     g = torch.Generator().manual_seed(1234)
     ids = torch.randint(0, cfg.vocab_size, (a.batch, a.prompt), generator=g).cuda()
+    if a.cachekv_int8:
+        m.calibrate_cache_scales(ids)                      # static scales from the benchmark's own prompts
     max_len = a.prompt + a.gen
     caches = m.allocate_caches(a.batch, max_len)
     # warm-up (kernel attributes, allocator)
@@ -63,7 +69,7 @@ def _run(a):
     layer_params = L * (h * (h + 2 * kvd) + h * h + 3 * h * I)
     # int8 layer weights: one byte each plus a bf16 scale per output channel; embeddings and head stay bf16
     w_bytes = (layer_params + L * (h + 2 * kvd + h + 2 * I + h) * 2 if a.quant_type else layer_params * 2) + V * h * 2
-    kv_per_tok = 2 * L * a.batch * kvd * 2
+    kv_per_tok = 2 * L * a.batch * kvd * (1 if a.cachekv_int8 else 2)
     mean_t = a.prompt + steps / 2.0
     bytes_per_step = w_bytes + kv_per_tok * mean_t
     # H100 SXM data-sheet HBM3 bandwidth unless a measured peak is supplied next to the repository
@@ -74,6 +80,7 @@ def _run(a):
                         "(BASELINE.json configs[4])" if (a.batch, a.prompt, a.gen, a.layers, a.preset) == (64, 128, 1920, 0, "llama3_8b")
                else f"{a.preset} decode, batch {a.batch}, prompt {a.prompt} -> +{a.gen}",
                batch=a.batch, prompt=a.prompt, gen=a.gen, layers=L, paged_kv=bool(a.block_attn), quant_type=a.quant_type,
+               cachekv_int8_type="static" if a.cachekv_int8 else None,
                prefill_ms=prefill_ms, decode_ms=decode_ms,
                ms_per_step=ms_step,
                decode_tokens_per_s=a.batch * steps / (decode_ms / 1e3), bytes_per_step_gb=bytes_per_step / 1e9,
@@ -95,6 +102,8 @@ def main():
     ap.add_argument("--block-attn", action="store_true", help="paged KV cache (FusedBlockMultiTransformer, 64-row blocks)")
     ap.add_argument("--quant-type", default="", choices=["", "weight_only_int8"],
                     help="weight_only_int8: int8 layer weights with per-channel scales (FusedMultiTransformerWeightOnly)")
+    ap.add_argument("--cachekv-int8", action="store_true",
+                    help="uint8 paged KV cache with static per-head scales calibrated on the benchmark's prompts (needs --block-attn)")
     a = ap.parse_args()
     print(json.dumps(_run(a)), flush=True)
 

@@ -92,18 +92,29 @@ def main():
     ap.add_argument("--seed", type=int, default=1234)
     ap.add_argument("--rounds", type=int, default=2, help="rounds of all modes, alternating")
     ap.add_argument("--quant-type", default="", choices=["", "weight_only_int8"], help="int8 layer weights (weight-only)")
+    ap.add_argument("--cachekv-int8", action="store_true",
+                    help="uint8 paged KV cache (static scales calibrated on the first requests' prompts), in the bf16 runs' "
+                         "cache bytes: twice the pages")
     a = ap.parse_args()
     if a.requests % STATIC_BATCH:
         raise SystemExit(f"--requests must be a multiple of {STATIC_BATCH}")
     make = gen_bench.PRESETS[a.preset]
     cfg = make(num_hidden_layers=a.layers) if a.layers else make()
-    m = LlamaForCausalLMInferenceModel(cfg, block_attn=True, append_attn=True, block_size=64, quant_type=a.quant_type)
+    m = LlamaForCausalLMInferenceModel(cfg, block_attn=True, append_attn=True, block_size=64, quant_type=a.quant_type,
+                                       cachekv_int8_type="static" if a.cachekv_int8 else None)
     m.init_random(seed=42)
     reqs = make_requests(a.requests, cfg.vocab_size, a.seed, a.prompt, a.out)
     max_prompt, max_out = a.prompt[1], a.out[1]
     useful = sum(n for _, n in reqs)
-    # the same cache bytes for every mode: the static batch's pages
-    num_blocks = STATIC_BATCH * math.ceil((max_prompt + max_out) / m.block_size)
+    if a.cachekv_int8:
+        calib = reqs[:16]
+        S = max(p.numel() for p, _ in calib)
+        ids = torch.zeros(len(calib), S, dtype=torch.int64)
+        for b, (p, _) in enumerate(calib):
+            ids[b, :p.numel()] = p
+        m.calibrate_cache_scales(ids, torch.tensor([p.numel() for p, _ in calib], dtype=torch.int32))
+    # the same cache bytes for every mode: the static batch's bf16 pages (twice as many uint8 pages)
+    num_blocks = STATIC_BATCH * math.ceil((max_prompt + max_out) / m.block_size) * (2 if a.cachekv_int8 else 1)
     # warm-up: module loads and allocator pools of both paths
     warm = make_requests(8, cfg.vocab_size, 1, (16, 64), (8, 32))
     m.continuous_generate(warm, max_batch_size=4, num_blocks=64)
@@ -118,8 +129,8 @@ def main():
     del m
     torch.cuda.empty_cache()
     ref = gen_bench.run(batch=STATIC_BATCH, prompt=128, gen=256, block_attn=True, preset=a.preset, layers=a.layers,
-                        quant_type=a.quant_type)
-    print(json.dumps(dict(preset=a.preset, quant_type=a.quant_type, requests=a.requests, prompt=a.prompt, out=a.out, useful_tokens=useful, **card(),
+                        quant_type=a.quant_type, cachekv_int8=a.cachekv_int8)
+    print(json.dumps(dict(preset=a.preset, quant_type=a.quant_type, cachekv_int8=a.cachekv_int8, requests=a.requests, prompt=a.prompt, out=a.out, useful_tokens=useful, **card(),
                           runs=runs, gen_bench_block_attn=dict(batch=STATIC_BATCH, ms_per_step=ref["ms_per_step"])),
                      indent=1), flush=True)
 
