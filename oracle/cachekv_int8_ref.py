@@ -31,6 +31,12 @@ def dequantize(u: torch.Tensor, o) -> torch.Tensor:
     return (u.to(torch.float64) - 128.0) * torch.as_tensor(o, dtype=BF16).double()
 
 
+def fake_quant(x: torch.Tensor, s, o) -> torch.Tensor:
+    """dequantize(quantize(x, s), o) in x's float dtype: the value a kernel reads back for the bf16 value x it cached.  (u - 128) o
+    is an integer of at most 8 bits times a bf16 scale, exact in fp32."""
+    return dequantize(quantize(x, s), o).to(x.dtype)
+
+
 def scales_from_absmax(absmax):
     """absmax [..., kvh] -> (s, o) bf16: s = 127 / absmax and o = 1 / s in fp64, each cast to bf16."""
     a = torch.as_tensor(absmax, dtype=torch.float64)

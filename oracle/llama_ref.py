@@ -222,8 +222,29 @@ def swiglu(g: torch.Tensor, u: torch.Tensor, mode: str) -> torch.Tensor:
     return rnd(torch.nn.functional.silu(g) * u, mode)   # fused swiglu op: fp32 math, one rounding (a6)
 
 
+@dataclass
+class KvQuant:
+    """A static int8 KV cache for the reference forward (oracle/cachekv_int8_ref.py).
+
+    scales      per layer (s_k, o_k, s_v, o_v), bf16 [kvh] each: quantise and dequantise scales
+    quant_from  [b] positions: query rows at positions >= quant_from[b] attend over fake-quantised post-RoPE K and V (what
+                the cache holds), earlier rows over the unquantised values.  0 restates append_attention, which attends over
+                the cache for every row; the prompt length restates the fused path, whose prefill attends over the
+                projection's bf16 K / V and whose decode rows read the cache."""
+    scales: list
+    quant_from: torch.Tensor
+
+
+def fake_quant_rows(x: torch.Tensor, s, o) -> torch.Tensor:
+    """x [b, s, kvh, d], s / o bf16 [kvh] -> the values the int8 cache holds for x, dequantised."""
+    from oracle import cachekv_int8_ref as C
+
+    return C.fake_quant(x, s.to(x.device).view(-1, 1), o.to(x.device).view(-1, 1))
+
+
 def decoder_layer(x: torch.Tensor, w: Dict[str, torch.Tensor], p: str, cfg: RefConfig, cos, sin, mode: str,
-                  position_ids=None, capture: Optional[dict] = None, mask_start=None) -> torch.Tensor:
+                  position_ids=None, capture: Optional[dict] = None, mask_start=None, kv_quant: Optional[KvQuant] = None,
+                  layer: int = 0) -> torch.Tensor:
     b, s, h = x.shape
     nh, kvh, d = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
     n1 = rms_norm(x, w[p + "input_layernorm.weight"], cfg.rms_norm_eps, mode)
@@ -232,7 +253,15 @@ def decoder_layer(x: torch.Tensor, w: Dict[str, torch.Tensor], p: str, cfg: RefC
     v = linear(n1, w[p + "self_attn.v_proj.weight"], w.get(p + "self_attn.v_proj.bias"), mode).reshape(b, s, kvh, d)
     q = apply_rope(q, cos, sin, mode, position_ids)
     k = apply_rope(k, cos, sin, mode, position_ids)
-    a = attention(q, k, v, mode, mask_start=mask_start)
+    if kv_quant is None:
+        a = attention(q, k, v, mode, mask_start=mask_start)
+    else:
+        s_k, o_k, s_v, o_v = kv_quant.scales[layer]
+        pos = (torch.arange(s, device=x.device).expand(b, s) if position_ids is None else position_ids.to(x.device))
+        quant = pos >= kv_quant.quant_from.to(x.device).view(-1, 1)
+        a = attention(q, fake_quant_rows(k, s_k, o_k), fake_quant_rows(v, s_v, o_v), mode, mask_start=mask_start)
+        if not bool(quant.all()):
+            a = torch.where(quant[:, :, None], a, attention(q, k, v, mode, mask_start=mask_start))
     o = linear(a, w[p + "self_attn.o_proj.weight"], None, mode)
     x1 = rnd(x + o, mode)
     n2 = rms_norm(x1, w[p + "post_attention_layernorm.weight"], cfg.rms_norm_eps, mode)
@@ -247,14 +276,15 @@ def decoder_layer(x: torch.Tensor, w: Dict[str, torch.Tensor], p: str, cfg: RefC
 
 
 def model_forward(input_ids: torch.Tensor, w: Dict[str, torch.Tensor], cfg: RefConfig, mode: str = "bf16",
-                  position_ids=None, return_hidden: bool = False):
-    """input_ids [b, s] int64 -> logits [b, s, V] (fp32 tensor holding bf16-rounded values in mode 'bf16')."""
+                  position_ids=None, return_hidden: bool = False, kv_quant: Optional[KvQuant] = None):
+    """input_ids [b, s] int64 -> logits [b, s, V] (fp32 tensor holding bf16-rounded values in mode 'bf16').  kv_quant: attend
+    over a static int8 KV cache (KvQuant); None is the plain forward."""
     pre = cfg.model_type
     x = w[f"{pre}.embed_tokens.weight"][input_ids]
     cos, sin = rope_tables(cfg.head_dim, max(input_ids.shape[1], int(position_ids.max()) + 1 if position_ids is not None else 0),
                            cfg.rope_theta, x.device, scaling=cfg.rope_scaling, max_position_embeddings=cfg.max_position_embeddings)
     for i in range(cfg.num_hidden_layers):
-        x = decoder_layer(x, w, f"{pre}.layers.{i}.", cfg, cos, sin, mode, position_ids)
+        x = decoder_layer(x, w, f"{pre}.layers.{i}.", cfg, cos, sin, mode, position_ids, kv_quant=kv_quant, layer=i)
     hf = rms_norm(x, w[f"{pre}.norm.weight"], cfg.rms_norm_eps, mode)
     logits = linear(hf, w["lm_head.weight"], None, mode)
     if return_hidden:

@@ -128,6 +128,25 @@ ROWS = (1, 5, 64, 128, 300, 4096)
 @pytest.mark.parametrize("name", ["qkv", "qkv_bias", "linear", "ffn1", "ffn2"])
 @pytest.mark.parametrize("preset", list(PRESETS))
 def test_gemm_against_fp64(preset, name):
+    _gemm_rows_against_fp64(preset, name, ROWS)
+
+
+# pick_nt() in weight_only.cu takes token tiles of 8, 16, 32, 64 and 128 rows: every row count through 40 (each 8-, 16- and
+# 32-row instantiation, full and partial), the partial 64- and 128-row tiles on both sides of their edges, and the first
+# two-tile counts above 128 and 256.  Continuous batching feeds the GEMM every row count up to max_batch_size.
+TILE_ROWS = tuple(range(1, 41)) + (63, 64, 65, 96, 127, 128, 129, 255, 256, 257)
+
+
+@pytest.mark.parametrize("preset,name", [("llama3-8b", "ffn2"), ("qwen2-0.5b", "ffn2"), ("qwen2-0.5b", "qkv_bias")])
+def test_gemm_every_token_tile(preset, name):
+    """Llama-3-8B ffn2 has the longest K (14 336), Qwen2-0.5B ffn2 the narrowest N (896); its qkv carries a bias."""
+    _gemm_rows_against_fp64(preset, name, TILE_ROWS)
+
+
+def _gemm_rows_against_fp64(preset, name, rows):
+    """Both forms at each row count, splits 0, 1 and 64 where K may split, against fp64: the bf16 form into a NaN-filled
+    output whose 8 padding columns stay NaN, the fp32 form into a zero workspace whose spare bytes stay zero, and the split-K
+    workspace zero after every bf16 call that may split."""
     o = _ops()
     mat = "qkv" if name == "qkv_bias" else name
     w, q, s, q_ref, s_ref, _ = _quantized(preset, mat)
@@ -135,7 +154,7 @@ def test_gemm_against_fp64(preset, name):
     q_ref = q_ref.to(DEV)
     g = _gen(_seed(preset, name, "x"))
     bias = (0.5 * torch.randn(N, generator=g, device=DEV)) if name == "qkv_bias" else None
-    for M in ROWS:
+    for M in rows:
         x = torch.randn(M, K, generator=g, device=DEV).to(BF16)
         ref, mag = _gemm_ref(x, q_ref, s_ref, bias)
         splits = (0, 1, 64) if M <= o.SKINNY_M else (0,)
@@ -274,12 +293,24 @@ W8_LAYER_WIDTHS = ("llama3-8b", "qwen2-1.5b")
 def test_fused_w8_decode_step_equals_unfused(preset, paged, pdl, monkeypatch):
     """split_k = 1: the fused int8 decode step (fp32 workspaces into rope-append, add_rmsnorm and swiglu_fwd_f32) equals
     weight_only_linear -> decode_rope_append -> decode_attention -> ... bit for bit: hidden states and caches."""
+    _fused_w8_vs_unfused(preset, paged, pdl, 64, monkeypatch)
+
+
+@pytest.mark.parametrize("B", [13, 29])
+@pytest.mark.parametrize("paged", [False, True])
+@pytest.mark.parametrize("preset", W8_LAYER_WIDTHS)
+def test_fused_w8_decode_step_equals_unfused_16_and_32_row_tiles(preset, paged, B, monkeypatch):
+    """The same at batch 13 and 29, which the W8 GEMM runs in 16- and 32-row token tiles."""
+    _fused_w8_vs_unfused(preset, paged, True, B, monkeypatch)
+
+
+def _fused_w8_vs_unfused(preset, paged, pdl, B, monkeypatch):
     from paddlenlp_b200.experimental.transformers import LlamaForCausalLMInferenceModel
 
     o = _ops()
     monkeypatch.setattr(o, "weight_only_linear_f32", functools.partial(o.weight_only_linear_f32, split_k=1))
     monkeypatch.setattr(o, "weight_only_linear", functools.partial(o.weight_only_linear, split_k=1))
-    B, max_len = 64, 256
+    max_len = 256
     m = LlamaForCausalLMInferenceModel(_config(preset, max_len), block_attn=paged, quant_type="weight_only_int8")
     m.init_random(7 + paged)
     t = m.transformer_block
@@ -301,7 +332,7 @@ def test_fused_w8_decode_step_equals_unfused(preset, paged, pdl, monkeypatch):
         monkeypatch.setattr(t, "SKINNY_M", 0)
         h_unf = t(src, unf_c, B=B, S=1, seq_lens_decoder=lens, time_step=0, **kw)
         torch.cuda.synchronize()
-    what = f"{preset} {'paged' if paged else 'dense'} pdl={pdl}"
+    what = f"{preset} {'paged' if paged else 'dense'} pdl={pdl} B={B}"
     assert bool(torch.isfinite(h_unf.float()).all())
     assert_same_bits(h_fused, h_unf, f"{what}: hidden states")
     for j, (a, b) in enumerate(zip(fused_c, unf_c)):
