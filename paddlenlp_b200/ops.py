@@ -446,6 +446,23 @@ def _tok_stride(t: torch.Tensor, heads: int, d: int) -> int:
     return ld
 
 
+def check_mask_form(mask_start: torch.Tensor) -> None:
+    """Raise ValueError unless FlashMask start rows [B, S] (or [B, 1, S]) have the form the attention kernels assume.
+
+    The kernels skip kv tiles (forward: the leading tiles; backward: the q tiles past a kv tile's last column) and decide
+    whether a tile needs the mask from one column of it, which is exact only if the canonical start rows (every column
+    visible at least to its own row: max(start, c + 1)) are non-decreasing along the sequence, i.e. contiguous packed
+    documents.  Any other layout would give wrong values silently.  Raw collator rows (right padding 0) are accepted.
+    Check host tensors before they are copied: on a device tensor this synchronises."""
+    ms = mask_start.reshape(-1, mask_start.shape[-1])
+    S = ms.shape[-1]
+    own = torch.arange(1, S + 1, dtype=ms.dtype, device=ms.device)
+    canon = torch.maximum(ms, own)
+    if S > 1 and bool((canon[:, 1:] < canon[:, :-1]).any()):
+        raise ValueError("attn_mask_startend_row_indices must be non-decreasing along the sequence (packed contiguous "
+                         "samples, each column -> end of its sample); general FlashMask patterns are not implemented")
+
+
 def _mask_rows(mask_start, B, S):
     if mask_start is None:
         return None

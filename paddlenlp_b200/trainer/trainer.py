@@ -29,6 +29,7 @@ import numpy as np
 import torch
 
 from .. import distributed as dist_env
+from .. import ops
 from ..optimizer import AdamW, ClipGradByGlobalNorm, get_scheduler
 from ..utils.batch_sampler import DistributedBatchSampler
 from .trainer_utils import EvalLoopOutput, EvalPrediction, IntervalStrategy, PredictionOutput
@@ -320,6 +321,9 @@ class Trainer:
     def _prepare_inputs(self, inputs: Dict[str, Any]) -> Dict[str, Any]:
         """Pinned host -> device (trainer.py:2099-2114)."""
         dev = self._engine().device
+        ms = inputs.get("attn_mask_startend_row_indices")
+        if isinstance(ms, torch.Tensor) and not ms.is_cuda:
+            ops.check_mask_form(ms)             # every batch, before the copy: a host check adds no device sync to the step
         out = {}
         for k, v in inputs.items():
             if isinstance(v, torch.Tensor):

@@ -330,16 +330,15 @@ class DecoderEngine:
         document — same result for every real token, finite values on the (label -100) padding rows."""
         if attn_mask_startend_row_indices is None:
             return None
+        if not attn_mask_startend_row_indices.is_cuda:
+            ops.check_mask_form(attn_mask_startend_row_indices.reshape(B, S))   # every batch, on the host: no device sync
         ms = attn_mask_startend_row_indices.to(device=self.device, dtype=torch.int32, non_blocking=True).reshape(B, S)
         own = torch.arange(1, S + 1, dtype=torch.int32, device=self.device)
         ms = torch.maximum(ms, own[None, :]).contiguous()
         if not getattr(self, "_mask_form_checked", False):
-            # one-time (first batch) check of the form the kernels rely on for tile skipping: non-decreasing start rows, i.e.
-            # contiguous packed documents.  Costs one host sync, once per engine.
+            # start rows that arrive on the device are checked on the first batch only: costs one host sync, once per engine
             self._mask_form_checked = True
-            if S > 1 and bool((ms[:, 1:] < ms[:, :-1]).any()):
-                raise ValueError("attn_mask_startend_row_indices must be non-decreasing along the sequence (packed contiguous "
-                                 "samples, each column -> end of its sample); general FlashMask patterns are not implemented")
+            ops.check_mask_form(ms)
         return ms
 
     def hidden_states(self, input_ids, position_ids=None, save: Optional[list] = None, attn_mask_startend_row_indices=None):

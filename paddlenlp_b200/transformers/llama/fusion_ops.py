@@ -158,6 +158,7 @@ def fusion_flash_attention(query_states, config, key_states, value_states, atten
     if attn_mask_startend_row_indices is not None:
         # fusion_ops.py:218-231: F.flashmask_attention(..., startend_row_indices=idx.unsqueeze(-1), causal=True); idx is
         # [b, s] or [b, 1, s].  Canonical form for the kernels: every column visible at least to its own row.
+        ops.check_mask_form(attn_mask_startend_row_indices.reshape(bsz, q_len))
         idx = attn_mask_startend_row_indices.reshape(bsz, q_len).to(device=query_states.device, dtype=torch.int32)
         own = torch.arange(1, q_len + 1, dtype=torch.int32, device=idx.device)
         mask_rows = torch.maximum(idx, own[None, :]).contiguous()
