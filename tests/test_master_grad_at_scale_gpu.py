@@ -25,7 +25,7 @@ import pytest
 import torch
 
 from oracle import optim_ref
-from test_kernels_at_scale_gpu import (HEAD_DIM, MODELS, ROW_TOL, _rows_with_spread, _tile_sums, assert_rows_close,  # noqa: F401
+from test_kernels_at_scale_gpu import (HEAD_DIM, MODELS, _rows_with_spread, _tile_sums,  # noqa: F401
                                        fp64_reference, gen, randn, sm_count, units)
 from test_master_grad_gpu import _acc
 
@@ -43,12 +43,12 @@ TILE_M, TILE_N = 128, 256      # GEMM output tile
 # to bf16).  Measured on an H100 80GB HBM3 (700 W power limit) over every weight-gradient shape below with random operands:
 # c_need <= 8.9e-7 at K = 4096 and <= 1.07e-6 at K = 8192.  c is ~4x the worst.
 GEMM_C32 = 4.5e-6
-# The same allowance for the engine's own gradients (section 4).  Measured there (Qwen2-1.5B width, K = 8192 tokens): c_need
-# 8.5e-5 for the lm_head dW and 7.4e-5 for the tied embedding's head term.  In those GEMMs a vocabulary column of dlogits
-# holds one term of -1/T at the label and thousands of softmax terms ~1e5 times smaller: the accumulator carries the large
-# term and every later k-step adds values that lie below its last bits.  The error then grows linearly in K, at about one
-# accumulator ulp per k-step, instead of as a random walk, which is what a truncating (not rounding) tensor-core adder
-# gives.  c is ~4x the worst.
+# The same allowance for the engine's own gradients (test_engine_call_by_call_gpu.py).  Measured there (Qwen2-1.5B width,
+# K = 8192 tokens): c_need 8.5e-5 for the lm_head dW and 7.4e-5 for the tied embedding's head term.  In those GEMMs a
+# vocabulary column of dlogits holds one term of -1/T at the label and thousands of softmax terms ~1e5 times smaller: the
+# accumulator carries the large term and every later k-step adds values that lie below its last bits.  The error then grows
+# linearly in K, at about one accumulator ulp per k-step, instead of as a random walk, which is what a truncating (not
+# rounding) tensor-core adder gives.  c is ~4x the worst.
 ENGINE_GEMM_C32 = 3.5e-4
 # Relative Frobenius error of one 128 x 256 output tile.  Measured on the same H100: <= 4.5e-6 at K = 4096, <= 9.3e-6 at
 # K = 8192 with random operands, <= 1.8e-5 on the engine's gradients; one bf16 rounding gives ~1.7e-3.  ~4x the worst.
@@ -700,112 +700,3 @@ def test_adamw_past_2_31():
         print(f"[adamw past 2^31 {dtype} n={n} decay_end={decay_end}] worst err/bound {r}")
         assert max(r.values()) <= 1.0, r
         del G
-
-
-# ----------------------------------------------------------------------------------------------------------
-# 4. The engine at Qwen2-1.5B width, call by call
-# ----------------------------------------------------------------------------------------------------------
-class _CallChecker:
-    """Wraps ops.gemm (fp32 outputs), ops.rmsnorm_bwd, ops.colsum and ops.embedding_bwd.  Every call is checked on the spot
-    against fp64 of the operands it was given plus what its gradient view must already hold: nothing on micro-batch 0 (the
-    gradient buffer starts as NaN), the previous contents on micro-batch 1.  The embedding scatter always adds: onto zero
-    (untied) or onto the head's GEMM term (tied)."""
-
-    KINDS = ("gemm", "rmsnorm_bwd", "colsum", "embedding_bwd")
-
-    def __init__(self, o, monkeypatch):
-        self.orig = {k: getattr(o, k) for k in self.KINDS}
-        self.mb = 0
-        self.count = dict.fromkeys(self.KINDS, 0)
-        self.worst = dict.fromkeys(self.KINDS, 0.0)
-        self.sms = sm_count()
-        for k in self.KINDS:
-            monkeypatch.setattr(o, k, getattr(self, k))
-
-    def _done(self, kind, st):
-        self.count[kind] += 1
-        self.worst[kind] = max(self.worst[kind], st["ratio"])
-        assert st["bf16_rejected"], f"{kind}: the check cannot tell this fp32 gradient from its bf16 rounding"
-
-    def gemm(self, a, b, out=None, **kw):
-        if out is None or out.dtype != F32:
-            return self.orig["gemm"](a, b, out=out, **kw)
-        assert kw.get("trans_a") and not kw.get("trans_b"), "a weight gradient is X^T dY"
-        old = out.clone() if self.mb else None
-        self.orig["gemm"](a, b, out=out, **kw)
-        self._done("gemm", assert_gemm_f32_close(out, a.t(), b, c_old=old, c=ENGINE_GEMM_C32,
-                                                 what=f"dW {tuple(out.shape)} mb {self.mb}"))
-        return out
-
-    def rmsnorm_bwd(self, dy, x, w, rstd, dw, dres=None, accumulate_dw=True, dx=None):
-        assert dw.dtype == F32, "norm weight gradient is not fp32"
-        old = dw.clone() if self.mb else None
-        dx = self.orig["rmsnorm_bwd"](dy, x, w, rstd, dw, dres=dres, accumulate_dw=accumulate_dw, dx=dx)
-        h = x.shape[-1]
-        rows = x.numel() // h
-        rs = rstd.double()[:, None]
-        xh = x.reshape(rows, h).double() * rs
-        dyd = dy.reshape(rows, h).double()
-        terms = dyd * xh.float().to(BF16).double()
-        st = assert_colsum_close(dw, terms, old, parts=min(rows, 2 * self.sms), what=f"norm dw mb {self.mb}")
-        del terms
-        gg = dyd * w.double()
-        dx_ref = rs * (gg - xh * (gg * xh).mean(-1, keepdim=True))
-        if dres is not None:
-            dx_ref += dres.reshape(rows, h).double()
-        assert_rows_close(dx.reshape(rows, h), dx_ref, ROW_TOL, what=f"norm dx mb {self.mb}")
-        self._done("rmsnorm_bwd", st)
-        return dx
-
-    def colsum(self, a, out, accumulate=True):
-        assert out.dtype == F32, "bias gradient is not fp32"
-        old = out.clone() if self.mb else None
-        self.orig["colsum"](a, out, accumulate=accumulate)
-        self._done("colsum", assert_colsum_close(out, a, old, parts=min(a.shape[0], 64), what=f"bias grad mb {self.mb}"))
-        return out
-
-    def embedding_bwd(self, ids, dout, dtable):
-        assert dtable.dtype == F32, "embedding gradient is not fp32"
-        old = dtable.clone()
-        self.orig["embedding_bwd"](ids, dout, dtable)
-        self._done("embedding_bwd", assert_scatter_close(dtable, old, ids.reshape(-1), dout.reshape(-1, dtable.shape[1]),
-                                                         what=f"embedding grad mb {self.mb}"))
-        return dtable
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("tied", [False, True], ids=["untied", "tied"])
-def test_engine_fp32_grads_call_by_call(tied, monkeypatch, fp64_reference):
-    """Two decoder layers at Qwen2-1.5B width (h 1536, I 8960, 12/2 heads, q/k/v bias, V 151 936), B = 4, S = 2048, fp32
-    gradients; two micro-batches, the first fresh and the second accumulated.  Catches wiring faults at the real shapes: a
-    bf16 view passed to an fp32 op, a wrong accumulate flag, the tied head's GEMM term overwritten by the token scatter."""
-    import paddlenlp_b200.transformers as T
-    from paddlenlp_b200.transformers.decoder_engine import DecoderEngine
-
-    o = ops()
-    B, S, V, L = 4, 2048, 151936, 2
-    cfg = T.Qwen2Config(vocab_size=V, hidden_size=1536, intermediate_size=8960, num_hidden_layers=L, num_attention_heads=12,
-                        num_key_value_heads=2, max_position_embeddings=S, rope_theta=1e6, rms_norm_eps=1e-6,
-                        tie_word_embeddings=tied)
-    eng = DecoderEngine(cfg, device=DEV)
-    eng.init_weights(7)
-    for i in range(L):
-        eng.p[f"l{i}.qkv_b"].normal_(0, 0.02)
-    eng.params_changed()
-    eng.set_master_grad(True)
-    eng.flat_grads.fill_(NAN)                              # a view that is accumulated into instead of written shows up
-    eng.clear_grad()
-    chk = _CallChecker(o, monkeypatch)
-    gcpu = torch.Generator().manual_seed(21)
-    for mb in range(2):
-        tok = torch.randint(0, V, (B, S + 1), generator=gcpu)
-        ids, lab = tok[:, :-1].to(DEV), tok[:, 1:].to(DEV)
-        chk.mb = mb
-        eng.forward_loss(ids, lab)
-        eng.backward()
-    monkeypatch.undo()
-    print(f"[engine qwen2-1.5b width L={L} {'tied' if tied else 'untied'}] checked calls {chk.count}, worst err/bound "
-          f"{chk.worst}")
-    assert chk.count == dict(gemm=2 * (4 * L + 1), rmsnorm_bwd=2 * (2 * L + 1), colsum=2 * L, embedding_bwd=2)
-    for name, v in eng.g.items():
-        assert bool(torch.isfinite(v).all()), f"gradient {name} not fully written"
