@@ -404,9 +404,11 @@ class Trainer:
         if a.amp_master_grad:
             # trainer.py:1921-1960: fp32 main_grad for every parameter, before the optimizer and the data-parallel wrapper
             getattr(self.model, "_layers", self.model).set_master_grad(True)
-        self.create_optimizer_and_scheduler(max_steps)
+        # wrap first: the wrapper broadcasts rank 0's parameters, and AdamW copies its fp32 master weights from the
+        # parameters it finds, so every rank starts from rank 0's weights even when the ranks initialised differently
         model = self._wrap_model(self.model)
         self.model_wrapped = model
+        self.create_optimizer_and_scheduler(max_steps)
         engine = self._engine()
         world = a.world_size
         self.optimizer.grad_scale = 1.0 / world
